@@ -3,7 +3,7 @@
 
 Headline (configs[1]): `fast_aggregate_verify tuples/s`, mainnet preset, T = 4096 attestation tuples x K = 512 public
 keys per tuple, strict mode (every key decompressed + validated in every call, as
-/root/reference/ethereum-consensus/src/crypto/bls.rs:119-123 does), on 1..N B200 (one process per GPU; tuples shard
+the reference's crypto/bls.rs:119-123 does), on 1..N H100 (one process per GPU; tuples shard
 with no data-path collective; the per-shard verdict vectors are exchanged with one NCCL all_gather).
 Secondary (configs[2]), same JSON line under "ssz": `hash_tree_root(BeaconState) ms`, deneb mainnet, 2**20 validators.
 
@@ -11,6 +11,9 @@ One step = one pass of the hot path over one batch.  `value` = device time (CUDA
 stream, inputs already in HBM); `e2e` = the same batch through the public C-ABI call with pinned HOST buffers,
 H2D + kernels + D2H of the verdicts inside the timed region.  `--impl reference` times the CPU restatement
 (oracle/, plain C; blst/ssz_rs themselves cannot be built offline — DESIGN.md) on the host cores.
+`--dump-outputs DIR` writes what the last timed step returned (DIR/<name>.npy, float64) for output-for-output
+comparison of two builds; the inputs are seeded, so equal arguments give equal inputs.
+Writes nothing into the tree: build() has already compiled the library and the CPU oracles.
 """
 from __future__ import annotations
 
@@ -19,7 +22,6 @@ import ctypes as C
 import hashlib
 import json
 import os
-import subprocess
 import sys
 import threading
 import time
@@ -29,25 +31,27 @@ import numpy as np
 
 ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
+sys.dont_write_bytecode = True   # the tree may be read-only: no __pycache__ for the modules imported below
 
 R_ORDER = 0x73eda753299d7d483339d80809a1d80553bda402fffe5bfeffffffff00000001
 SEED = 0xB200
 # a point of E'(Fp2) outside G2 (iso3(sswu(5+7u)) compressed; produced by oracle/bls_oracle.py, see tests/golden)
 SIG_NOT_IN_GROUP = None  # filled from tests/golden/bls_cases.json
-# integer-arithmetic SASS instructions per 64-byte pair hash (2 compressions): 2 033 LOP3/SHF/IADD3 + 246 adds / moves the
-# compiler places on the FMA pipe (IMAD.IADD, PRMT, ...) — counted by tools/count_sha_sass.py from cuobjdump of the shipped
-# k_validator_roots (8 pair hashes of straight-line code per thread; 2 340 instructions in all); the denominator
+# integer-arithmetic SASS instructions per 64-byte pair hash (2 compressions): 2 051 LOP3/SHF/IADD3 + 264 adds / moves the
+# compiler places on the FMA pipe (IMAD.IADD, PRMT, ...) — counted by tools/count_sha_sass.py from cuobjdump of the sm_90a
+# k_validator_roots (8 pair hashes of straight-line code per thread); the denominator
 # b200_measure_int_peak(2) is the same kind of mix, which the compiler also spreads over both pipes (DESIGN.md §4)
-SASS_OPS_PER_PAIR_HASH = 2279
+SASS_OPS_PER_PAIR_HASH = 2315
 ORACLE_BUILD = "gcc -O3"   # set by load_oracles()
+HBM_PEAK_GBS = 3350.0       # denominator of the HBM rooflines (not a reached figure)
+HBM_PEAK_SOURCE = "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------ helpers
 def load_oracles():
-    import fcntl
-    with open(ROOT / "oracle" / ".build.lock", "w") as lk:  # ranks of one node must not rebuild the .so concurrently
-        fcntl.flock(lk, fcntl.LOCK_EX)
-        subprocess.run(["make", "-s", "-C", str(ROOT / "oracle")], check=True)
+    for name in ("liboracle_bls.so", "liboracle_ssz.so"):
+        if not (ROOT / "oracle" / name).exists():
+            raise SystemExit(f"oracle/{name} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` first")
     # the timed CPU arm gets the mulx / adx build when this host's CPU has both features (same results, ~20 % faster products)
     global ORACLE_BUILD
     try:
@@ -177,6 +181,8 @@ def main():
     ap.add_argument("--skip-rlc", action="store_true", help="skip the RLC whole-batch check")
     ap.add_argument("--skip-block", action="store_true", help="skip the configs[3] block signature set")
     ap.add_argument("--strong-tuples", type=int, default=2048)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     # Libraries (NCCL's version banner, make, ...) may write to fd 1; the contract is ONE JSON line on stdout from rank 0.
     real_stdout = os.dup(1)
@@ -184,6 +190,11 @@ def main():
 
     def emit(obj):
         os.write(real_stdout, (json.dumps(obj) + "\n").encode())
+
+    def dump(name, values):
+        if args.dump_outputs and int(os.environ.get("RANK", "0")) == 0:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), np.asarray(values, dtype=np.float64))
 
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
@@ -296,6 +307,7 @@ def main():
     launches = lib.b200_launch_count() - launches0
     collectives = lib.b200_collective_count() - coll0
     assert codes.tolist() == w["expect"].tolist()
+    dump("fast_aggregate_verify_codes", codes)   # the T verdict codes of this rank's shard, last timed step
 
     ms_dev = max_over_ranks(sum(dev_ms) / len(dev_ms))
     ms_e2e = max_over_ranks(1e3 * sum(wall) / len(wall))
@@ -330,7 +342,7 @@ def main():
             sc = parallel.sharded_verify_batch(spk, soff, smsg, ssig)
         assert sc.tolist() == ws["expect"].tolist(), "sharded verdicts differ from the constructed expectation"
         s_wall, s_dev = [], []
-        for _ in range(max(3, args.steps)):
+        for _ in range(args.steps):
             flush_l2()
             barrier()
             t0 = time.perf_counter()
@@ -431,7 +443,6 @@ def main():
         assert sset.first_failure(got) is None
 
     line = dict(base)
-    peaks = {}
     if rank == 0:
         # ---- CPU baseline: bounded sample of the same workload on the host cores (all threads) + parity on that sample
         sample = min(T, 8 * host_threads)
@@ -459,29 +470,19 @@ def main():
         mads_per_key = (fp_mul_per_key - fp_sqr_per_key) * 288 + fp_sqr_per_key * 222
 
         # integer-pipe denominators (DESIGN.md §4): IMAD.WIDE.U32 issues at one warp instruction per 4 cycles per SM
-        # sub-partition = 32 lane-MADs / clk / SM (B300_MICROARCH "rt_SMSP"); the microbenchmarks are the measured
-        # cross-check (kind 7: multiplicand from another chain; kind 0: round 1's self-dependent variant)
+        # sub-partition = 32 lane-MADs / clk / SM; the microbenchmarks are the measured
+        # cross-check (kind 7: multiplicand from another chain; kind 0: the self-dependent variant)
         clocks = clk.summary()
-        sm_mhz = clocks.get("sm_mhz") or 1965.0
+        sm_mhz = clocks.get("sm_mhz") or 1980.0   # H100 SXM maximum SM clock, when NVML is unavailable
         n_sm = torch.cuda.get_device_properties(local_rank).multi_processor_count
         imad_issue_peak = n_sm * 32 * sm_mhz * 1e6 / 1e9           # G wide-MAD/s at the clock seen during the run
         imad_meas = {"self_dependent": crypto.measure_int_peak(0), "cross_chain": crypto.measure_int_peak(7),
                      "cross_chain_immediate": crypto.measure_int_peak(8)}
         alu_peak = crypto.measure_int_peak(2)
-        try:
-            peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
-        except Exception:
-            pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
         dom = sum(dom_ms) / len(dom_ms)
         alg_bytes = T * (48 * K + 128)
         k1_mads = T * K * mads_per_key / (dom / 1e3) / 1e9   # algorithmic G MAD/s of the dominant kernel, per launch
         imad_peak = max(imad_issue_peak, max(imad_meas.values()))
-        ncu_traffic = None
-        try:   # dram__bytes_read.sum + dram__bytes_write.sum of this kernel from the committed ncu capture of THIS build
-            ncu_traffic = json.loads((ROOT / "profiles" / "r2_k1_traffic.json").read_text()).get(f"T{T}_K{K}")
-        except Exception:
-            pass
         line.update({
             "value": value, "ms_per_step": ms_dev, "gpu_launches": int(launches), "nccl_collectives_in_library": int(collectives),
             "e2e": {"value": e2e_value, "unit": "tuples/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4 * T},
@@ -496,11 +497,11 @@ def main():
                          "peak_measured_microbench": imad_meas, "peak_issue_rate_model": imad_issue_peak,
                          "fp_products_per_key": fp_mul_per_key, "of_which_squarings": fp_sqr_per_key,
                          "mads_per_product": 288, "mads_per_squaring": 222, "mads_per_key": mads_per_key,
-                         "traffic": ncu_traffic, "algorithmic_bytes": T * K * (48 + 104),
+                         "algorithmic_bytes": T * K * (48 + 104),
                          "kernel_ms": dom, "share_of_step": dom / ms_dev},
-            "hbm_roofline": {"bound": "hbm", "achieved": alg_bytes / (dom / 1e3) / 1e9, "peak": hbm_peak, "unit": "GB/s",
-                             "frac": alg_bytes / (dom / 1e3) / 1e9 / hbm_peak,
-                             "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "fallback",
+            "hbm_roofline": {"bound": "hbm", "achieved": alg_bytes / (dom / 1e3) / 1e9, "peak": HBM_PEAK_GBS, "unit": "GB/s",
+                             "frac": alg_bytes / (dom / 1e3) / 1e9 / HBM_PEAK_GBS,
+                             "peak_source": HBM_PEAK_SOURCE,
                              "note": "not the binding limit: 48 B in + 104 B out per key against ~440 k multiply-adds"},
             "int_roofline": {"unit": "G 32x32 multiply-adds/s", "fp_mul_per_tuple_cpu_oracle_count": fp_mul_per_tuple,
                              "squarings_per_tuple": fp_sqr_per_tuple,
@@ -645,6 +646,7 @@ def main():
             resident_sharded = {"ms_wall_max_over_ranks": sum(r[0] for r in rs) / len(rs), "ms_device_max_over_ranks": sum(r[1] for r in rs) / len(rs)}
         if args.validators == 1 << 20 and golden:
             assert root.hex() == golden, "hash_tree_root(BeaconState) differs from the hashlib golden root"
+        dump("beacon_state_root_bytes", np.frombuffer(root, dtype=np.uint8))   # the 32-byte root of the last timed step
         if rank == 0:
             out32 = C.create_string_buffer(32)
             t0 = time.perf_counter()
@@ -657,7 +659,6 @@ def main():
             n_hash = 10_117_927 if args.validators == 1 << 20 else None
             k_ms = (sum(ks) / len(ks)) if ks else None
             alu_peak_ssz = crypto.measure_int_peak(2)
-            hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
             # SHA-256 is ALU-pipe bound: SASS_OPS_PER_PAIR_HASH LOP3/SHF/IADD3-class instructions per 64-byte pair hash
             # (two compressions; counted from cuobjdump of k_merkle_stage, DESIGN.md §4) against the measured issue rate
             # of that instruction mix on this GPU (b200_measure_int_peak(2))
@@ -679,8 +680,8 @@ def main():
                                         "sha256_compressions_per_s": (2 * n_hash / (k_ms / 1e3)) if (single_gpu and k_ms and n_hash) else None,
                                         "peak_source": "measured on this GPU (b200_measure_int_peak(2))"},
                            "hbm_roofline": {"bound": "hbm", "achieved": (n_hash * 96 / (k_ms / 1e3) / 1e9) if (single_gpu and k_ms and n_hash) else None,
-                                            "peak": hbm_peak, "unit": "GB/s",
-                                            "frac": (n_hash * 96 / (k_ms / 1e3) / 1e9 / hbm_peak) if (single_gpu and k_ms and n_hash) else None,
+                                            "peak": HBM_PEAK_GBS, "unit": "GB/s", "peak_source": HBM_PEAK_SOURCE,
+                                            "frac": (n_hash * 96 / (k_ms / 1e3) / 1e9 / HBM_PEAK_GBS) if (single_gpu and k_ms and n_hash) else None,
                                             "note": "algorithmic bytes = 10 117 927 pair-hashes x 96 B (SURVEY.md §8d); not the binding limit"},
                            "cpu_baseline": {"ms_1_thread": cpu1, f"ms_{host_threads}_threads": cpun, "kind": "port",
                                             "note": "plain-C restatement with SHA-NI when the host has it (not ssz_rs)"}}

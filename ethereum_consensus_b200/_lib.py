@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI declared in include/b200_consensus.h.
 
 The CUDA library is the product: there is NO CPU fallback.  `load()` raises if the shared object is missing,
-`init()` raises if no B200 is visible.
+`init()` raises if no usable CUDA device is visible.
 """
 from __future__ import annotations
 
@@ -103,7 +103,7 @@ def load():
 
 
 def init(device: int | None = None):
-    """Bind this process to one GPU (one process per GPU).  Raises EngineError when no B200 is usable."""
+    """Bind this process to one GPU (one process per GPU).  Raises EngineError when no usable GPU is visible."""
     global _inited_device
     lib = load()
     if device is None:

@@ -4,9 +4,9 @@ execution order so the observable behaviour is the reference's:
 
 * the first failing check aborts with that check's error,
 * except deposits, whose invalid signatures are skipped silently
-  (/root/reference/ethereum-consensus/src/phase0/block_processing.rs:389-392),
+  (ethereum-consensus/src/phase0/block_processing.rs:389-392),
 * `is_valid_indexed_attestation`'s host-side checks (non-empty, sorted, unique, index in range) run before any
-  signature work and fail first (/root/reference/ethereum-consensus/src/phase0/helpers.rs:94-131).
+  signature work and fail first (ethereum-consensus/src/phase0/helpers.rs:94-131).
 
 Deposits are NOT deferred with the rest (ADVICE round 1): `apply_deposit` returns before `add_validator_to_registry` when
 the signature check fails (phase0/block_processing.rs:375-401), so the verdict decides a state mutation that later

@@ -1,4 +1,4 @@
-"""Builds the CUDA C-ABI library in-tree: ethereum_consensus_b200/libb200_consensus.so (sm_100a only)."""
+"""Builds the CUDA C-ABI library in-tree: ethereum_consensus_b200/libb200_consensus.so (sm_90a only)."""
 from __future__ import annotations
 
 import os
@@ -12,14 +12,13 @@ CSRC = PKG / "csrc"
 LIB = PKG / "libb200_consensus.so"
 OBJ = PKG / "build"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper)
+FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 # Per-TU ptxas optimisation level.  The three BLS translation units whose kernels are chains of inline-PTX Montgomery
 # products are assembled at -O1: at the default level ptxas interleaves more carry chains than it has predicate
-# registers and spills the carries into a GPR bitmask (bls_g1.cu: 13.3 k LOP3 + 1.8 k P2R + 1.8 k ISETP of 51 k
-# instructions); at -O1 the same IMAD.WIDE remain, four chains stay interleaved and the spill code is gone.
-# Measured on B200 (profiles/r2_ab_variants.txt, T=4096, K=512): per-key kernel 161.9 -> 136.0 ms (bls_g1.cu),
-# signature/message kernels 10.5 -> 7.5 ms (bls_g2.cu), Miller + final-exponentiation VM 15.96 -> 15.2 ms (bls_vm.cu).
+# registers and spills the carries into a GPR bitmask (LOP3 / P2R / ISETP around every product); at -O1 the same
+# IMAD.WIDE remain, four chains stay interleaved and the spill code is gone.
 # `B200_PTXAS_OPT=bls_g1.cu:3` restores the default level for a TU.  NVVM still runs at -O3.
 DEFAULT_PTXAS_OPT = {"bls_g1.cu": 1, "bls_g2.cu": 1, "bls_vm.cu": 1}
 
@@ -34,8 +33,8 @@ def _stale(target: Path, deps) -> bool:
 def build(force: bool = False, verbose: bool = False, defines=(), suffix: str = "", ptxas_opt=None) -> Path:
     """`defines`/`suffix`: alternate tuning build, e.g. build(defines=["B200_FP_SQR_VIA_MUL"], suffix="_sqrmul").
     `ptxas_opt`: {"bls_g1.cu": 1, ...} compiles those translation units with `-Xptxas -O<n>` (A/B knob: at -O1 ptxas
-    stops interleaving more carry chains than it has predicate registers — 34 k instead of 51 k instructions in the
-    per-key kernel, same IMAD.WIDE count; see DESIGN.md §8).  Use a `suffix` so the default objects are not reused."""
+    stops interleaving more carry chains than it has predicate registers — fewer instructions in the per-key kernel,
+    same IMAD.WIDE count; see DESIGN.md §8).  Use a `suffix` so the default objects are not reused."""
     global LIB, OBJ
     env_opt = {kv.split(":")[0]: int(kv.split(":")[1]) for kv in os.environ.get("B200_PTXAS_OPT", "").split(",") if kv}
     ptxas_opt = {**DEFAULT_PTXAS_OPT, **env_opt, **dict(ptxas_opt or {})}
@@ -76,7 +75,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), suffix: str = 
                 print(msg, file=sys.stderr)
     objs = [OBJ / (s.stem + ".o") for s in srcs]
     if force or jobs or _stale(LIB, objs):
-        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-o", str(LIB), *map(str, objs), *ARCH,
                "-Xcompiler", "-fPIC", "-cudart", "static"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

@@ -1,6 +1,6 @@
 """Host-side mirror of `ethereum_consensus::crypto` (BLS), backed by the CUDA library — no CPU fallback.
 
-Same names, argument meaning and error behaviour as /root/reference/ethereum-consensus/src/crypto/bls.rs:
+Same names, argument meaning and error behaviour as ethereum-consensus/src/crypto/bls.rs:
 `verify_signature` (:64-77), `aggregate` (:79-93), `aggregate_verify` (:95-112), `fast_aggregate_verify` (:114-132),
 `eth_aggregate_public_keys` (:135-148), `eth_fast_aggregate_verify` (:150-160), `hash` (:12-20), the byte newtypes
 `PublicKey` (:227-239) / `Signature` (:287-290) with their length checks (:257-266, :318-327) and

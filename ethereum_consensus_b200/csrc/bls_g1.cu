@@ -1,22 +1,20 @@
 // G1 side of the BLS pipeline: per-public-key validation (the dominant cost of the reference's
-// fast_aggregate_verify, /root/reference/ethereum-consensus/src/crypto/bls.rs:119-123 -> :283) and the per-tuple
+// fast_aggregate_verify, ethereum-consensus/src/crypto/bls.rs:119-123 -> :283) and the per-tuple
 // aggregation blst performs in `AggregatePublicKey::aggregate`.
 //
 // k_g1_validate : one thread per key, Fp limbs in registers; 48 B in, 100 B out.  Integer-pipe bound.
 // k_g1_aggregate: one warp per tuple; lanes stride over the tuple's keys with mixed additions, then a
 //                 5-round shared-memory tree of Jacobian additions; lane 0 normalises to affine.
-// Squarings (~75 % of this kernel's products) use the dedicated PTX square (222 wide MADs instead of 288).  Measured
-// on B200 at ptxas -O1 (profiles/r2_ab_variants.txt, 2^21 keys): 132.1 -> 128.2 ms with 256-thread CTAs at 224
-// registers; it LOSES with the 168-register cap (136.0 -> 143.2 ms: the square's wider live range spills) and lost at
-// ptxas' default level in round 1 (predicate spills).  -DB200_G1_SQR_VIA_MUL restores squares-by-product.
+// Squarings (~75 % of this kernel's products) use the dedicated PTX square (222 wide MADs instead of 288).  It pays
+// with 256-thread CTAs at 224 registers; with the 168-register cap the square's wider live range spills, and at ptxas'
+// default level it loses to predicate spills.  -DB200_G1_SQR_VIA_MUL restores squares-by-product.
 #if defined(B200_G1_SQR_VIA_MUL)
 #define B200_FP_SQR_VIA_MUL 1
 #endif
 // Products as by-value function CALLS (operands and result in registers, 0-byte frames) instead of ~70 inlined copies:
 // the inlined kernel is 0.5 MB of straight-line code, far beyond the instruction caches, and only pays at 8 warps per SM
-// where the warps stay in step.  With calls the kernel body is 170 KB and 12 warps per SM win.  Measured on B200
-// (profiles/r2_ab_variants.txt, 2^21 keys, lazily reduced arithmetic): inline 8 warps 118.6 ms, inline 12 warps 125.6,
-// calls 8 warps 124.7, **calls 12 warps 111.8**.  -DB200_G1_INLINE_MUL restores the inlined products.
+// where the warps stay in step.  With calls the kernel body is about a third of that and 12 warps per SM
+// win.  -DB200_G1_INLINE_MUL restores the inlined products.
 #if !defined(B200_G1_INLINE_MUL)
 #define B200_FP_MUL_CALL 1
 #endif
@@ -45,9 +43,8 @@ __device__ __forceinline__ void g1_validate_body(const uint8_t* __restrict__ key
 }
 // Default (variant 7): 384 threads capped at 168 registers = 12 warps per SM (with call-based products, see the top of
 // this file).  Variant 0: 256-thread CTAs at 224 registers (8 warps per SM, no spills).  Variant 6: 512 threads at 128
-// registers = 16 warps per SM.  Measured on B200, 2^21 keys: at ptxas' default level 164.5 vs 161.9 ms (round 1,
-// variant 7 was the default); at -O1 the spill-free variant wins, 132.1 vs 136.0 ms, and 128.2 vs 143.2 ms with the
-// dedicated square (profiles/r2_ab_variants.txt).  (__maxnreg__ cannot be combined with __launch_bounds__.)
+// registers = 16 warps per SM.  The register budgets follow from the SM's 64 K-entry register file;
+// B200_G1_VARIANT selects a variant at run time for A/B runs.  (__maxnreg__ cannot be combined with __launch_bounds__.)
 __global__ void __maxnreg__(224) k_g1_validate_main(const uint8_t* __restrict__ keys, uint32_t n, G1Aff* __restrict__ out,
                                                     int32_t* __restrict__ codes) {
     g1_validate_body(keys, n, out, codes);

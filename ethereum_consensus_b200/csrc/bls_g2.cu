@@ -1,13 +1,12 @@
 // G2 side of the BLS pipeline: signature decompression + subgroup check (blst `Signature::from_bytes` and the
-// `sig_groupcheck = true` of /root/reference/ethereum-consensus/src/crypto/bls.rs:71,106,126) and hash_to_G2 of
+// `sig_groupcheck = true` of ethereum-consensus/src/crypto/bls.rs:71,106,126) and hash_to_G2 of
 // the signing roots.  One thread per signature / message; these kernels see only T (thousands) of items, so
 // they run concurrently with the wide G1 kernels on a second stream.
 #define B200_FP_MUL_CALL 1
 // Fp2 products are INLINED into the curve routines here and the kernels may use 255 registers: these kernels run one or two
 // warps per SM, so the only thing that matters is the length of one thread's dependent chain — and at T = 4096 the 3-5 KB
-// stack frames of the earlier build (Fp2 products as calls, 128 registers) overflowed L1.  Measured (profiles/r2_ab_variants.txt,
-// calls 22 / 23): the step's wait for these kernels in registry mode 7.95 -> 4.97 ms at T = 4096 (either change alone: 7.7 / 6.4),
-// registry step 10.15 -> 9.90 ms at T = 1024; strict step unchanged (116.7 ms: they hide under the per-key kernel).
+// stack frames of the earlier build (Fp2 products as calls, 128 registers) overflowed L1.  In strict mode they hide under the
+// per-key kernel either way; in registry mode the step waits for them.
 // -DB200_G2_FP2_CALLS / -DB200_G2_MAXREG=128 restore the earlier build.
 #if defined(B200_G2_FP2_CALLS)
 #define B200_FP2_NOINLINE 1
@@ -23,8 +22,7 @@ namespace {
 
 // One warp per CTA: with only T items there is at most a warp or two per SM, so these kernels are latency-bound and
 // spread as 32-thread CTAs over every SM (128-thread CTAs when they run under a big per-key kernel, capi_bls.cu).
-// Round 1 (Fp2 products as calls): 128-register cap 14.4 ms, uncapped 24.4 ms for both kernels at T = 4096 — with calls, more
-// registers in the caller meant more saves / restores around every product.  Round 2 inlines the Fp2 products and lifts the cap
+// With Fp2 products as calls, more registers in the caller meant more saves / restores around every product.  Round 2 inlines the Fp2 products and lifts the cap
 // (see the top of this file).
 constexpr int kSmallCta = 32;
 #if !defined(B200_G2_MAXREG)

@@ -1,6 +1,6 @@
 // Pairing side of the BLS pipeline: one Miller loop per (G1, G2) pair and, per tuple, the Gt product + final
 // exponentiation + comparison with one — the check blst performs inside `fast_aggregate_verify` /
-// `aggregate_verify` (/root/reference/ethereum-consensus/src/crypto/bls.rs:106,126), plus the code merge that
+// `aggregate_verify` (ethereum-consensus/src/crypto/bls.rs:106,126), plus the code merge that
 // reproduces the wrapper's precedence: first bad public key -> signature decoding error -> verification.
 #define B200_FP_MUL_CALL 1
 #define B200_FP2_NOINLINE 1

@@ -1,7 +1,7 @@
 // Lane-parallel pairing kernels: a TEAM of 8 or 16 lanes per (G1, G2) pair / per tuple replays the statically
 // scheduled Fp2 programs of tools/gen_pairing_vm.py (Miller loop, final exponentiation) on a shared-memory register
 // file.  Replaces the one-thread-per-pair kernels of bls_pairing.cu on the batch path: those expose only 2T threads
-// (a ~40 ms latency floor at T = 4096); here 16x more lanes work on the same tuples, products stay inlined PTX.
+// (a latency floor of tens of ms at T = 4096); here 16x more lanes work on the same tuples, products stay inlined PTX.
 // -DB200_VM_MUL_CALL: field products as by-value function calls (fp.cuh) instead of ~15 inlined copies per kernel
 // (141 KB of straight-line code per VM kernel -> instruction-fetch stalls; see DESIGN.md §4)
 #if defined(B200_VM_MUL_CALL)
@@ -151,7 +151,7 @@ static Fp2* g_d_consts = nullptr;
 static uint32_t g_team16_max = 2048;
 // threads per CTA of the VM kernels (32 | 64 | 128): teams never synchronise across warps, so this only sets how finely the
 // shared-memory register files pack an SM and how the last wave spreads (B200_VM_CTA)
-static int g_vm_cta = 32;   // measured, T = 4096: registry step 23.70 (128) / 23.82 (64) / 23.20 ms (32); T = 2048: 18.40 / 18.40 / 17.56
+static int g_vm_cta = 32;   // the registry step was fastest with 32-thread CTAs at T = 2048 and 4096
 void set_vm_team16_max(uint32_t n) { g_team16_max = n; }
 void set_vm_cta(int threads) { if (threads == 32 || threads == 64 || threads == 128) g_vm_cta = threads; }
 

@@ -1,6 +1,6 @@
 // extern "C" entry points — the BLS half of include/b200_consensus.h — and the host orchestration of the batch
 // pipeline.  Every function below is a drop-in for one body in
-// /root/reference/ethereum-consensus/src/crypto/bls.rs (line ranges in the header); all curve arithmetic runs in
+// ethereum-consensus/src/crypto/bls.rs (line ranges in the header); all curve arithmetic runs in
 // the kernels of bls_g1.cu / bls_g2.cu / bls_pairing.cu.  The host only stages bytes and index arrays.
 //
 // Flow for T tuples with NK public keys in total (strict mode):
@@ -27,10 +27,9 @@ struct BlsState {
     // Chunked strict batches (OFF by default): the per-key kernel goes out in `chunks` key ranges on the engine stream, and
     // each range's aggregate -> Miller loops -> final exponentiation chain runs on `sd` UNDER the next range's per-key
     // kernel (B200_BLS_CHUNKS, 1 = one range; B200_BLS_CHUNK_MIN_TUPLES; B200_BLS_CHUNK_K1_CTA = 128 | 384).
-    // Measured on B200, T = 4096 x K = 512 (profiles/r2_ab_variants.txt, call 15): one range 130.2 ms; 2 ranges 137.3;
-    // 4 ranges 144.4 (138.8 with 384-thread K1 CTAs); 8 ranges 158.1.  The pairing chain does not fit under the per-key
+    // At T = 4096 x K = 512 every extra range made the step slower.  The pairing chain does not fit under the per-key
     // kernel: its CTAs need the registers / shared memory of a retiring per-key CTA, both kernels then run at reduced
-    // occupancy, and the per-key kernel loses more (114 -> 129 ms) than the 14 ms chain it hides.
+    // occupancy, and the per-key kernel loses more than the chain it hides.
     static constexpr uint32_t kMaxChunks = 16;
     cudaStream_t sd = nullptr, se = nullptr;   // se: odd key ranges, so that range c+1's CTAs fill range c's draining tail
     cudaEvent_t ev_ck[kMaxChunks] = {nullptr}, ev_join = nullptr;
@@ -40,7 +39,6 @@ struct BlsState {
     bool key_split = true;   // B200_BLS_KEY_SPLIT / b200_tune("bls_key_split")
     // CTA size of the first (4-wave) per-key launch of a split batch, the one the signature / message kernels run under: as three
     // 128-thread CTAs per SM a side kernel's CTA displaces a third of an SM's per-key work instead of all of it
-    // (T = 4096: 116.84 -> 116.43 ms per step, profiles/r2_ab_variants.txt call 32)
     int k1_first_cta = 128;
     cudaEvent_t ev_in = nullptr, ev_b = nullptr, ev_c = nullptr, ev_k0 = nullptr, ev_k1 = nullptr, ev_d0 = nullptr, ev_d1 = nullptr;
     DevBuf keys, key_aff, key_code, g1pts, g1pre, pk_code, flags, sigs, g2pts, sig_code, msgs, small, f, out, h2c_tmp, gath;
@@ -56,10 +54,9 @@ struct BlsState {
     bool trace = false;          // B200_BLS_TRACE=1: per-phase CUDA-event timings on stderr
     cudaEvent_t ev_t[8] = {nullptr};
     // B200_SMALL_ORDER: where the signature / message kernels go relative to the per-key kernel K1: 0 (default) under it on
-    // high-priority streams, 1 before it, 2 after it.  Round 1 measured 211 / 199 / 201 ms per step (T=4096, K=512) and ran
-    // them first; with round 2's K1 (call-based products: a fifth of the code, 12 warps/SM) the overlap wins:
-    // 130.9 / 136.2 ms at T=4096 with 128-thread CTAs, 18.2 / 25.2 ms at T=256 with 32-thread CTAs
-    // (profiles/r2_ab_variants.txt).  B200_SMALL_CTA overrides the CTA size (default: 32 up to 1 024 tuples, else 128).
+    // high-priority streams, 1 before it, 2 after it.  With the call-based
+    // per-key kernel (a fifth of the code, 12 warps/SM) the overlap beats running them first, with 128-thread CTAs at
+    // T = 4096 and 32-thread CTAs at T = 256.  B200_SMALL_CTA overrides the CTA size (default: 32 up to 1 024 tuples, else 128).
     int small_order = 0;
     int small_cta_override = 0;
     bool use_vm = true;  // lane-parallel pairing kernels (B200_PAIRING_VM=0 selects the one-thread-per-pair kernels)
@@ -266,6 +263,8 @@ static int32_t run_verify_impl(Engine& e, BlsState& s, PairMode mode, const uint
     // Big strict batches: the first kSplitWaves full waves of the per-key kernel start as soon as THEIR keys have arrived; the rest of
     // the key bytes (~90 MB at T = 4096) cross PCIe on stream E under that first launch, and the second launch follows them there
     // (two streams, so its CTAs fill the first launch's draining tail).  b200_tune("bls_key_split", 0) restores the single copy.
+    // The split point is a fixed key count (4 x 148 x 384), not whole waves of this GPU: on an H100 (132 SMs) sizing it and the
+    // thresholds below from the SM count made the T = 4096 step ~1 % slower.
     constexpr uint32_t kSplitWaves = 4, kSplitKeys = kSplitWaves * 148u * 384u;
     const uint32_t k_split = (s.key_split && have_k1 && !registry && n_chunks == 1 && s.small_order == 0 && n_keys >= 4u * kSplitKeys)
                                  ? kSplitKeys : n_keys;

@@ -1,8 +1,8 @@
 // Fp: the BLS12-381 base field, 381-bit, 12 x 32-bit limbs kept in registers, Montgomery form (R = 2^384).
 //
 // This is the arithmetic blst implements in x86-64 assembly for the reference
-// (/root/reference/ethereum-consensus/src/crypto/bls.rs:4 `use blst::{min_pk as bls_impl, ..}`), re-designed for
-// the B200 integer pipe: a Montgomery product is 2 x 12 x 12 32x32->64 multiply-adds (IMAD.WIDE on the fma
+// (ethereum-consensus/src/crypto/bls.rs:4 `use blst::{min_pk as bls_impl, ..}`), re-designed for
+// the GPU integer pipe: a Montgomery product is 2 x 12 x 12 32x32->64 multiply-adds (IMAD.WIDE on the fma
 // pipe) plus carry propagation on the ALU pipe.  No tensor cores: this is modular integer arithmetic.
 //
 // The same source compiles for the host (`B200_HD` = inline) so that every layer above Fp (towers, curves,
@@ -356,8 +356,8 @@ static const uint32_t h_exp_p_minus_1_div_2[12] = B200_EXP_P_MINUS_1_DIV_2;
 //
 // Where the table (8 x 48 B per thread) lives:
 //  * default: thread-local memory.  Its L1 residency depends on how the driver has laid out the context's local-memory
-//    pool, and that layout changes once ANY other CUDA module has launched a kernel in the process (measured: the
-//    per-key kernel went 167 -> 197 ms, profiles/r1_tuning.md "foreign module effect").
+//    pool, and that layout changes once ANY other CUDA module has launched a kernel in the process (the per-key
+//    kernel then slows down by a sixth).
 //  * B200_POW_TAB_SMEM (defined by a TU before including this header): dynamic shared memory, word-interleaved
 //    [(entry*12 + limb) * blockDim.x + threadIdx.x] so every access is bank-conflict-free.  Every kernel of that TU that
 //    reaches fp_pow must be launched with fp_pow_smem_bytes(threads) of dynamic shared memory.
@@ -429,7 +429,7 @@ B200_HD void fp_inv_fermat(Fp& r, const Fp& a) { fp_pow(r, a, B200_EXP_TABLE(exp
 
 // Inverse by Kaliski's "almost Montgomery inverse": 381..762 rounds of 384-bit shifts, adds and selects (no products),
 // then two products to fix the power of two.  a^(p-2) is 461 DEPENDENT products — for one thread (hash_to_G2's
-// normalisation) or one lane of a pairing-VM team (the Fp12 inversion of the final exponentiation: 0.8 of its 3.0 ms
+// normalisation) or one lane of a pairing-VM team (the Fp12 inversion of the final exponentiation: over a quarter of its
 // latency floor) that chain is pure latency; this loop is ~70 k short-latency ALU instructions with 12-way limb parallelism.
 // Branch-free inside the loop (a conditional swap keeps "the side to halve" in slot 1), so the lanes of a warp stay together.
 // Invariants (Kaliski 1995), x = the input integer: x*r = -u*2^k, x*s = v*2^k (mod p); u, v end at (1, 0) or (0, 1).

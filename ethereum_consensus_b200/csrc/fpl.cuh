@@ -1,6 +1,6 @@
 // FpL: "lazily reduced" base-field elements for the per-key kernel (bls_g1.cu) — any representative in [0, 2p).
 //
-// Why: ncu on the per-key kernel (profiles/r2b_k_g1_validate_main_O1_sqr_ncu.txt) shows the FMA-heavy pipe 65 % busy with
+// Why: a profile of the per-key kernel shows the FMA-heavy pipe only two-thirds busy with
 // `wait` as the top stall; the SASS explains it: every IMAD.WIDE carries a 4-cycle issue stall, so ONE warp streaming
 // wide MADs already saturates its scheduler's share of the pipe, and the pipe idles exactly while warps run the
 // ALU-only glue between products — the conditional subtraction after every Montgomery product and the add/sub/select

@@ -1,6 +1,6 @@
 // G1 / G2 of BLS12-381: ZCash (de)compression with blst's error taxonomy, subgroup membership, psi, cofactor
 // clearing.  Semantics restated from the reference wrapper (the checks blst runs for
-// /root/reference/ethereum-consensus/src/crypto/bls.rs:279-285 `key_validate` and :330-336 `from_bytes`):
+// ethereum-consensus/src/crypto/bls.rs:279-285 `key_validate` and :330-336 `from_bytes`):
 //   BAD_ENCODING(1): compression bit clear, infinity flag with payload, coordinate >= p
 //   POINT_NOT_ON_CURVE(2), POINT_NOT_IN_GROUP(3), PK_IS_INFINITY(6)
 #pragma once

@@ -1,5 +1,5 @@
 // hash_to_G2 for the ciphersuite BLS_SIG_BLS12381G2_XMD:SHA-256_SSWU_RO_POP_ (the DST at
-// /root/reference/ethereum-consensus/src/crypto/bls.rs:22): RFC 9380 hash_to_curve =
+// ethereum-consensus/src/crypto/bls.rs:22): RFC 9380 hash_to_curve =
 // expand_message_xmd(SHA-256) -> 2 x Fp2 -> simplified SWU on the 3-isogenous curve E'' -> 3-isogeny to E' ->
 // add -> clear cofactor.  blst computes the same function for every `verify`/`sign` of the reference.
 #pragma once

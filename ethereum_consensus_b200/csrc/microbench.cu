@@ -1,10 +1,10 @@
-// Integer-pipe peak microbenchmarks: the roofline denominators for the two hot paths, MEASURED on the box the bench
-// runs on (MEASURED_PEAKS.json only carries HBM / bf16 figures).  kind 0: IMAD.WIDE.U32 (32x32+64, the Montgomery
+// Integer-pipe peak microbenchmarks: the roofline denominators for the two hot paths, MEASURED on the GPU the bench
+// runs on.  kind 0: IMAD.WIDE.U32 (32x32+64, the Montgomery
 // multiply-add), kind 1: IMAD.U32 lo, kind 2: LOP3/SHF/IADD3 mix (the SHA-256 round ops), all dependency-limited
 // only by 8 independent chains per thread with the SMs fully occupied.
 // kind 7 / 8 (round 2): IMAD.WIDE.U32 whose multiplicand is the low word of ANOTHER chain's accumulator, multiplier in a
-// register (7) or an immediate (8), instead of the addend's own low word — kind 0 reads its 64-bit accumulator pair as BOTH a source and the addend, which the round-1
-// review showed saturates below the pipe's real issue rate (ncu sm__pipe_fmaheavy at 67 % while kind 0 said "peak").
+// register (7) or an immediate (8), instead of the addend's own low word — kind 0 reads its 64-bit accumulator pair as BOTH a source and the addend, which a profile
+// showed saturating below the pipe's real issue rate (the FMA-heavy pipe two-thirds busy while kind 0 said "peak").
 #include <cuda_runtime.h>
 
 #include "engine.h"

@@ -1,7 +1,7 @@
 // Optimal-ate pairing check for BLS12-381: Miller loop over |z| with Jacobian line functions on the M-twist and
 // the final exponentiation (easy part + Hayashida-Hayasaka-Teruya hard part, exponent 3(p^4-p^2+1)/r).
 // This is what blst runs under `Signature::{verify, fast_aggregate_verify, aggregate_verify}` for
-// /root/reference/ethereum-consensus/src/crypto/bls.rs:64-132.
+// ethereum-consensus/src/crypto/bls.rs:64-132.
 //
 // Line through T (Jacobian X,Y,Z on E') evaluated at P = (xP, yP) in G1, scaled by factors in Fp2 (killed by the
 // final exponentiation), in the basis 1, v, v*w of Fp12:

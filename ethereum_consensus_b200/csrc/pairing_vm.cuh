@@ -18,8 +18,7 @@ struct VmRfDense {
     B200_HD void store(uint32_t i, const Fp2& v) const { p[i] = v; }
 };
 // Slot stride in words.  28 (default) / 24: 16-byte aligned slots moved with 128-bit LDS/STS; 25 (round 1, -DB200_VM_SLOT_WORDS=25):
-// scalar LDS/STS, conflict-free for any slot pattern.  Measured on B200, T = 4096 (profiles/r2_ab_variants.txt): Miller 8.95 /
-// 8.41 / 8.05 ms and final exponentiation 6.32 / 6.35 / 6.21 ms for 25 / 24 / 28.
+// scalar LDS/STS, conflict-free for any slot pattern.  28 had the shortest Miller loop and final exponentiation of the three.
 // 16-byte aligned slots moved with 128-bit LDS/STS — 6 + 6 + 6 wide accesses per light op instead of 24 + 24 + 24.
 #if !defined(B200_VM_SLOT_WORDS)
 #define B200_VM_SLOT_WORDS 28
@@ -34,7 +33,7 @@ B200_HD constexpr uint32_t vm_team_words(uint32_t n_slots) { return n_slots * 24
 B200_HD constexpr uint32_t vm_slot_word(uint32_t i) { return i * uint32_t(kVmSlotWords); }
 B200_HD constexpr uint32_t vm_team_words(uint32_t n_slots) { return n_slots * uint32_t(kVmSlotWords); }
 #endif
-constexpr int kVmMaxSmemBytes = 227 * 1024;          // opt-in dynamic shared memory per CTA on sm_100
+constexpr int kVmMaxSmemBytes = 227 * 1024;          // opt-in dynamic shared memory per CTA on sm_90 (H100)
 constexpr uint32_t kVmBlobMagic = 0xB200564Du;       // run-time program blobs (vm_load_programs)
 struct VmRfStrided {
     uint32_t* p;

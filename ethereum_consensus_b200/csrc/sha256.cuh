@@ -1,8 +1,8 @@
-// SHA-256 device primitives for the SSZ Merkle kernels and hash_to_field (sm_100a).
+// SHA-256 device primitives for the SSZ Merkle kernels and hash_to_field (sm_90a).
 //
 // Replaces, on the device, what the reference gets from `sha2 0.10.8` through `ssz_rs` (merkleization,
-// /root/reference/ethereum-consensus/src/ssz/mod.rs:4-7) and `crypto::hash`
-// (/root/reference/ethereum-consensus/src/crypto/bls.rs:12-20).
+// ethereum-consensus/src/ssz/mod.rs:4-7) and `crypto::hash`
+// (ethereum-consensus/src/crypto/bls.rs:12-20).
 //
 // Node representation: a 32-byte Merkle node is kept in HBM as 8 big-endian-decoded 32-bit words ("word
 // form"), i.e. exactly the SHA-256 state words, so a parent = compress(compress(IV, left||right), PAD) needs

@@ -1,9 +1,9 @@
 // Committee shuffling on the device (SURVEY.md §8f-3): the step immediately BEFORE the BLS hot path — every
 // `process_attestation` resolves its committee through `get_beacon_committee`
-// (/root/reference/ethereum-consensus/src/phase0/helpers.rs:775-806), which scans the registry for active validators
+// (ethereum-consensus/src/phase0/helpers.rs:775-806), which scans the registry for active validators
 // (:646-676) and runs the 90-round swap-or-not shuffle (:249-283 per index, :287-360 for a whole list).
 //
-// B200 formulation (not the reference's in-place swap walk, which is inherently sequential):
+// Device formulation (not the reference's in-place swap walk, which is inherently sequential):
 //   k_shuffle_sources : every SHA-256 the shuffle can need is independent of the data: for each round r the pivot
 //                       hash(seed || r) and one "source" block hash(seed || r || le32(b)) per 256 positions —
 //                       rounds x (ceil(n/256) + 1) single-block hashes, one thread each (ALU-pipe bound).

@@ -1,12 +1,12 @@
-// SSZ hash_tree_root kernels for sm_100a.
+// SSZ hash_tree_root kernels for sm_90a.
 //
 // One `k_merkle_stage` launch processes one step of *every* big field of the container at once (a stage is a
 // list of jobs; blocks find their job through `block_begin`), so a full deneb BeaconState root is
 // ~6 wide launches + one single-CTA finisher for the small containers, the virtual zero-hash padding chains
 // (List limits of 2^40 => 40 levels, only the populated part is ever hashed), the length mix-ins and the
 // 28-field top tree.  Replaces ssz_rs' `merkleize` / derived `hash_tree_root`
-// (/root/reference/ethereum-consensus/src/deneb/beacon_state.rs:10-64, called at
-// /root/reference/ethereum-consensus/src/deneb/spec/mod.rs:3215,3288).
+// (ethereum-consensus/src/deneb/beacon_state.rs:10-64, called at
+// ethereum-consensus/src/deneb/spec/mod.rs:3215,3288).
 //
 // Work decomposition: every thread owns a complete small subtree (8 leaves -> 1 node = 7 hashes, or one
 // 121-byte Validator -> 8 hashes) and runs it entirely in registers: no idle lanes on the upper levels, no

@@ -398,7 +398,7 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
                 const PJob& pj = validator_jobs_[0];
                 const uint64_t n = pj.n_in;
                 // up to 16 slices, none smaller than 32 768 records (a multi-GPU shard is 1/world of the list: slices
-                // that cannot fill the 148 SMs would cost more in launches than the overlap buys)
+                // that cannot fill the SMs would cost more in launches than the overlap buys)
                 const uint64_t n_slices = std::min<uint64_t>(16, std::max<uint64_t>(1, n / 32768));
                 const uint64_t per = ((n + n_slices - 1) / n_slices + kStageThreads - 1) / kStageThreads * kStageThreads;  // whole CTAs per slice
                 int k = 0;
@@ -458,8 +458,8 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
         }
     }
     if (trace) cudaEventRecord(tev[1], s);
-    // (Measured and dropped, round 2 call 16: running the non-Validator stage chains on the copy stream UNDER the Validator
-    // kernel made the resident full re-hash slower, 1.60 -> 1.74 ms — the chains' CTAs take SM slots from the kernel that
+    // (Measured and dropped: running the non-Validator stage chains on the copy stream UNDER the Validator
+    // kernel made the resident full re-hash slower — the chains' CTAs take SM slots from the kernel that
     // is the critical path, and the join adds two event waits.)
     if (!validators_launched)
         for (auto& pj : validator_jobs_) {
@@ -526,7 +526,7 @@ struct Preset {
     uint64_t slots_per_historical_root, historical_roots_limit, eth1_data_votes_bound, validator_registry_limit,
         epochs_per_historical_vector, epochs_per_slashings_vector, sync_committee_size;
 };
-// /root/reference/ethereum-consensus/src/phase0/presets/{mainnet.rs:5-36,82-83, minimal.rs:20-25},
+// ethereum-consensus/src/phase0/presets/{mainnet.rs:5-36,82-83, minimal.rs:20-25},
 // altair/presets/{mainnet,minimal}.rs:19
 const Preset kPresets[2] = {
     {8192, 1ull << 24, 2048, 1ull << 40, 65536, 8192, 512},

@@ -133,7 +133,7 @@ private:
 
 int depth_for(uint64_t n);
 
-// deneb BeaconState (/root/reference/ethereum-consensus/src/deneb/beacon_state.rs:26-63): byte offsets of the
+// deneb BeaconState (ethereum-consensus/src/deneb/beacon_state.rs:26-63): byte offsets of the
 // fixed-size fields and of the nine variable-size fields inside the SSZ serialization.
 struct StateOffsets {
     size_t fixed = 0;

@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's committee-shuffling helpers, computed on the device (SURVEY.md §8f-3).
 
-`compute_shuffled_indices`      — /root/reference/ethereum-consensus/src/phase0/helpers.rs:287-360
+`compute_shuffled_indices`      — ethereum-consensus/src/phase0/helpers.rs:287-360
 `compute_shuffled_index`        — :249-283 (one position of the same permutation)
 `get_active_validator_indices`  — :646-676
 `compute_committee`             — :459-483   (slice of the shuffled list)

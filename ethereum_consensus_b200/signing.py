@@ -1,10 +1,10 @@
 """Mirror of the reference's signing helpers, hashing on the device.
 
-`compute_signing_root` / `verify_signed_data`  — /root/reference/ethereum-consensus/src/signing.rs:14-41
-`compute_domain` / `compute_fork_data_root`    — /root/reference/ethereum-consensus/src/phase0/helpers.rs:506-529
-`get_domain` (previous / current fork version)  — /root/reference/ethereum-consensus/src/phase0/helpers.rs:190-222
-`compute_epoch_at_slot`                        — /root/reference/ethereum-consensus/src/phase0/helpers.rs (slot / SLOTS_PER_EPOCH)
-`DomainType`                                   — /root/reference/ethereum-consensus/src/domains.rs:1-30
+`compute_signing_root` / `verify_signed_data`  — ethereum-consensus/src/signing.rs:14-41
+`compute_domain` / `compute_fork_data_root`    — ethereum-consensus/src/phase0/helpers.rs:506-529
+`get_domain` (previous / current fork version)  — ethereum-consensus/src/phase0/helpers.rs:190-222
+`compute_epoch_at_slot`                        — ethereum-consensus/src/phase0/helpers.rs (slot / SLOTS_PER_EPOCH)
+`DomainType`                                   — ethereum-consensus/src/domains.rs:1-30
 """
 from __future__ import annotations
 

@@ -1,10 +1,10 @@
 """Host-side mirror of the reference's SSZ merkleization surface, backed by the CUDA library.
 
 Mirrors what `ethereum_consensus::ssz::prelude` re-exports from ssz_rs
-(/root/reference/ethereum-consensus/src/ssz/mod.rs:4-7): `merkleize`, `mix_in_length`,
+(ethereum-consensus/src/ssz/mod.rs:4-7): `merkleize`, `mix_in_length`,
 `is_valid_merkle_branch`, and `hash_tree_root` for the containers on the hot path
-(`deneb::BeaconState`, /root/reference/ethereum-consensus/src/deneb/beacon_state.rs:13-64;
-`List<Validator, N>`, /root/reference/ethereum-consensus/src/phase0/validator.rs:10-26).
+(`deneb::BeaconState`, ethereum-consensus/src/deneb/beacon_state.rs:13-64;
+`List<Validator, N>`, ethereum-consensus/src/phase0/validator.rs:10-26).
 Every hash is computed on the GPU; there is no CPU fallback.
 """
 from __future__ import annotations

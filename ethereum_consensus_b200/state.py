@@ -1,7 +1,7 @@
 """Synthetic deneb `BeaconState` instances (numpy) and their SSZ serialization.
 
-Field order and sizes follow /root/reference/ethereum-consensus/src/deneb/beacon_state.rs:26-63 and the presets
-(/root/reference/ethereum-consensus/src/phase0/presets/mainnet.rs:5-36,82-83, altair/presets/mainnet.rs:19).
+Field order and sizes follow ethereum-consensus/src/deneb/beacon_state.rs:26-63 and the presets
+(ethereum-consensus/src/phase0/presets/mainnet.rs:5-36,82-83, altair/presets/mainnet.rs:19).
 Used by bench.py (config 3 of BASELINE.json: 2**20 validators) and by the parity tests.  Data is synthetic:
 pubkeys are pseudo-random 48-byte strings unless `pubkeys=` is given (hashing does not interpret them).
 """
@@ -22,7 +22,7 @@ PRESETS: Dict[str, Dict[str, int]] = {
                     EPOCHS_PER_SLASHINGS_VECTOR=64, SYNC_COMMITTEE_SIZE=32),
 }
 
-# SSZ `Validator` (121 bytes) — /root/reference/ethereum-consensus/src/phase0/validator.rs:10-26
+# SSZ `Validator` (121 bytes) — ethereum-consensus/src/phase0/validator.rs:10-26
 VALIDATOR_DTYPE = np.dtype([
     ("public_key", "V48"), ("withdrawal_credentials", "V32"), ("effective_balance", "<u8"), ("slashed", "u1"),
     ("activation_eligibility_epoch", "<u8"), ("activation_epoch", "<u8"), ("exit_epoch", "<u8"),

@@ -1,17 +1,17 @@
 /*
- * b200_consensus.h — C ABI of the B200-native batch-crypto engine.
+ * b200_consensus.h — C ABI of the H100-native batch-crypto engine.
  *
  * This is the drop-in boundary for ralexstokes/ethereum_consensus' hot path (SURVEY.md §8b):
  *   - BLS:  the seven free functions re-exported at
- *           /root/reference/ethereum-consensus/src/crypto/mod.rs:4-8 (bodies in crypto/bls.rs:64-160), whose only
+ *           ethereum-consensus/src/crypto/mod.rs:4-8 (bodies in crypto/bls.rs:64-160), whose only
  *           backend today is `use blst::{min_pk as bls_impl, BLST_ERROR}` (crypto/bls.rs:4);
  *   - SSZ:  `HashTreeRoot::hash_tree_root` / `merkleize` / `is_valid_merkle_branch` from
- *           `pub use ssz_rs::prelude::*` (/root/reference/ethereum-consensus/src/ssz/mod.rs:6).
+ *           `pub use ssz_rs::prelude::*` (ethereum-consensus/src/ssz/mod.rs:6).
  * Plain pointers and sizes only; the caller owns every buffer; calls are synchronous and thread-safe (one
  * process-global context per device).  INTEGRATION.md shows the Rust `extern "C"` block that binds these.
  *
  * Return codes: 0..7 are blst's BLST_ERROR values (order pinned by
- * /root/reference/ethereum-consensus/src/crypto/bls.rs:48-62); >= 0x100 are engine failures (CUDA, bad
+ * ethereum-consensus/src/crypto/bls.rs:48-62); >= 0x100 are engine failures (CUDA, bad
  * arguments, malformed SSZ) and are NEVER conflated with a signature verdict.  There is no CPU fallback: if
  * the device or the CUDA library is unavailable every entry point returns B200_ERR_NO_DEVICE / B200_ERR_CUDA.
  */
@@ -65,7 +65,7 @@ B200_API uint64_t b200_launch_count(void);
 B200_API float b200_last_kernel_ms(void);
 
 /* ---- SSZ / SHA-256 Merkle (replaces ssz_rs merkleize / hash_tree_root; sha2 one-shot) -------------- */
-/* crypto::hash — /root/reference/ethereum-consensus/src/crypto/bls.rs:12-20 (computed on the device). */
+/* crypto::hash — ethereum-consensus/src/crypto/bls.rs:12-20 (computed on the device). */
 B200_API int32_t b200_sha256(const uint8_t* data, size_t len, uint8_t out[32]);
 
 /* merkleize(chunks, limit): `n_chunks` 32-byte chunks, virtually zero-padded to `limit` chunks
@@ -74,7 +74,7 @@ B200_API int32_t b200_merkleize(const uint8_t* chunks, size_t n_chunks, uint64_t
 /* mix_in_length(root, len) */
 B200_API int32_t b200_mix_in_length(const uint8_t root[32], uint64_t length, uint8_t out[32]);
 /* is_valid_merkle_branch(leaf, branch[depth], depth, index, root): *ok = 1/0.
- * Used at /root/reference/ethereum-consensus/src/phase0/block_processing.rs:428-437 and deneb/blob_sidecar.rs:58-63. */
+ * Used at ethereum-consensus/src/phase0/block_processing.rs:428-437 and deneb/blob_sidecar.rs:58-63. */
 B200_API int32_t b200_is_valid_merkle_branch(const uint8_t leaf[32], const uint8_t* branch, size_t depth, uint64_t index,
                                     const uint8_t root[32], int32_t* ok);
 
@@ -86,7 +86,7 @@ B200_API int32_t b200_htr_packed(const uint8_t* data, size_t nbytes, uint64_t li
                         uint8_t out[32]);
 
 /* hash_tree_root(deneb::BeaconState) from its SSZ serialization
- * (/root/reference/ethereum-consensus/src/deneb/beacon_state.rs:13-64; called at deneb/spec/mod.rs:3215,3288). */
+ * (ethereum-consensus/src/deneb/beacon_state.rs:13-64; called at deneb/spec/mod.rs:3215,3288). */
 B200_API int32_t b200_htr_beacon_state_deneb(const uint8_t* ssz, size_t len, int32_t preset, uint8_t out[32]);
 
 /* Device-resident state: upload once, re-hash many times (kernel-only cost; SURVEY.md §8f-2 groundwork). */
@@ -123,7 +123,7 @@ B200_API int32_t b200_htr_beacon_state_deneb_combine(const uint8_t* ssz, size_t 
                                             const uint8_t* all_roots /* world*5*32 */, uint8_t out[32]);
 
 /* ---- committee shuffling (SURVEY.md §8f-3): the step before the BLS hot path ---------------------------------- */
-/* compute_shuffled_indices — /root/reference/ethereum-consensus/src/phase0/helpers.rs:287-360 (whole list; equal to
+/* compute_shuffled_indices — ethereum-consensus/src/phase0/helpers.rs:287-360 (whole list; equal to
  * mapping every position through compute_shuffled_index, :249-283): out[i] = indices[shuffled_index(i, n, seed)].
  * `indices` == NULL means the identity list 0..n-1; `rounds` = SHUFFLE_ROUND_COUNT (90 on mainnet, 10 on minimal). */
 B200_API int32_t b200_compute_shuffled_indices(const uint64_t* indices, size_t n, const uint8_t seed[32], uint32_t rounds,

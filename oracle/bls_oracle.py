@@ -1,7 +1,7 @@
 """BLS12-381 signature oracle in pure Python big-ints (TEST INFRASTRUCTURE — never imported by the product path).
 
-The reference's BLS arithmetic lives in the un-vendored crate `blst = "0.3.11"` (/root/reference/Cargo.toml:21);
-what /root/reference holds is the byte-typed wrapper /root/reference/ethereum-consensus/src/crypto/bls.rs.  This
+The reference's BLS arithmetic lives in the un-vendored crate `blst = "0.3.11"` (Cargo.toml:21);
+what the reference checkout holds is the byte-typed wrapper ethereum-consensus/src/crypto/bls.rs.  This
 file restates, slowly and obviously:
 
 * the wrapper semantics — which checks run, in which order, what maps to Ok/Err:

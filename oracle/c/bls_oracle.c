@@ -3,11 +3,11 @@
  * only tests/, __graft_entry__.smoke() and bench.py (cpu_baseline / --impl reference, workload generation) may
  * load this.  The product path never does.
  *
- * What it restates: the byte-level behaviour of /root/reference/ethereum-consensus/src/crypto/bls.rs
+ * What it restates: the byte-level behaviour of ethereum-consensus/src/crypto/bls.rs
  *   verify_signature :64-77, aggregate :79-93, aggregate_verify :95-112, fast_aggregate_verify :114-132,
  *   eth_aggregate_public_keys :135-148, eth_fast_aggregate_verify :150-160, key_validate :279-285,
  *   Signature::from_bytes :330-336, SecretKey::{public_key,sign} :212-220,
- * whose arithmetic the reference takes from the un-vendored crate blst 0.3.11 (/root/reference/Cargo.toml:21).
+ * whose arithmetic the reference takes from the un-vendored crate blst 0.3.11 (Cargo.toml:21).
  * Algorithms are the published ones (IETF BLS signatures with the DST at crypto/bls.rs:22, RFC 9380
  * hash_to_curve, ZCash serialization, optimal-ate pairing).  Every derived constant (Frobenius coefficients, psi,
  * the G1 endomorphism) is computed at start-up from first principles; only the RFC 9380 isogeny coefficients

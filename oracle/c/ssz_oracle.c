@@ -3,11 +3,11 @@
  * bench.py's cpu_baseline / --impl reference legs may link or load this.  The product path never does.
  *
  * Restates, for the CPU, the merkleization the reference gets from the un-vendored `ssz_rs @ 84ef2b71`
- * (/root/reference/Cargo.toml:20; surface re-exported at /root/reference/ethereum-consensus/src/ssz/mod.rs:4-7)
- * and the one-shot SHA-256 of /root/reference/ethereum-consensus/src/crypto/bls.rs:12-20 (sha2 0.10.8, which
+ * (Cargo.toml:20; surface re-exported at ethereum-consensus/src/ssz/mod.rs:4-7)
+ * and the one-shot SHA-256 of ethereum-consensus/src/crypto/bls.rs:12-20 (sha2 0.10.8, which
  * dispatches to SHA-NI at run time — so does this file).  Container shapes:
- *   deneb::BeaconState   /root/reference/ethereum-consensus/src/deneb/beacon_state.rs:13-64
- *   Validator            /root/reference/ethereum-consensus/src/phase0/validator.rs:10-26
+ *   deneb::BeaconState   ethereum-consensus/src/deneb/beacon_state.rs:13-64
+ *   Validator            ethereum-consensus/src/phase0/validator.rs:10-26
  * Validated against oracle/ssz_oracle.py (hashlib) and the reference KAT B-3 in tests/test_oracle_ssz.py.
  */
 #include <stdint.h>

@@ -1,8 +1,8 @@
 """CPU oracle for committee shuffling — TEST INFRASTRUCTURE ONLY (tests/, smoke, bench's cpu_baseline may import it).
 
 Two independent restatements of the reference's two formulations, pinned against each other:
-  * `compute_shuffled_index`   — the per-index swap-or-not map, /root/reference/ethereum-consensus/src/phase0/helpers.rs:249-283
-  * `compute_shuffled_indices` — the whole-list walk,            /root/reference/ethereum-consensus/src/phase0/helpers.rs:287-360
+  * `compute_shuffled_index`   — the per-index swap-or-not map, ethereum-consensus/src/phase0/helpers.rs:249-283
+  * `compute_shuffled_indices` — the whole-list walk,            ethereum-consensus/src/phase0/helpers.rs:287-360
     (the reference's own runner asserts both equal the spec vector `mapping`, spec-tests/runners/shuffling.rs:35-45)
 plus a numpy-vectorised form of the first for 2**20-size checks, and `get_active_validator_indices` (:646-676).
 Parity pin: the `consensus-spec-tests` shuffling vectors are absent offline, and the reference tree holds no shuffling

@@ -1,19 +1,19 @@
 """SSZ merkleization oracle (TEST INFRASTRUCTURE — never imported by the product path).
 
 CPU restatement, with `hashlib.sha256`, of the SSZ `hash_tree_root` / `merkleize` semantics that the
-reference obtains from the un-vendored crate `ssz_rs @ 84ef2b71` (`/root/reference/Cargo.toml:20`,
-re-exported at `/root/reference/ethereum-consensus/src/ssz/mod.rs:4-7`).  The algorithm restated is the
+reference obtains from the un-vendored crate `ssz_rs @ 84ef2b71` (`Cargo.toml:20`,
+re-exported at `ethereum-consensus/src/ssz/mod.rs:4-7`).  The algorithm restated is the
 consensus-specs `ssz/simple-serialize.md` merkleization; the container shapes follow the reference:
 
-* `deneb::BeaconState`           /root/reference/ethereum-consensus/src/deneb/beacon_state.rs:13-64
-* `Validator`                    /root/reference/ethereum-consensus/src/phase0/validator.rs:10-26
+* `deneb::BeaconState`           ethereum-consensus/src/deneb/beacon_state.rs:13-64
+* `Validator`                    ethereum-consensus/src/phase0/validator.rs:10-26
 * `Fork`, `Checkpoint`, `Eth1Data`, `BeaconBlockHeader`
-                                 /root/reference/ethereum-consensus/src/phase0/{beacon_state.rs:15-22,operations.rs:13-17,66-71,beacon_block.rs:83-91}
-* `SyncCommittee`                /root/reference/ethereum-consensus/src/altair/sync.rs:17-22
-* `ExecutionPayloadHeader`       /root/reference/ethereum-consensus/src/deneb/execution_payload.rs:47-76
-* `HistoricalSummary`            /root/reference/ethereum-consensus/src/phase0/beacon_state.rs:42-45
-* `SigningData`, `compute_signing_root`  /root/reference/ethereum-consensus/src/signing.rs:9-22
-* `is_valid_merkle_branch` use   /root/reference/ethereum-consensus/src/deneb/blob_sidecar.rs:47-64
+                                 ethereum-consensus/src/phase0/{beacon_state.rs:15-22,operations.rs:13-17,66-71,beacon_block.rs:83-91}
+* `SyncCommittee`                ethereum-consensus/src/altair/sync.rs:17-22
+* `ExecutionPayloadHeader`       ethereum-consensus/src/deneb/execution_payload.rs:47-76
+* `HistoricalSummary`            ethereum-consensus/src/phase0/beacon_state.rs:42-45
+* `SigningData`, `compute_signing_root`  ethereum-consensus/src/signing.rs:9-22
+* `is_valid_merkle_branch` use   ethereum-consensus/src/deneb/blob_sidecar.rs:47-64
 
 Pinned by the reference's own KAT B-3 (blob-sidecar inclusion proof, `deneb/blob_sidecar.rs:70-132`) in
 `tests/test_oracle_ssz.py`.  Full-state roots are not pinned by any in-tree reference test (the
@@ -30,7 +30,7 @@ ZERO_CHUNK = b"\x00" * 32
 
 
 def sha256(data: bytes) -> bytes:
-    """`crypto::hash` — /root/reference/ethereum-consensus/src/crypto/bls.rs:12-20."""
+    """`crypto::hash` — ethereum-consensus/src/crypto/bls.rs:12-20."""
     return hashlib.sha256(data).digest()
 
 
@@ -93,8 +93,8 @@ def mix_in_length(root: bytes, length: int) -> bytes:
 
 
 def is_valid_merkle_branch(leaf: bytes, branch: Sequence[bytes], depth: int, index: int, root: bytes) -> bool:
-    """ssz_rs `is_valid_merkle_branch` as used at /root/reference/ethereum-consensus/src/deneb/blob_sidecar.rs:58-63
-    and /root/reference/ethereum-consensus/src/phase0/block_processing.rs:428-437."""
+    """ssz_rs `is_valid_merkle_branch` as used at ethereum-consensus/src/deneb/blob_sidecar.rs:58-63
+    and ethereum-consensus/src/phase0/block_processing.rs:428-437."""
     value = leaf
     for i in range(depth):
         if (index >> i) & 1:
@@ -132,7 +132,7 @@ class Boolean(UInt):
 
 
 class ByteVector(SszType):
-    """`ByteVector<N>` — /root/reference/ethereum-consensus/src/ssz/byte_vector.rs:11-22."""
+    """`ByteVector<N>` — ethereum-consensus/src/ssz/byte_vector.rs:11-22."""
     def __init__(self, n: int): self.n = n
     def is_fixed(self): return True
     def fixed_size(self): return self.n
@@ -144,7 +144,7 @@ class ByteVector(SszType):
 
 
 class ByteList(SszType):
-    """`ByteList<N>` — /root/reference/ethereum-consensus/src/ssz/byte_list.rs:11-12."""
+    """`ByteList<N>` — ethereum-consensus/src/ssz/byte_list.rs:11-12."""
     def __init__(self, limit: int): self.limit = limit
     def is_fixed(self): return False
     def serialize(self, v): return bytes(v)
@@ -291,13 +291,13 @@ def execution_payload_header_type(bytes_per_logs_bloom: int = 256, max_extra_dat
 
 
 PRESETS = {
-    # /root/reference/ethereum-consensus/src/phase0/presets/mainnet.rs:5-36,82-83; altair/presets/mainnet.rs:19;
+    # ethereum-consensus/src/phase0/presets/mainnet.rs:5-36,82-83; altair/presets/mainnet.rs:19;
     # bellatrix/presets/mainnet.rs:23-24
     "mainnet": dict(SLOTS_PER_HISTORICAL_ROOT=8192, HISTORICAL_ROOTS_LIMIT=1 << 24, ETH1_DATA_VOTES_BOUND=2048,
                     VALIDATOR_REGISTRY_LIMIT=1 << 40, EPOCHS_PER_HISTORICAL_VECTOR=65536,
                     EPOCHS_PER_SLASHINGS_VECTOR=8192, SYNC_COMMITTEE_SIZE=512, BYTES_PER_LOGS_BLOOM=256,
                     MAX_EXTRA_DATA_BYTES=32),
-    # /root/reference/ethereum-consensus/src/phase0/presets/minimal.rs:20-25; altair/presets/minimal.rs:19
+    # ethereum-consensus/src/phase0/presets/minimal.rs:20-25; altair/presets/minimal.rs:19
     "minimal": dict(SLOTS_PER_HISTORICAL_ROOT=64, HISTORICAL_ROOTS_LIMIT=1 << 24, ETH1_DATA_VOTES_BOUND=32,
                     VALIDATOR_REGISTRY_LIMIT=1 << 40, EPOCHS_PER_HISTORICAL_VECTOR=64,
                     EPOCHS_PER_SLASHINGS_VECTOR=64, SYNC_COMMITTEE_SIZE=32, BYTES_PER_LOGS_BLOOM=256,
@@ -306,7 +306,7 @@ PRESETS = {
 
 
 def beacon_state_type(preset: str = "mainnet") -> Container:
-    """deneb `BeaconState` — field order = /root/reference/ethereum-consensus/src/deneb/beacon_state.rs:26-63."""
+    """deneb `BeaconState` — field order = ethereum-consensus/src/deneb/beacon_state.rs:26-63."""
     p = PRESETS[preset]
     return Container("BeaconState", [
         ("genesis_time", u64),
@@ -342,11 +342,11 @@ def beacon_state_type(preset: str = "mainnet") -> Container:
 
 
 def compute_signing_root(object_root: bytes, domain: bytes) -> bytes:
-    """`compute_signing_root` — /root/reference/ethereum-consensus/src/signing.rs:14-22."""
+    """`compute_signing_root` — ethereum-consensus/src/signing.rs:14-22."""
     return SigningData.htr({"object_root": object_root, "domain": domain})
 
 
 def compute_domain(domain_type: bytes, fork_version: bytes, genesis_validators_root: bytes) -> bytes:
-    """`compute_domain` — /root/reference/ethereum-consensus/src/phase0/helpers.rs:506-529."""
+    """`compute_domain` — ethereum-consensus/src/phase0/helpers.rs:506-529."""
     fork_data_root = ForkData.htr({"current_version": fork_version, "genesis_validators_root": genesis_validators_root})
     return domain_type + fork_data_root[:28]

@@ -3,7 +3,7 @@ ethereum_consensus_b200/csrc/*.cuh — the same source the kernels compile) agai
 tens of thousands of random and adversarial inputs.  SURVEY.md §8c asks for >= 10^4 such cases because the reference's
 own offline KATs only pin the accept side.
 
-    python tests/soak_parity.py [scale] > profiles/r1_soak_parity.txt        (scale 1.0 ~ a few minutes on 8 cores)
+    python tests/soak_parity.py [scale] > soak_parity.txt        (scale 1.0 ~ a few minutes on 8 cores)
 """
 import ctypes as C, hashlib, subprocess, sys, time
 from pathlib import Path

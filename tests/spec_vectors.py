@@ -1,6 +1,6 @@
 """Consumer for the reference's REAL parity vectors: the `consensus-spec-tests` tree its `spec-tests` crate walks
-(/root/reference/spec-tests/main.rs:20,56-112 — `tests/<config>/<fork>/<runner>/<handler>/<suite>/<case>/`), with the
-case semantics of /root/reference/spec-tests/runners/bls.rs:17-58 (per-handler `data.yaml`: `input`, `output`) and
+(spec-tests/main.rs:20,56-112 — `tests/<config>/<fork>/<runner>/<handler>/<suite>/<case>/`), with the
+case semantics of spec-tests/runners/bls.rs:17-58 (per-handler `data.yaml`: `input`, `output`) and
 runners/ssz_static.rs:13-36 (`roots.yaml` + `serialized.ssz_snappy`, raw snappy as test_utils.rs:30-37 decodes it).
 
 The vectors are downloaded by the reference's justfile and are absent offline; anyone who has the tarball points

@@ -13,12 +13,12 @@ ROOT = Path(__file__).resolve().parent.parent
 GOLDEN = json.loads((Path(__file__).parent / "golden" / "bls_cases.json").read_text())
 F1, F2 = bo.F1, bo.F2
 
-# KAT B-2: /root/reference/ethereum-consensus/src/crypto/bls.rs:530-544 (`test_can_sign`)
+# KAT B-2: ethereum-consensus/src/crypto/bls.rs:530-544 (`test_can_sign`)
 B2_SK = int("40094c5c6c378857eac09b8ec64c87182f58700c056a8b371ad0eb0a5b983d50", 16)
 B2_MSG = b"blst is such a blast"
 B2_SIG = bytes.fromhex("a01e49276730e4752eef31b0570c8707de501398dac70dd144438cd1bd05fb9b9bb3e1a9ceef0a68cc08904362cafa3f"
                        "1005e5b699a41847fff6f5552260468846de5bdbf94a9aedeb29bc6cdb2c1d34922d9e9af4c0593a69ae978a90b5aba6")
-# KAT B-1: /root/reference/ethereum-consensus/src/bin/ec/validator/keystores.rs:239-249 (EIP-2335)
+# KAT B-1: ethereum-consensus/src/bin/ec/validator/keystores.rs:239-249 (EIP-2335)
 B1_SK = int("000000000019d6689c085ae165831e934ff763ae46a2a6c172b3f1b60a8ce26f", 16)
 B1_PK = bytes.fromhex("9612d7a727c9d0a22e185a1c768478dfe919cada9266988cb32359c11f2b7b27f4ae4040902382ae2910c15e2b420d07")
 # KAT B-2b: decode-only points, crypto/bls.rs:381-390 and :453-461

@@ -13,7 +13,7 @@ from ethereum_consensus_b200 import state as S
 
 GOLDEN = json.loads((Path(__file__).parent / "golden" / "ssz_roots.json").read_text())
 
-# KAT B-3: /root/reference/ethereum-consensus/src/deneb/blob_sidecar.rs:70-132 (live sepolia blob sidecar)
+# KAT B-3: ethereum-consensus/src/deneb/blob_sidecar.rs:70-132 (live sepolia blob sidecar)
 B3_COMMITMENT = bytes.fromhex("8da04bbe26b2bbc6b042f4db18a36f1b4714123706065ed3946a3c3aeb681f98d3e67a3483b088612cb9b0c5322723a0")
 B3_BODY_ROOT = bytes.fromhex("940ebac04b768dab430d21b4b2d7ecd5d3f87e0486293a5612c16b9e8d4c078a")
 B3_BRANCH = [bytes.fromhex(x) for x in """

@@ -1,5 +1,5 @@
 """GPU parity for committee shuffling (SURVEY.md §8f-3) against the oracle's two formulations of
-/root/reference/ethereum-consensus/src/phase0/helpers.rs:249-360 and `get_active_validator_indices` (:646-676)."""
+ethereum-consensus/src/phase0/helpers.rs:249-360 and `get_active_validator_indices` (:646-676)."""
 import hashlib
 
 import numpy as np

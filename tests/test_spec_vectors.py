@@ -1,4 +1,4 @@
-"""Runner for the reference's conformance vectors (layout of /root/reference/spec-tests/runners/bls.rs:17-58 and
+"""Runner for the reference's conformance vectors (layout of spec-tests/runners/bls.rs:17-58 and
 ssz_static.rs:13-36).  With the `consensus-spec-tests` tarball present (CONSENSUS_SPEC_TESTS=<dir> or
 <repo>/consensus-spec-tests) every `bls/*` case runs against the CPU oracle (and, under -m gpu, against the CUDA path),
 and every deneb `ssz_static/BeaconState` case against both hash_tree_root implementations.  Offline (this container,

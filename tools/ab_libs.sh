@@ -3,8 +3,7 @@
 # run (T=4096, K=512, per-phase trace) and its GPU parity tests.  Build the variants beforehand (no GPU needed), e.g.
 #   python -m ethereum_consensus_b200.build --suffix=_o1 --ptxas-opt=bls_g1.cu:1,bls_vm.cu:1
 #   python -m ethereum_consensus_b200.build --suffix=_o1g1 --ptxas-opt=bls_g1.cu:1
-# then:  gpurun --timeout 900 -- 'bash tools/ab_libs.sh > gpurun_out/ab.txt 2>&1'   (remove the variants afterwards:
-# each adds ~23 MB to every push).
+# then, on the GPU machine:  bash tools/ab_libs.sh > ab.txt 2>&1
 for lib in ethereum_consensus_b200/libb200_consensus*.so; do
   echo "== $lib"
   B200_LIB=$PWD/$lib B200_BLS_TRACE=1 python bench.py --steps 3 --warmup 3 --skip-ssz 2> /tmp/ab.err \

@@ -1,5 +1,5 @@
 // Diagnostic only: tiny "foreign" CUDA module used by tools/tune_k1_diag3.py to find out which property of another
-// module loaded into the same context slows k_g1_validate_main (see profiles/r1_tuning.md, "foreign module effect").
+// module loaded into the same context slows k_g1_validate_main (DESIGN.md, "foreign module effect").
 #include <cassert>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Generates ethereum_consensus_b200/csrc/fp_mul_ptx.cuh: the tuned Montgomery product and square for sm_100a, each as
+"""Generates ethereum_consensus_b200/csrc/fp_mul_ptx.cuh: the tuned Montgomery product and square for sm_90a, each as
 ONE inline-PTX block (a carry chain must never be split across asm statements), plus a C emulation of exactly the
 same instruction lists (`fp_mul_emul_core`, `fp_sqr_emul_core`, host-testable) so the sequences are verified against
 big-ints on the CPU before the PTX ever runs on a GPU (tests/test_oracle_bls.py::test_fp_mul_ptx_emulation).

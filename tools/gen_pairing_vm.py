@@ -3,7 +3,7 @@ final exponentiation, list-scheduled into rounds of <= TEAM independent operatio
 kernels (csrc/pairing_vm.cuh).  One tuple is handled by a TEAM of lanes; every lane executes one Fp2 operation per
 round on a shared-memory register file, rounds are separated by __syncwarp().
 
-Why: with one thread per pair / per tuple the pairing kernels expose only T..2T threads (T = 4096) — a ~40 ms latency
+Why: with one thread per pair / per tuple the pairing kernels expose only T..2T threads (T = 4096) — a latency
 floor that no amount of per-thread tuning removes.  The Miller loop and the final exponentiation have no
 data-dependent control flow, so they can be *traced once* (symbolic Fp2 values below, mirroring pairing.cuh /
 fp12.cuh formula by formula) and replayed with 8-18 way parallelism.
@@ -570,8 +570,8 @@ def main():
         HEAVY_MIN = int(sys.argv[i + 1])
         del sys.argv[i:i + 2]
     team = int(sys.argv[1]) if len(sys.argv) > 1 else 8
-    # scheduling windows (Miller, final): measured trade-off between heavy rounds and register-file slots, see
-    # profiles/r1_tuning.md; defaults: team 16 -> (256, 48), team 8 -> (96, 96).  BOTH headers ship: teams of 8 lanes have the
+    # scheduling windows (Miller, final): trade-off between heavy rounds and register-file slots;
+    # defaults: team 16 -> (256, 48), team 8 -> (96, 96).  BOTH headers ship: teams of 8 lanes have the
     # higher throughput (big batches), teams of 16 the shorter critical path (batches too small to fill the machine):
     #   python tools/gen_pairing_vm.py 8 && python tools/gen_pairing_vm.py 16
     window = int(sys.argv[2]) if len(sys.argv) > 2 else (256 if team == 16 else 96)

@@ -1,5 +1,5 @@
 """Extracts the metrics the roofline discussion uses from an .ncu-rep (run here, no GPU needed):
-   python tools/ncu_summary.py gpurun_out/prof.ncu-rep > profiles/<name>.txt"""
+   python tools/ncu_summary.py prof.ncu-rep > summary.txt"""
 import csv
 import subprocess
 import sys
