@@ -43,6 +43,7 @@ _lib.register_protos({
     "b200_fast_aggregate_verify_batch_all_sharded": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int32)]),
     "b200_last_dominant_kernel_ms": (C.c_float, []),
     "b200_fp_selftest": (C.c_int32, [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]),
+    "b200_fp_eval": (C.c_int32, [C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_measure_int_peak": (C.c_int32, [C.c_int32, C.POINTER(C.c_double)]),
 })
 
@@ -270,6 +271,25 @@ def fp_selftest(n: int = 1 << 16, seed: int = 1) -> int:
     m = C.c_uint32(0)
     _lib.check(_lib.lib().b200_fp_selftest(n, seed, C.byref(m)), "fp_selftest")
     return int(m.value)
+
+
+# operations of fp_eval (bls_kernels.cuh FP_EVAL_* / FP2_EVAL_*)
+FP_EVAL_OPS = {"fp_mul": 0, "fp_sqr": 1, "fpl_mul": 2, "fpl_sqr": 3, "fp_add": 4, "fp_sub": 5, "fp_neg": 6, "fpl_add": 7,
+               "fpl_sub": 8, "fpl_neg": 9, "fp_add_raw": 10, "fp_sub_raw": 11, "fp_inv_kaliski": 12, "fp_inv_fermat": 13,
+               "fp_sqrt": 14, "fpl_pow_sqrt": 15, "fp_is_lex_largest": 16,
+               "fp2_mul": 32, "fp2_sqr": 33, "fp2_inv": 34, "fp2_sqrt": 35, "fp2_sgn0": 36}
+
+
+def fp_eval(op: str, a, b=None) -> np.ndarray:
+    """Self-test: one device field operation on raw limbs.  a, b: uint32[n, 24] (Fp in columns 0..11, Fp2 c0 | c1);
+    returns uint32[n, 25]: the result's limbs, then the flag word (carry, borrow, is-square, lex-largest or sgn0)."""
+    a = np.ascontiguousarray(a, dtype=np.uint32)
+    b = np.zeros_like(a) if b is None else np.ascontiguousarray(b, dtype=np.uint32)
+    if a.ndim != 2 or a.shape[1] != 24 or b.shape != a.shape:
+        raise ValueError("operands must be uint32[n, 24]")
+    out = np.zeros((max(a.shape[0], 1), 25), dtype=np.uint32)
+    _lib.check(_lib.lib().b200_fp_eval(FP_EVAL_OPS[op], a.shape[0], _lib.ptr(a), _lib.ptr(b), _lib.ptr(out)), f"fp_eval({op})")
+    return out[:a.shape[0]]
 
 
 def tune(knob: str, value: int) -> None:

@@ -208,6 +208,43 @@ __global__ void k_fp_selftest(uint32_t n, uint32_t seed, uint32_t* out_mismatch)
     if (bad) atomicAdd(out_mismatch, bad);
 }
 
+// Field self-test against big integers (b200_fp_eval): one operation per launch on raw operands, so that the host can
+// check the exact representative.  Compiled here so that it runs the per-key kernel's products (fp_mul_call /
+// fpl_mul_call), its shared-memory pow table and this unit's ptxas level.
+__global__ void k_fp_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
+                          uint32_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fp x, y, r = fp_zero();
+    for (int k = 0; k < 12; k++) { x.l[k] = a[size_t(i) * kFpEvalIn + k]; y.l[k] = b[size_t(i) * kFpEvalIn + k]; }
+    const FpL xl = fpl_from_fp(x), yl = fpl_from_fp(y);
+    FpL rl;
+    uint32_t flag = 0;
+    switch (op) {
+    case FP_EVAL_MUL: fp_mul(r, x, y); break;
+    case FP_EVAL_SQR: fp_sqr(r, x); break;
+    case FPL_EVAL_MUL: f_mul(rl, xl, yl); r = rl.v; break;
+    case FPL_EVAL_SQR: f_sqr(rl, xl); r = rl.v; break;
+    case FP_EVAL_ADD: fp_add(r, x, y); break;
+    case FP_EVAL_SUB: fp_sub(r, x, y); break;
+    case FP_EVAL_NEG: fp_neg(r, x); break;
+    case FPL_EVAL_ADD: f_add(rl, xl, yl); r = rl.v; break;
+    case FPL_EVAL_SUB: f_sub(rl, xl, yl); r = rl.v; break;
+    case FPL_EVAL_NEG: f_neg(rl, xl); r = rl.v; break;
+    case FP_EVAL_ADD_RAW: flag = fp_add_raw(r, x, y); break;
+    case FP_EVAL_SUB_RAW: flag = fp_sub_raw(r, x, y); break;
+    case FP_EVAL_INV_KALISKI: fp_inv_kaliski(r, x); break;
+    case FP_EVAL_INV_FERMAT: fp_inv_fermat(r, x); break;
+    case FP_EVAL_SQRT: flag = fp_sqrt(r, x) ? 1u : 0u; break;
+    case FPL_EVAL_POW_SQRT: fpl_pow(rl, xl, B200_EXP_TABLE(exp_sqrt)); r = rl.v; break;
+    case FP_EVAL_IS_LEX_LARGEST: flag = fp_is_lex_largest(x) ? 1u : 0u; break;
+    default: break;
+    }
+    uint32_t* o = out + size_t(i) * kFpEvalOut;
+    for (int k = 0; k < 12; k++) { o[k] = r.l[k]; o[12 + k] = 0; }
+    o[24] = flag;
+}
+
 }  // namespace
 
 // dynamic shared memory for fp_pow's table; opts the kernel in to > 48 KiB once
@@ -262,6 +299,10 @@ void launch_g1_compress(const G1Aff* p, uint8_t* out48, void* stream) {
 void launch_neg_g1(G1Aff* out, G1Pre* out_pre, void* stream) { k_neg_g1<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(out, out_pre); }
 void launch_fp_selftest(uint32_t n, uint32_t seed, uint32_t* out_mismatch, void* stream) {
     k_fp_selftest<<<(n + 127) / 128, 128, with_pow_tab(k_fp_selftest, 128), static_cast<cudaStream_t>(stream)>>>(n, seed, out_mismatch);
+}
+void launch_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream) {
+    if (!n) return;
+    k_fp_eval<<<(n + 127) / 128, 128, with_pow_tab(k_fp_eval, 128), static_cast<cudaStream_t>(stream)>>>(op, n, a, b, out);
 }
 
 }  // namespace b200

@@ -108,6 +108,31 @@ __global__ void __launch_bounds__(32) k_g2_sum_compress(const G2Aff* __restrict_
     }
 }
 
+// Fp2 self-test against big integers (b200_fp_eval): compiled here so that it runs this unit's inlined Fp2 products,
+// register cap and ptxas level
+__global__ void B200_G2_BOUNDS k_fp2_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
+                                          uint32_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fp2 x, y, r = fp2_zero();
+    for (int k = 0; k < 12; k++) {
+        x.c0.l[k] = a[size_t(i) * kFpEvalIn + k]; x.c1.l[k] = a[size_t(i) * kFpEvalIn + 12 + k];
+        y.c0.l[k] = b[size_t(i) * kFpEvalIn + k]; y.c1.l[k] = b[size_t(i) * kFpEvalIn + 12 + k];
+    }
+    uint32_t flag = 0;
+    switch (op) {
+    case FP2_EVAL_MUL: fp2_mul(r, x, y); break;
+    case FP2_EVAL_SQR: fp2_sqr(r, x); break;
+    case FP2_EVAL_INV: fp2_inv(r, x); break;
+    case FP2_EVAL_SQRT: flag = fp2_sqrt(r, x) ? 1u : 0u; if (!flag) r = fp2_zero(); break;
+    case FP2_EVAL_SGN0: flag = fp2_sgn0(x); break;
+    default: break;
+    }
+    uint32_t* o = out + size_t(i) * kFpEvalOut;
+    for (int k = 0; k < 12; k++) { o[k] = r.c0.l[k]; o[12 + k] = r.c1.l[k]; }
+    o[24] = flag;
+}
+
 }  // namespace
 
 constexpr size_t kPowTab = 0;  // thread-local table here (see above)
@@ -130,6 +155,10 @@ void launch_hash_to_g2(const uint8_t* msgs, const uint32_t* moff, uint32_t n, G2
 }
 void launch_g2_sum_compress(const G2Aff* sigs, const int32_t* sig_code, uint32_t n, uint8_t* out96, int32_t* out_code, void* stream) {
     k_g2_sum_compress<<<1, 32, kPowTab, static_cast<cudaStream_t>(stream)>>>(sigs, sig_code, n, out96, out_code);
+}
+void launch_fp2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream) {
+    if (!n) return;
+    k_fp2_eval<<<(n + kSmallCta - 1) / kSmallCta, kSmallCta, kPowTab, static_cast<cudaStream_t>(stream)>>>(op, n, a, b, out);
 }
 
 }  // namespace b200

@@ -70,5 +70,21 @@ void launch_g1_compress(const G1Aff* p, uint8_t* out48, void* stream);
 void launch_neg_g1(G1Aff* out, G1Pre* out_pre, void* stream);
 // on-device self-test of Fp arithmetic (portable vs tuned paths), returns mismatches in *out
 void launch_fp_selftest(uint32_t n, uint32_t seed, uint32_t* out_mismatch, void* stream);
+// on-device self-test: one field operation on n raw operand pairs, for comparison with big integers on the host.
+// Operand slots are kFpEvalIn words (Fp: words 0..11; Fp2: c0 in 0..11, c1 in 12..23), result slots kFpEvalOut words
+// (the same limbs, then one flag word: carry, borrow, "is a square", lex-largest or sgn0).  Limbs are little-endian 32-bit
+// words of the raw representative (Montgomery form where the operation works in it).
+enum : int32_t {
+    FP_EVAL_MUL = 0, FP_EVAL_SQR = 1, FPL_EVAL_MUL = 2, FPL_EVAL_SQR = 3,
+    FP_EVAL_ADD = 4, FP_EVAL_SUB = 5, FP_EVAL_NEG = 6, FPL_EVAL_ADD = 7, FPL_EVAL_SUB = 8, FPL_EVAL_NEG = 9,
+    FP_EVAL_ADD_RAW = 10, FP_EVAL_SUB_RAW = 11, FP_EVAL_INV_KALISKI = 12, FP_EVAL_INV_FERMAT = 13,
+    FP_EVAL_SQRT = 14, FPL_EVAL_POW_SQRT = 15, FP_EVAL_IS_LEX_LARGEST = 16,
+    FP_EVAL_N_OPS = 17,                                              // bls_g1.cu: the per-key kernel's build
+    FP2_EVAL_MUL = 32, FP2_EVAL_SQR = 33, FP2_EVAL_INV = 34, FP2_EVAL_SQRT = 35, FP2_EVAL_SGN0 = 36,
+    FP2_EVAL_END = 37                                                // bls_g2.cu: the signature / hash kernels' build
+};
+constexpr uint32_t kFpEvalIn = 24, kFpEvalOut = 25;
+void launch_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
+void launch_fp2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
 
 }  // namespace b200

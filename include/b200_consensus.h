@@ -256,6 +256,10 @@ B200_API int32_t b200_tune(const char* knob, int64_t value);
 B200_API int32_t b200_vm_load_programs(const uint32_t* blob, size_t n_words);
 /* On-device self-test of the field arithmetic over `n` pseudo-random triples; *mismatches must come back 0. */
 B200_API int32_t b200_fp_selftest(uint32_t n, uint32_t seed, uint32_t* mismatches);
+/* On-device self-test of single field operations, for comparison with big integers: `op` (bls_kernels.cuh, FP_EVAL_* /
+ * FP2_EVAL_*) is applied to `n` operand pairs.  a, b: n x 24 raw little-endian 32-bit limbs (Fp in the first 12, Fp2 as
+ * c0 then c1); out: n x 25 (the result's limbs, then a carry / borrow / square / sign flag).  Test use only. */
+B200_API int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
 
 #ifdef __cplusplus
 }
