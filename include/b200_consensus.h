@@ -206,10 +206,13 @@ B200_API int32_t b200_fast_aggregate_verify_batch(const uint8_t* pks_flat, const
 /* Optimistic WHOLE-BATCH check by random linear combination (north_star: "Miller loops fused across the batch, partial Gt
  * products reduced with warp shuffles"): *all_ok = 1 iff every tuple of the batch would return 0 above — decided with
  * T Miller loops and ONE final exponentiation instead of 2T and T:  prod_t e(r_t agg_t, H(msg_t)) * e(-g1, sum_t r_t sig_t) == 1
- * for 64-bit scalars r_t = SHA-256(seed || t).  Valid batches are always accepted; a batch with an invalid tuple is
- * accepted with probability <= 2^-64 over the seed (seed32 == NULL: the library draws one from the OS; tests pass a fixed
- * seed).  This is the normal-case path of process_block (every signature of a block is expected to verify); on
- * *all_ok == 0 the caller asks b200_fast_aggregate_verify_batch, which remains the only source of per-tuple codes. */
+ * for 64-bit scalars r_t = the first 8 bytes, little-endian, of SHA-256(seed || le64(t)) (forced non-zero).  Valid batches
+ * are always accepted; a batch with an invalid tuple is accepted with probability <= 2^-64 over the seed (seed32 == NULL:
+ * the library draws one from the OS; tests pass a fixed seed).  A caller-supplied seed must be unpredictable to whoever
+ * produced the signatures: anyone who knows the seed can build a batch in which every tuple is invalid and the defects
+ * cancel, and that batch is accepted.  This is the normal-case path of process_block (every signature of a block is
+ * expected to verify); on *all_ok == 0 the caller asks b200_fast_aggregate_verify_batch, which remains the only source of
+ * per-tuple codes. */
 B200_API int32_t b200_fast_aggregate_verify_batch_all(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs32,
                                                       const uint8_t* sigs, size_t n_tuples, const uint8_t* seed32, int32_t* all_ok);
 /* Registry mode: validate the (append-only, immutable-pubkey) validator registry once, keep the affine keys in
@@ -228,7 +231,10 @@ B200_API int32_t b200_fast_aggregate_verify_batch_mixed(const uint8_t* extra_pks
                                                         size_t n_tuples, int32_t* out_codes);
 /* RLC whole-batch check over registry indices, and over all ranks of the communicator: every rank passes the same batch
  * and the same (non-NULL) seed, verifies its block, and ONE ncclAllGather moves the per-rank Gt partial (576 B) and G2
- * partial (288 B); every rank then finishes the same final exponentiation and returns the same boolean. */
+ * partial (288 B); every rank then finishes the same final exponentiation and returns the same boolean.  Rank k scales
+ * its tuples with r_t of their global index t.  The sharded call requires the caller's seed, so the caller must draw it
+ * unpredictably (for instance from the OS after the signatures are fixed) and share it among the ranks: a seed known to
+ * whoever produced the signatures lets them build an all-invalid batch that is accepted. */
 B200_API int32_t b200_fast_aggregate_verify_batch_indexed_all(const uint32_t* indices, const uint32_t* offsets,
                                                               const uint8_t* msgs32, const uint8_t* sigs, size_t n_tuples,
                                                               const uint8_t* seed32, int32_t* all_ok);
