@@ -171,17 +171,29 @@ def _nbytes(buf) -> int:
     return len(buf)
 
 
+def _batch_size(off, msgs32, sigs, keys=None, indices=None, seed=None) -> int:
+    """T of a batch call.  The C side reads raw pointers: refuse T + 1 offsets whose buffers (48-byte `keys` or uint32
+    `indices`, 32-byte messages, 96-byte signatures) disagree with them, and a seed that is not 32 bytes."""
+    t = len(off) - 1
+    if t < 0:
+        raise ValueError("offsets must hold T + 1 entries")
+    n = int(off[-1])
+    if ((keys is not None and _nbytes(keys) != 48 * n) or (indices is not None and len(indices) != n)
+            or _nbytes(msgs32) != 32 * t or _nbytes(sigs) != 96 * t):
+        raise ValueError(f"buffer sizes do not match the offsets: {n} keys, msgs {_nbytes(msgs32)} B, sigs {_nbytes(sigs)} B "
+                         f"for {t} tuples")
+    if seed is not None and len(seed) != 32:
+        raise ValueError("seed must be 32 bytes")
+    return t
+
+
 def fast_aggregate_verify_batch(pks_flat, pk_offsets, msgs32, sigs) -> np.ndarray:
     """T tuples at once -> int32 code per tuple (0 Ok, 5 InvalidSignature, 1/2/3/6 BLST decode errors).
     pks_flat: (sum K) x 48 bytes; pk_offsets: uint32[T+1]; msgs32: T x 32; sigs: T x 96 (host buffers)."""
     off = np.ascontiguousarray(pk_offsets, dtype=np.uint32)
-    t = len(off) - 1
-    if t < 0 or (t >= 0 and int(off[0]) != 0):
-        raise ValueError("pk_offsets must hold T+1 entries starting at 0")
-    # the C side reads raw pointers: refuse buffers whose sizes disagree with the offsets
-    if _nbytes(pks_flat) != 48 * int(off[-1]) or _nbytes(msgs32) != 32 * t or _nbytes(sigs) != 96 * t:
-        raise ValueError(f"buffer sizes do not match the offsets: keys {_nbytes(pks_flat)} B for {int(off[-1])} keys, "
-                         f"msgs {_nbytes(msgs32)} B, sigs {_nbytes(sigs)} B for {t} tuples")
+    t = _batch_size(off, msgs32, sigs, keys=pks_flat)
+    if int(off[0]) != 0:
+        raise ValueError("pk_offsets must start at 0")
     out = np.empty(max(t, 1), dtype=np.int32)
     _lib.check(_lib.lib().b200_fast_aggregate_verify_batch(_lib.ptr(pks_flat), _lib.ptr(off), _lib.ptr(msgs32), _lib.ptr(sigs),
                                                            t, _lib.ptr(out)), "fast_aggregate_verify_batch")
@@ -194,11 +206,7 @@ def fast_aggregate_verify_batch_all(pks_flat, pk_offsets, msgs32, sigs, seed: by
     `fast_aggregate_verify_batch` for the per-tuple codes.  `sharded`: all ranks of the library's communicator share the
     batch (same arguments and seed on every rank); the Gt / G2 partials travel in one ncclAllGather."""
     off = np.ascontiguousarray(pk_offsets, dtype=np.uint32)
-    t = len(off) - 1
-    if t < 0 or _nbytes(pks_flat) != 48 * int(off[-1]) or _nbytes(msgs32) != 32 * t or _nbytes(sigs) != 96 * t:
-        raise ValueError("buffer sizes do not match the offsets")
-    if seed is not None and len(seed) != 32:
-        raise ValueError("seed must be 32 bytes")
+    t = _batch_size(off, msgs32, sigs, keys=pks_flat, seed=seed)
     if sharded and seed is None:
         raise ValueError("the ranks must share the seed")
     sd = np.frombuffer(bytes(seed), dtype=np.uint8) if seed is not None else None
@@ -228,9 +236,7 @@ class Registry:
         self.n + j names extra key j, which this call validates like the strict path would (`..._batch_mixed`)."""
         idx = np.ascontiguousarray(indices, dtype=np.uint32)
         off = np.ascontiguousarray(offsets, dtype=np.uint32)
-        t = len(off) - 1
-        if t < 0 or len(idx) != int(off[-1]) or _nbytes(msgs32) != 32 * t or _nbytes(sigs) != 96 * t:
-            raise ValueError("indices / offsets / msgs / sigs sizes are inconsistent")
+        t = _batch_size(off, msgs32, sigs, indices=idx)
         out = np.empty(max(t, 1), dtype=np.int32)
         if extra_keys is not None and _nbytes(extra_keys):
             if _nbytes(extra_keys) % 48:
@@ -242,21 +248,16 @@ class Registry:
                                                                            _lib.ptr(sigs), t, _lib.ptr(out)), "verify_batch_indexed")
         return out[:t]
 
-
-def _registry_verify_batch_all(self, indices, offsets, msgs32, sigs, seed: bytes = None) -> bool:
-    idx = np.ascontiguousarray(indices, dtype=np.uint32)
-    off = np.ascontiguousarray(offsets, dtype=np.uint32)
-    t = len(off) - 1
-    if t < 0 or len(idx) != int(off[-1]) or _nbytes(msgs32) != 32 * t or _nbytes(sigs) != 96 * t:
-        raise ValueError("indices / offsets / msgs / sigs sizes are inconsistent")
-    sd = np.frombuffer(bytes(seed), dtype=np.uint8) if seed is not None else None
-    ok = C.c_int32(0)
-    _lib.check(_lib.lib().b200_fast_aggregate_verify_batch_indexed_all(_lib.ptr(idx), _lib.ptr(off), _lib.ptr(msgs32), _lib.ptr(sigs), t,
-                                                                       _lib.ptr(sd) if sd is not None else 0, C.byref(ok)), "verify_batch_indexed_all")
-    return bool(ok.value)
-
-
-Registry.verify_batch_all = _registry_verify_batch_all
+    def verify_batch_all(self, indices, offsets, msgs32, sigs, seed: bytes = None) -> bool:
+        """`fast_aggregate_verify_batch_all` over registry indices."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint32)
+        off = np.ascontiguousarray(offsets, dtype=np.uint32)
+        t = _batch_size(off, msgs32, sigs, indices=idx, seed=seed)
+        sd = np.frombuffer(bytes(seed), dtype=np.uint8) if seed is not None else None
+        ok = C.c_int32(0)
+        _lib.check(_lib.lib().b200_fast_aggregate_verify_batch_indexed_all(_lib.ptr(idx), _lib.ptr(off), _lib.ptr(msgs32), _lib.ptr(sigs), t,
+                                                                           _lib.ptr(sd) if sd is not None else 0, C.byref(ok)), "verify_batch_indexed_all")
+        return bool(ok.value)
 
 
 def last_kernel_ms() -> float:

@@ -10,7 +10,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdlib>
 
 #include "bls_kernels.cuh"
 #include "pairing_vm.cuh"
@@ -147,10 +146,10 @@ static VmProgramDev g_miller_prog[2], g_final_prog[2];
 static Fp2* g_d_consts = nullptr;
 // Batches with at most this many teams' worth of work run on 16-lane teams: they cannot fill the machine anyway, so the
 // shorter critical path (1 918 / 3 094 rounds instead of 2 493 / 3 842) wins; above it the 8-lane programs' higher
-// throughput does.  B200_VM_TEAM16_MAX overrides (0: never).
+// throughput does.  b200_tune("vm_team16_max") / B200_VM_TEAM16_MAX overrides (0: never).
 static uint32_t g_team16_max = 2048;
 // threads per CTA of the VM kernels (32 | 64 | 128): teams never synchronise across warps, so this only sets how finely the
-// shared-memory register files pack an SM and how the last wave spreads (B200_VM_CTA)
+// shared-memory register files pack an SM and how the last wave spreads (b200_tune("vm_cta") / B200_VM_CTA)
 static int g_vm_cta = 32;   // the registry step was fastest with 32-thread CTAs at T = 2048 and 4096
 void set_vm_team16_max(uint32_t n) { g_team16_max = n; }
 void set_vm_cta(int threads) { if (threads == 32 || threads == 64 || threads == 128) g_vm_cta = threads; }
@@ -214,8 +213,6 @@ int vm_load_programs(const uint32_t* blob, size_t n_words, void* stream) {
 int vm_init(void* stream) {
     if (g_d_consts) return 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (const char* v = getenv("B200_VM_TEAM16_MAX")) g_team16_max = uint32_t(atol(v));
-    if (const char* v = getenv("B200_VM_CTA")) set_vm_cta(atoi(v));
     uint32_t* d_plain = nullptr;
     if (vm_upload<8>(0, st) || vm_upload<16>(1, st)) return 1;
     if (cudaMalloc(&g_d_consts, sizeof(Fp2) * kVmConsts) != cudaSuccess) return 1;

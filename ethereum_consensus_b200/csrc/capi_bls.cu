@@ -9,9 +9,19 @@
 //   stream C: H2D msgs | K4 hash_to_G2 (2T + T threads)                   }
 //   stream A: K5 Miller loops (2T teams of 8 lanes) | K6 Gt product + final exponentiation (T teams) | D2H codes
 // Registry mode skips K1: validated affine keys stay resident in HBM and K2 gathers them by validator index.
+//
+// Every entry point describes its work as one Batch; run_verify() runs it through these phases, in this order:
+//   reserve_buffers  grow-only device buffers
+//   stage_small      the small index arrays, built on the host, one pinned copy to the device (stream A)
+//   key_phase        the key copy and K1, and where K3 / K4 go: one key range (keys_one_range, with the split key copy of
+//                    big strict batches) or several (keys_chunked, which also queues each range's K2 -> K5 -> K6)
+//   pairing_tail     K5 / K6 per tuple: lane-parallel VM or one thread per pair   | or rlc_tail: the whole-batch check
+//   readback         verdicts to the host, event times; then the B200_BLS_TRACE line
 #include <algorithm>
+#include <cctype>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <random>
 #include <string>
 #include <vector>
@@ -56,37 +66,68 @@ struct BlsState {
     // B200_SMALL_ORDER: where the signature / message kernels go relative to the per-key kernel K1: 0 (default) under it on
     // high-priority streams, 1 before it, 2 after it.  With the call-based
     // per-key kernel (a fifth of the code, 12 warps/SM) the overlap beats running them first, with 128-thread CTAs at
-    // T = 4096 and 32-thread CTAs at T = 256.  B200_SMALL_CTA overrides the CTA size (default: 32 up to 1 024 tuples, else 128).
+    // T = 4096 and 32-thread CTAs at T = 256.  B200_BLS_SMALL_CTA overrides the CTA size (default: 32 up to 1 024 tuples, else 128).
     int small_order = 0;
     int small_cta_override = 0;
     bool use_vm = true;  // lane-parallel pairing kernels (B200_PAIRING_VM=0 selects the one-thread-per-pair kernels)
+
+    // only a bls_state() that fails part-way destroys one: a completed state lives as long as the process
+    ~BlsState() {
+        for (cudaStream_t st : {sb, sc, sd, se}) if (st) cudaStreamDestroy(st);
+        for (cudaEvent_t ev : ev_ck) if (ev) cudaEventDestroy(ev);
+        for (cudaEvent_t ev : ev_t) if (ev) cudaEventDestroy(ev);
+        for (cudaEvent_t ev : {ev_join, ev_in, ev_b, ev_c, ev_k0, ev_k1, ev_d0, ev_d1}) if (ev) cudaEventDestroy(ev);
+        cudaFree(d_negg1);
+        cudaFree(d_negg1_pre);
+    }
 };
+
+// Launch-shape knobs: b200_tune(name, value), and at first use the environment variable B200_<NAME> (the name upper-cased),
+// both through the row's setter.
+struct Knob {
+    const char* name;
+    void (*set)(BlsState&, int64_t);
+};
+static const Knob kKnobs[] = {
+    {"bls_chunks", [](BlsState& s, int64_t v) { s.chunks = uint32_t(std::max<int64_t>(1, v)); }},
+    {"bls_chunk_min_tuples", [](BlsState& s, int64_t v) { s.chunk_min_tuples = uint32_t(std::max<int64_t>(2, v)); }},
+    {"bls_chunk_k1_cta", [](BlsState& s, int64_t v) { s.chunk_k1_cta = int(v); }},
+    {"bls_chunk_alt", [](BlsState& s, int64_t v) { s.chunk_alt = v != 0; }},
+    {"bls_key_split", [](BlsState& s, int64_t v) { s.key_split = v != 0; }},
+    {"bls_k1_first_cta", [](BlsState& s, int64_t v) { s.k1_first_cta = (v == 128) ? 128 : 384; }},
+    {"bls_small_cta", [](BlsState& s, int64_t v) { s.small_cta_override = int(v); }},
+    {"vm_team16_max", [](BlsState&, int64_t v) { set_vm_team16_max(uint32_t(std::max<int64_t>(0, v))); }},
+    {"vm_cta", [](BlsState&, int64_t v) { set_vm_cta(int(v)); }},
+};
+
+// The knobs' environment variables, then the settings b200_tune does not take: kernel variants, the pairing kernels,
+// tracing, the side kernels' order and the streams' priorities are fixed for the process at first use.
+static void read_env(BlsState& s, int* side_prio, int* pair_prio) {
+    for (const Knob& k : kKnobs) {
+        std::string var = "B200_";
+        for (const char* c = k.name; *c; c++) var += char(toupper(static_cast<unsigned char>(*c)));
+        if (const char* v = getenv(var.c_str())) k.set(s, atoll(v));
+    }
+    if (const char* v = getenv("B200_G1_VARIANT")) set_g1_variant(atoi(v));
+    if (const char* v = getenv("B200_G1_SMALL_N")) set_g1_small_n(uint32_t(atol(v)));
+    if (const char* v = getenv("B200_PAIRING_VM")) s.use_vm = atoi(v) != 0;
+    if (const char* v = getenv("B200_BLS_TRACE")) s.trace = atoi(v) != 0;
+    if (const char* v = getenv("B200_SMALL_ORDER")) s.small_order = atoi(v);
+    if (const char* v = getenv("B200_SMALL_STREAM_PRIORITY")) *side_prio = atoi(v);   // A/B knob
+    *pair_prio = *side_prio;
+    if (const char* v = getenv("B200_PAIR_STREAM_PRIORITY")) *pair_prio = atoi(v);
+}
 
 static int32_t bls_state(Engine& e, BlsState** out) {
     if (!e.bls) {
-        BlsState* s = new BlsState();
-        if (const char* v = getenv("B200_G1_VARIANT")) set_g1_variant(atoi(v));
-        if (const char* v = getenv("B200_G1_SMALL_N")) set_g1_small_n(uint32_t(atol(v)));
-        if (const char* v = getenv("B200_PAIRING_VM")) s->use_vm = atoi(v) != 0;
-        if (const char* v = getenv("B200_BLS_TRACE")) s->trace = atoi(v) != 0;
-        if (const char* v = getenv("B200_SMALL_ORDER")) s->small_order = atoi(v);
-        if (const char* v = getenv("B200_SMALL_CTA")) s->small_cta_override = atoi(v);
+        std::unique_ptr<BlsState> s(new BlsState());   // freed if a step below fails; the next call starts over
         for (auto& ev : s->ev_t) B200_CUDA_TRY(cudaEventCreate(&ev));
         // High priority only matters for B200_SMALL_ORDER=0 (dispatch under the per-key kernel as its CTAs retire).
-        int prio_lo = 0, prio = 0;
+        int prio_lo = 0, prio = 0, prio_d = 0;
         B200_CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio));          // highest priority
-        if (const char* v = getenv("B200_SMALL_STREAM_PRIORITY")) prio = atoi(v);  // A/B knob
+        read_env(*s, &prio, &prio_d);
         B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->sb, cudaStreamNonBlocking, prio));
         B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->sc, cudaStreamNonBlocking, prio));
-        if (const char* v = getenv("B200_BLS_CHUNKS")) s->chunks = uint32_t(std::max(1, atoi(v)));
-        if (const char* v = getenv("B200_BLS_CHUNK_MIN_TUPLES")) s->chunk_min_tuples = uint32_t(std::max(2, atoi(v)));
-        if (const char* v = getenv("B200_BLS_CHUNK_K1_CTA")) s->chunk_k1_cta = atoi(v);
-        if (const char* v = getenv("B200_BLS_CHUNK_ALT")) s->chunk_alt = atoi(v) != 0;
-        if (const char* v = getenv("B200_BLS_KEY_SPLIT")) s->key_split = atoi(v) != 0;
-        if (const char* v = getenv("B200_BLS_K1_FIRST_CTA")) s->k1_first_cta = atoi(v) == 384 ? 384 : 128;
-        if (const char* v = getenv("B200_BLS_SMALL_CTA")) s->small_cta_override = atoi(v);
-        int prio_d = prio;
-        if (const char* v = getenv("B200_PAIR_STREAM_PRIORITY")) prio_d = atoi(v);
         B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->sd, cudaStreamNonBlocking, prio_d));
         B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->se, cudaStreamNonBlocking, prio_lo));
         for (auto& ev : s->ev_ck) B200_CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
@@ -106,20 +147,9 @@ static int32_t bls_state(Engine& e, BlsState** out) {
         e.launches++;
         B200_CUDA_TRY(cudaGetLastError());
         B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
-        e.bls = s;
+        e.bls = s.release();
     }
     *out = static_cast<BlsState*>(e.bls);
-    return B200_SUCCESS;
-}
-
-struct Guard {
-    std::unique_lock<std::mutex> lk;
-    explicit Guard(Engine& e) : lk(e.mu) {}
-};
-static int32_t check_ready(Engine& e) {
-    if (!e.ready) { e.last_error = "b200_init has not been called (or failed)"; return B200_ERR_NOT_INITIALIZED; }
-    cudaError_t ce = cudaSetDevice(e.device);
-    if (ce != cudaSuccess) { e.last_error = cudaGetErrorString(ce); return B200_ERR_CUDA; }
     return B200_SUCCESS;
 }
 
@@ -128,10 +158,8 @@ enum PairMode { MODE_FAST_AGGREGATE = 0, MODE_AGGREGATE = 1 };
 constexpr size_t kMaxBatchTuples = size_t(1) << 26;
 // keys a `..._batch_mixed` call may bring along (a block carries <= 16 deposits + 16 bls-to-execution changes)
 constexpr size_t kRegistryExtraKeys = size_t(1) << 16;
+constexpr size_t kRlcPart = sizeof(Fp12) + sizeof(G2Jac) + 16;   // one rank's exchanged RLC partial: Gt | G2 | bad flag
 
-// Core: `n_tuples` tuples.  MODE_FAST_AGGREGATE: tuple t sums keys [key_off[t], key_off[t+1]) and checks
-// e(sum, H(msg_t)) e(-g1, sig_t) == 1.  MODE_AGGREGATE: one tuple, pairs (key_i, H(msg_i)) + (-g1, sig).
-// keys: host bytes (strict) or nullptr with `index` (registry gather).  msgs: host bytes + offsets (n_msgs + 1).
 // whole-batch RLC request: when passed, the pairing phase answers ONE boolean for all tuples instead of T codes
 struct RlcReq {
     const uint8_t* seed32;  // scalars r_t = H(seed || t0 + t)
@@ -139,43 +167,79 @@ struct RlcReq {
     bool exchange;          // all-gather the per-rank (Gt, G2) partials over the library's communicator
     int32_t all_ok;         // out
 };
-static int32_t run_verify_impl(Engine& e, BlsState& s, PairMode mode, const uint8_t* keys, uint32_t n_keys,
-                               const uint32_t* index, uint32_t n_index, const uint32_t* key_off, const uint8_t* msgs,
-                               const uint32_t* msg_off, uint32_t n_msgs, const uint8_t* sigs, uint32_t n_tuples,
-                               bool force_fail_shape, int32_t* out_codes, RlcReq* rlc);
-// An early error return must not leave work queued on the side streams (they read the caller's host buffers and the
-// engine's grow-only device buffers): drain all three before handing the error back.
-static int32_t run_verify(Engine& e, BlsState& s, PairMode mode, const uint8_t* keys, uint32_t n_keys,
-                          const uint32_t* index, uint32_t n_index, const uint32_t* key_off, const uint8_t* msgs,
-                          const uint32_t* msg_off, uint32_t n_msgs, const uint8_t* sigs, uint32_t n_tuples,
-                          bool force_fail_shape, int32_t* out_codes, RlcReq* rlc = nullptr) {
-    const int32_t rc = run_verify_impl(e, s, mode, keys, n_keys, index, n_index, key_off, msgs, msg_off, n_msgs, sigs,
-                                       n_tuples, force_fail_shape, out_codes, rlc);
-    if (rc != B200_SUCCESS) {
-        cudaStreamSynchronize(e.stream);
-        cudaStreamSynchronize(s.sb);
-        cudaStreamSynchronize(s.sc);
-        cudaStreamSynchronize(s.sd);
-        cudaStreamSynchronize(s.se);
-        cudaGetLastError();
-    }
-    return rc;
-}
-static int32_t run_verify_impl(Engine& e, BlsState& s, PairMode mode, const uint8_t* keys, uint32_t n_keys,
-                               const uint32_t* index, uint32_t n_index, const uint32_t* key_off, const uint8_t* msgs,
-                               const uint32_t* msg_off, uint32_t n_msgs, const uint8_t* sigs, uint32_t n_tuples,
-                               bool force_fail_shape, int32_t* out_codes, RlcReq* rlc) {
-    if (rlc && (mode != MODE_FAST_AGGREGATE || !s.use_vm)) return B200_ERR_BAD_ARG;
-    // registry gather; with `keys` as well: `n_keys` EXTRA keys (deposits, bls-to-execution changes) validated by this call into
-    // the registry arrays' spare tail, named by indices reg_n + j
-    const bool registry = index != nullptr;
-    const uint32_t T = n_tuples;
-    const uint32_t n_g1 = (mode == MODE_FAST_AGGREGATE ? T : n_keys) + 1;  // + (-g1)
-    const uint32_t n_pairs = (mode == MODE_FAST_AGGREGATE) ? 2 * T : (force_fail_shape ? 0 : n_msgs + 1);
-    const uint32_t n_g2 = n_msgs + T;
-    const uint32_t msg_bytes = msg_off[n_msgs];
 
-    // ---- device buffers
+// One call's work: T tuples.  MODE_FAST_AGGREGATE: tuple t sums keys [key_off[t], key_off[t+1]) and checks
+// e(sum, H(msg_t)) e(-g1, sig_t) == 1.  MODE_AGGREGATE: one tuple, pairs (key_i, H(msg_i)) + (-g1, sig).
+struct Batch {
+    PairMode mode = MODE_FAST_AGGREGATE;
+    // host key bytes (strict); with `index` as well: n_keys EXTRA keys (deposits, bls-to-execution changes) validated by this
+    // call into the registry arrays' spare tail, named by indices reg_n + j
+    const uint8_t* keys = nullptr;
+    uint32_t n_keys = 0;
+    const uint32_t* index = nullptr;   // non-null: registry gather by validator index
+    uint32_t n_index = 0;
+    const uint32_t* key_off = nullptr;
+    const uint8_t* msgs = nullptr;     // host bytes + offsets (n_msgs + 1)
+    const uint32_t* msg_off = nullptr;
+    uint32_t n_msgs = 0;
+    const uint8_t* sigs = nullptr;
+    uint32_t T = 0;
+    bool force_fail_shape = false;     // MODE_AGGREGATE: no pairs, the tuple is flagged EMPTY
+    RlcReq* rlc = nullptr;
+};
+
+// One run_verify call in phases.  The members are the sizes every phase derives from the batch, set once here, and where
+// stage_small put the index arrays.
+struct VerifyRun {
+    Engine& e;
+    BlsState& s;
+    const Batch& b;
+    const uint32_t T = b.T, n_keys = b.n_keys, n_msgs = b.n_msgs;
+    const bool fa = b.mode == MODE_FAST_AGGREGATE, registry = b.index != nullptr;
+    const uint32_t n_g1 = (fa ? T : n_keys) + 1;  // + (-g1)
+    const uint32_t n_pairs = fa ? 2 * T : (b.force_fail_shape ? 0 : n_msgs + 1);
+    const uint32_t n_g2 = n_msgs + T;
+    const uint32_t msg_bytes = b.msg_off[n_msgs];
+    const uint32_t rlc_world = b.rlc && b.rlc->exchange ? uint32_t(comm().world) : 1u;
+    const cudaStream_t sa = e.stream;
+    // set by stage_small: word offsets in s.small, the pair arrays on the device, the pinned area results come back to
+    size_t o_koff = 0, o_index = 0, o_moff = 0;
+    const uint32_t *d_small = nullptr, *d_g1i = nullptr, *d_g2i = nullptr, *d_ptu = nullptr, *d_poff = nullptr;
+    int32_t* h_out = nullptr;
+    bool chunked = false;   // set by key_phase: the pairing chain is already queued on stream D
+
+    int32_t run(int32_t* out_codes);
+    int32_t reserve_buffers();
+    int32_t stage_small();
+    int32_t key_phase();
+    int32_t keys_chunked(uint32_t n_chunks);
+    int32_t keys_one_range(uint32_t k_split);
+    int32_t launch_small();
+    void pairing_tail();
+    int32_t rlc_tail();
+    int32_t readback(void* h_dst, const void* d_src, size_t bytes);
+};
+
+int32_t VerifyRun::run(int32_t* out_codes) {
+    if (b.rlc && (!fa || !s.use_vm)) return B200_ERR_BAD_ARG;
+    int32_t rc;
+    if ((rc = reserve_buffers()) || (rc = stage_small()) || (rc = key_phase())) return rc;
+    if (b.rlc) return rlc_tail();
+    if (!chunked) pairing_tail();   // chunked: every range's Miller loops and final exponentiations are already queued (joined)
+    if ((rc = readback(h_out + 4, s.out.p, size_t(T) * 4))) return rc;
+    if (s.trace) {
+        float a = 0, b1 = 0, c = 0, d = 0, f2 = 0, g2 = 0;
+        cudaEventElapsedTime(&a, s.ev_k0, s.ev_d0); cudaEventElapsedTime(&b1, s.ev_t[0], s.ev_t[1]);
+        cudaEventElapsedTime(&c, s.ev_t[1], s.ev_t[2]); cudaEventElapsedTime(&d, s.ev_t[2], s.ev_t[3]);
+        cudaEventElapsedTime(&f2, s.ev_t[3], s.ev_k1); cudaEventElapsedTime(&g2, s.ev_k0, s.ev_k1);
+        fprintf(stderr, "[b200 bls] pre-K1 %.2f | K1 %.2f | K2 %.2f | wait(streamB) %.2f | miller %.2f | final %.2f | total %.2f ms\n",
+                a, s.last_dominant_ms, b1, c, d, f2, g2);
+    }
+    for (uint32_t t = 0; t < T; t++) out_codes[t] = h_out[4 + t];
+    return B200_SUCCESS;
+}
+
+int32_t VerifyRun::reserve_buffers() {
     B200_CUDA_TRY(s.keys.reserve(size_t(n_keys) * 48 + 64));
     B200_CUDA_TRY(s.key_aff.reserve(size_t(n_keys + 1) * sizeof(G1Aff)));
     B200_CUDA_TRY(s.key_code.reserve(size_t(n_keys + 1) * 4));
@@ -190,40 +254,41 @@ static int32_t run_verify_impl(Engine& e, BlsState& s, PairMode mode, const uint
     B200_CUDA_TRY(s.f.reserve(size_t(n_pairs + 1) * sizeof(Fp12)));
     B200_CUDA_TRY(s.out.reserve(size_t(T + 1) * 4));
     B200_CUDA_TRY(s.h2c_tmp.reserve(size_t(2 * n_msgs + 2) * sizeof(G2Jac)));
-    const uint32_t rlc_world = rlc && rlc->exchange ? uint32_t(comm().world) : 1u;
+    if (!b.rlc) return B200_SUCCESS;
     const uint32_t rlc_part = (T + 31) / 32 + rlc_world + 2;   // capacity of one reduction level (+ gathered partials)
-    if (rlc) {
-        B200_CUDA_TRY(s.rlc_jac.reserve(size_t(T + 1) * sizeof(G1Jac)));
-        B200_CUDA_TRY(s.rlc_g1.reserve(size_t(T + 2) * sizeof(G1Pre)));
-        B200_CUDA_TRY(s.rlc_q.reserve(size_t(T + 1) * sizeof(G2Jac)));
-        B200_CUDA_TRY(s.rlc_fa.reserve(size_t(rlc_part) * sizeof(Fp12)));
-        B200_CUDA_TRY(s.rlc_fb.reserve(size_t(rlc_part) * sizeof(Fp12)));
-        B200_CUDA_TRY(s.rlc_qa.reserve(size_t(rlc_part) * sizeof(G2Jac)));
-        B200_CUDA_TRY(s.rlc_qb.reserve(size_t(rlc_part) * sizeof(G2Jac)));
-        B200_CUDA_TRY(s.rlc_zero.reserve(size_t(T + 8) * 4));
-        B200_CUDA_TRY(s.rlc_idx.reserve(size_t(2 * (T + 1)) * 4));
-        B200_CUDA_TRY(s.rlc_misc.reserve(256));
-        B200_CUDA_TRY(s.rlc_xch.reserve(size_t(rlc_world + 1) * (sizeof(Fp12) + sizeof(G2Jac) + 16)));
-    }
+    B200_CUDA_TRY(s.rlc_jac.reserve(size_t(T + 1) * sizeof(G1Jac)));
+    B200_CUDA_TRY(s.rlc_g1.reserve(size_t(T + 2) * sizeof(G1Pre)));
+    B200_CUDA_TRY(s.rlc_q.reserve(size_t(T + 1) * sizeof(G2Jac)));
+    B200_CUDA_TRY(s.rlc_fa.reserve(size_t(rlc_part) * sizeof(Fp12)));
+    B200_CUDA_TRY(s.rlc_fb.reserve(size_t(rlc_part) * sizeof(Fp12)));
+    B200_CUDA_TRY(s.rlc_qa.reserve(size_t(rlc_part) * sizeof(G2Jac)));
+    B200_CUDA_TRY(s.rlc_qb.reserve(size_t(rlc_part) * sizeof(G2Jac)));
+    B200_CUDA_TRY(s.rlc_zero.reserve(size_t(T + 8) * 4));
+    B200_CUDA_TRY(s.rlc_idx.reserve(size_t(2 * (T + 1)) * 4));
+    B200_CUDA_TRY(s.rlc_misc.reserve(256));
+    B200_CUDA_TRY(s.rlc_xch.reserve(size_t(rlc_world + 1) * kRlcPart));
+    return B200_SUCCESS;
+}
 
-    // ---- small host-built arrays, one staged copy: [key_off | index | msg_off | g1_idx | g2_idx | pair_tuple | pair_off]
-    const uint32_t n_koff = (mode == MODE_FAST_AGGREGATE) ? T + 1 : 2;
+// small host-built arrays, one staged copy on stream A: [key_off | index | msg_off | g1_idx | g2_idx | pair_tuple | pair_off]
+int32_t VerifyRun::stage_small() {
+    const uint32_t n_koff = fa ? T + 1 : 2;
     std::vector<uint32_t> small;
-    small.reserve(size_t(n_koff) + n_index + n_msgs + 1 + 3 * size_t(n_pairs) + T + 1 + 8);
-    const size_t o_koff = small.size();
-    if (mode == MODE_FAST_AGGREGATE) small.insert(small.end(), key_off, key_off + T + 1);
+    small.reserve(size_t(n_koff) + b.n_index + n_msgs + 1 + 3 * size_t(n_pairs) + T + 1 + 8);
+    o_koff = small.size();
+    if (fa) small.insert(small.end(), b.key_off, b.key_off + T + 1);
     else { small.push_back(0); small.push_back(n_keys); }
-    const size_t o_index = small.size();
-    if (registry) small.insert(small.end(), index, index + n_index);
-    const size_t o_moff = small.size();
-    small.insert(small.end(), msg_off, msg_off + n_msgs + 1);
+    o_index = small.size();
+    if (registry) small.insert(small.end(), b.index, b.index + b.n_index);
+    o_moff = small.size();
+    small.insert(small.end(), b.msg_off, b.msg_off + n_msgs + 1);
     const size_t o_g1i = small.size();
     small.resize(small.size() + 3 * size_t(n_pairs) + T + 1);
     uint32_t* g1i = small.data() + o_g1i;
     uint32_t* g2i = g1i + n_pairs;
     uint32_t* ptu = g2i + n_pairs;
     uint32_t* poff = ptu + n_pairs;
-    if (mode == MODE_FAST_AGGREGATE) {
+    if (fa) {
         for (uint32_t t = 0; t < T; t++) {
             g1i[2 * t] = t;          g2i[2 * t] = t;          // (agg_t, H(msg_t))
             g1i[2 * t + 1] = T;      g2i[2 * t + 1] = n_msgs + t;  // (-g1, sig_t)
@@ -237,28 +302,26 @@ static int32_t run_verify_impl(Engine& e, BlsState& s, PairMode mode, const uint
         poff[0] = 0; poff[1] = n_pairs;
     }
     const size_t small_bytes = small.size() * 4;
-    const size_t kRlcPart = sizeof(Fp12) + sizeof(G2Jac) + 16;   // one rank's exchanged partial: Gt | G2 | bad flag
     B200_CUDA_TRY(s.stage.reserve(small_bytes + size_t(T + 1) * 4 + 64 +
-                                  (rlc ? 256 + size_t(rlc_world) * kRlcPart + size_t(8 + 2 * (T + 1)) * 4 : 0)));
+                                  (b.rlc ? 256 + size_t(rlc_world) * kRlcPart + size_t(8 + 2 * (T + 1)) * 4 : 0)));
     B200_CUDA_TRY(s.small.reserve(small_bytes + 64));
     memcpy(s.stage.p, small.data(), small_bytes);
-    int32_t* h_out = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(s.stage.p) + ((small_bytes + 15) & ~size_t(15)));
-
-    cudaStream_t sa = e.stream, sb = s.sb, sc = s.sc;
-    uint32_t* d_small = static_cast<uint32_t*>(s.small.p);
-    G1Aff* d_g1 = static_cast<G1Aff*>(s.g1pts.p);
-    G2Aff* d_g2 = static_cast<G2Aff*>(s.g2pts.p);
-    const G1Aff* key_aff = registry ? static_cast<const G1Aff*>(s.reg_aff.p) : static_cast<const G1Aff*>(s.key_aff.p);
-    const int32_t* key_code = registry ? static_cast<const int32_t*>(s.reg_code.p) : static_cast<const int32_t*>(s.key_code.p);
-    // where the per-key kernel writes: the call's own arrays, or (registry + extra keys) the tail behind the reg_n resident keys
-    G1Aff* k1_aff = registry ? static_cast<G1Aff*>(s.reg_aff.p) + s.reg_n : static_cast<G1Aff*>(s.key_aff.p);
-    int32_t* k1_code = registry ? static_cast<int32_t*>(s.reg_code.p) + s.reg_n : static_cast<int32_t*>(s.key_code.p);
-
-    // ---- small arrays + keys (stream A); signatures / messages on streams B, C (they overlap the 100 MB key copy)
-    B200_CUDA_TRY(cudaMemcpyAsync(d_small, s.stage.p, small_bytes, cudaMemcpyHostToDevice, sa));
+    h_out = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(s.stage.p) + ((small_bytes + 15) & ~size_t(15)));
+    d_small = static_cast<const uint32_t*>(s.small.p);
+    d_g1i = d_small + o_g1i;
+    d_g2i = d_g1i + n_pairs;
+    d_ptu = d_g2i + n_pairs;
+    d_poff = d_ptu + n_pairs;
+    B200_CUDA_TRY(cudaMemcpyAsync(s.small.p, s.stage.p, small_bytes, cudaMemcpyHostToDevice, sa));
     B200_CUDA_TRY(cudaEventRecord(s.ev_in, sa));
+    return B200_SUCCESS;
+}
+
+// Key copy and K1, with the signature / message kernels placed by B200_SMALL_ORDER.  The one place that picks the shape:
+// several key ranges (b200_tune("bls_chunks")), one range with the key copy split in two, or one plain range.
+int32_t VerifyRun::key_phase() {
     const bool have_k1 = n_keys != 0;
-    const uint32_t n_chunks = (mode == MODE_FAST_AGGREGATE && !rlc && s.use_vm && have_k1 && !registry && s.small_order == 0 && !force_fail_shape &&
+    const uint32_t n_chunks = (fa && !b.rlc && s.use_vm && have_k1 && !registry && s.small_order == 0 && !b.force_fail_shape &&
                                s.chunks > 1 && T >= s.chunk_min_tuples) ? std::min(s.chunks, BlsState::kMaxChunks) : 1u;
     // Big strict batches: the first kSplitWaves full waves of the per-key kernel start as soon as THEIR keys have arrived; the rest of
     // the key bytes (~90 MB at T = 4096) cross PCIe on stream E under that first launch, and the second launch follows them there
@@ -268,20 +331,8 @@ static int32_t run_verify_impl(Engine& e, BlsState& s, PairMode mode, const uint
     constexpr uint32_t kSplitWaves = 4, kSplitKeys = kSplitWaves * 148u * 384u;
     const uint32_t k_split = (s.key_split && have_k1 && !registry && n_chunks == 1 && s.small_order == 0 && n_keys >= 4u * kSplitKeys)
                                  ? kSplitKeys : n_keys;
-    if (n_keys) B200_CUDA_TRY(cudaMemcpyAsync(s.keys.p, keys, size_t(k_split) * 48, cudaMemcpyHostToDevice, sa));
+    if (n_keys) B200_CUDA_TRY(cudaMemcpyAsync(s.keys.p, b.keys, size_t(k_split) * 48, cudaMemcpyHostToDevice, sa));
     B200_CUDA_TRY(cudaEventRecord(s.ev_k0, sa));
-    auto launch_small = [&]() -> int32_t {
-        B200_CUDA_TRY(cudaStreamWaitEvent(sb, s.ev_in, 0));
-        B200_CUDA_TRY(cudaStreamWaitEvent(sc, s.ev_in, 0));
-        if (T) B200_CUDA_TRY(cudaMemcpyAsync(s.sigs.p, sigs, size_t(T) * 96, cudaMemcpyHostToDevice, sb));
-        if (msg_bytes) B200_CUDA_TRY(cudaMemcpyAsync(s.msgs.p, msgs, msg_bytes, cudaMemcpyHostToDevice, sc));
-        launch_g2_sig_decode(static_cast<const uint8_t*>(s.sigs.p), T, d_g2 + n_msgs, static_cast<int32_t*>(s.sig_code.p), sb);
-        launch_hash_to_g2(static_cast<const uint8_t*>(s.msgs.p), d_small + o_moff, n_msgs, d_g2, s.h2c_tmp.p, sc);
-        e.launches += (T ? 1 : 0) + (n_msgs ? 2 : 0);
-        B200_CUDA_TRY(cudaEventRecord(s.ev_b, sb));
-        B200_CUDA_TRY(cudaEventRecord(s.ev_c, sc));
-        return B200_SUCCESS;
-    };
     // packed CTAs only when there is a big per-key kernel to run under; alone (registry mode, small batches) they spread
     set_small_cta(s.small_cta_override ? s.small_cta_override : ((have_k1 && n_keys >= 148u * 384u && s.small_order == 0 && T > 1024) ? 128 : 32));
     if (have_k1 && s.small_order == 1) {   // signatures / messages first, the per-key kernel only afterwards
@@ -292,246 +343,333 @@ static int32_t run_verify_impl(Engine& e, BlsState& s, PairMode mode, const uint
     }
     // ---- stream A: public keys
     B200_CUDA_TRY(cudaEventRecord(s.ev_d0, sa));
-    const uint32_t* d_g1i = nullptr; const uint32_t* d_g2i = nullptr; const uint32_t* d_ptu = nullptr; const uint32_t* d_poff = nullptr;
-    bool chunked = false;
-    const G1Aff* pair_g1 = d_g1;
-    if (n_chunks > 1) {
-        // Chunked strict batch: tuple range c's keys are validated on stream A while range c-1's aggregate -> Miller ->
-        // final-exponentiation chain (latency-bound: ~1/3 of the IMAD pipe when alone) runs on stream D in the slots the
-        // per-key kernel's retiring 128-thread CTAs leave.  Same kernels, same per-tuple arithmetic, same code vector.
-        chunked = true;
-        cudaStream_t sd = s.sd;
-        d_g1i = d_small + o_g1i; d_g2i = d_g1i + n_pairs; d_ptu = d_g2i + n_pairs; d_poff = d_ptu + n_pairs;
-        uint32_t tb[BlsState::kMaxChunks + 1];
-        for (uint32_t c = 0; c <= n_chunks; c++) tb[c] = uint32_t(uint64_t(T) * c / n_chunks);
-        B200_CUDA_TRY(cudaStreamWaitEvent(s.se, s.ev_k0, 0));   // the key bytes
-        for (uint32_t c = 0; c < n_chunks; c++) {
-            const uint32_t k0 = key_off[tb[c]], k1 = key_off[tb[c + 1]];
-            cudaStream_t sk = ((c & 1u) && s.chunk_alt) ? s.se : sa;
-            launch_g1_validate(static_cast<const uint8_t*>(s.keys.p) + size_t(k0) * 48, k1 - k0, static_cast<G1Aff*>(s.key_aff.p) + k0,
-                               static_cast<int32_t*>(s.key_code.p) + k0, sk, s.chunk_k1_cta);
-            if (k1 > k0) e.launches++;
-            B200_CUDA_TRY(cudaEventRecord(s.ev_ck[c], sk));
-            if (c == 0) {   // signature / message kernels right behind the first range, as in the one-range flow
-                int32_t rc = launch_small();
-                if (rc) return rc;
-            }
-        }
-        if (s.chunk_alt)
-            for (uint32_t c = 1; c < n_chunks; c += 2) B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_ck[c], 0));
-        B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
-        B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_in, 0));   // the small index arrays
-        B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_b, 0));
-        B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_c, 0));
-        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sd));
-        int32_t* d_pk = static_cast<int32_t*>(s.pk_code.p);
-        uint32_t* d_fl = static_cast<uint32_t*>(s.flags.p);
-        const int32_t* d_sc = static_cast<const int32_t*>(s.sig_code.p);
-        for (uint32_t c = 0; c < n_chunks; c++) {
-            const uint32_t t0 = tb[c], nt = tb[c + 1] - tb[c];
-            if (!nt) continue;
-            B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_ck[c], 0));
-            launch_g1_aggregate(key_aff, key_code, nullptr, d_small + o_koff + t0, nt, nullptr, static_cast<G1Pre*>(s.g1pre.p) + t0,
-                                d_pk + t0, d_fl + t0, 0u, sd, nullptr);
-            // pair-indexed arrays start at 2 t0 (values are absolute); tuple-indexed code arrays are read through pair_tuple
-            launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i + 2 * t0, d_g2, d_g2i + 2 * t0, d_ptu + 2 * t0, d_pk, d_fl, d_sc,
-                             2 * nt, static_cast<Fp12*>(s.f.p) + 2 * size_t(t0), sd);
-            // f BASE + absolute pair offsets; tuple-indexed arrays start at t0
-            launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff + t0, d_pk + t0, d_fl + t0, d_sc + t0, nt,
-                            static_cast<int32_t*>(s.out.p) + t0, sd);
-            e.launches += 3;
-        }
-        B200_CUDA_TRY(cudaEventRecord(s.ev_join, sd));
-        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_join, 0));
-        if (s.trace) { cudaEventRecord(s.ev_t[0], sa); cudaEventRecord(s.ev_t[1], sa); cudaEventRecord(s.ev_t[2], sa); cudaEventRecord(s.ev_t[3], sa); }
-    }
-    if (!chunked) {
-        if (have_k1) {
-            launch_g1_validate(static_cast<const uint8_t*>(s.keys.p), k_split, k1_aff, k1_code, sa, k_split < n_keys ? s.k1_first_cta : 0);
-            e.launches++;
-        }
-        if (!(have_k1 && s.small_order == 1)) {
-            if (have_k1 && s.small_order == 2) {  // strictly after the per-key kernel
-                B200_CUDA_TRY(cudaEventRecord(s.ev_in, sa));
-            }
+    chunked = n_chunks > 1;
+    return chunked ? keys_chunked(n_chunks) : keys_one_range(k_split);
+}
+
+// Chunked strict batch: tuple range c's keys are validated on stream A while range c-1's aggregate -> Miller ->
+// final-exponentiation chain (latency-bound: ~1/3 of the IMAD pipe when alone) runs on stream D in the slots the
+// per-key kernel's retiring 128-thread CTAs leave.  Same kernels, same per-tuple arithmetic, same code vector.
+int32_t VerifyRun::keys_chunked(uint32_t n_chunks) {
+    cudaStream_t sd = s.sd;
+    uint32_t tb[BlsState::kMaxChunks + 1];
+    for (uint32_t c = 0; c <= n_chunks; c++) tb[c] = uint32_t(uint64_t(T) * c / n_chunks);
+    B200_CUDA_TRY(cudaStreamWaitEvent(s.se, s.ev_k0, 0));   // the key bytes
+    for (uint32_t c = 0; c < n_chunks; c++) {
+        const uint32_t k0 = b.key_off[tb[c]], k1 = b.key_off[tb[c + 1]];
+        cudaStream_t sk = ((c & 1u) && s.chunk_alt) ? s.se : sa;
+        launch_g1_validate(static_cast<const uint8_t*>(s.keys.p) + size_t(k0) * 48, k1 - k0, static_cast<G1Aff*>(s.key_aff.p) + k0,
+                           static_cast<int32_t*>(s.key_code.p) + k0, sk, s.chunk_k1_cta);
+        if (k1 > k0) e.launches++;
+        B200_CUDA_TRY(cudaEventRecord(s.ev_ck[c], sk));
+        if (c == 0) {   // signature / message kernels right behind the first range, as in the one-range flow
             int32_t rc = launch_small();
             if (rc) return rc;
         }
-        if (k_split < n_keys) {   // the remaining keys: copy strictly after the first part's (one PCIe link), then their launch
-            B200_CUDA_TRY(cudaStreamWaitEvent(s.se, s.ev_k0, 0));
-            B200_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(s.keys.p) + size_t(k_split) * 48, keys + size_t(k_split) * 48,
-                                          size_t(n_keys - k_split) * 48, cudaMemcpyHostToDevice, s.se));
-            launch_g1_validate(static_cast<const uint8_t*>(s.keys.p) + size_t(k_split) * 48, n_keys - k_split, k1_aff + k_split,
-                               k1_code + k_split, s.se, 384);
-            e.launches++;
-            B200_CUDA_TRY(cudaEventRecord(s.ev_ck[0], s.se));
-            B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_ck[0], 0));
-        }
-        B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
-        if (s.trace) cudaEventRecord(s.ev_t[0], sa);
-        const uint32_t n_agg_tuples = (mode == MODE_FAST_AGGREGATE) ? T : 1;
-        launch_g1_aggregate(key_aff, key_code, registry ? d_small + o_index : nullptr, d_small + o_koff, n_agg_tuples,
-                            (mode == MODE_FAST_AGGREGATE && !s.use_vm) ? d_g1 : nullptr,
-                            (mode == MODE_FAST_AGGREGATE && s.use_vm) ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
-                            static_cast<int32_t*>(s.pk_code.p), static_cast<uint32_t*>(s.flags.p),
-                            force_fail_shape ? uint32_t(TUPLE_FLAG_EMPTY) : 0u, sa,
-                            rlc ? static_cast<G1Jac*>(s.rlc_jac.p) : nullptr);
-        e.launches++;
-        if (mode == MODE_FAST_AGGREGATE) {
-            B200_CUDA_TRY(cudaMemcpyAsync(d_g1 + T, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
-            B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
-        } else {
-            G1Aff* ka = static_cast<G1Aff*>(s.key_aff.p);
-            B200_CUDA_TRY(cudaMemcpyAsync(ka + n_keys, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
-            pair_g1 = ka;  // len(msgs) != len(pks) or no keys: flagged EMPTY above -> VERIFY_FAIL after the decoding checks
-        }
-        // ---- join, pairing
-        if (s.trace) cudaEventRecord(s.ev_t[1], sa);
-        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_b, 0));
-        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_c, 0));
-        if (s.trace) cudaEventRecord(s.ev_t[2], sa);
     }
-    d_g1i = d_small + o_g1i;
-    d_g2i = d_g1i + n_pairs;
-    d_ptu = d_g2i + n_pairs;
-    d_poff = d_ptu + n_pairs;
-    if (rlc) {
-        // ---- RLC whole-batch check (bls_rlc.cu): T Miller loops + ONE final exponentiation
-        const size_t kPart = kRlcPart;
-        uint8_t* h_x = reinterpret_cast<uint8_t*>(h_out + 16);                    // gathered partials (their bad flags are read on the host)
-        uint32_t* d_zero = static_cast<uint32_t*>(s.rlc_zero.p);  // "every tuple alive" code arrays for the VM kernels
-        uint32_t* d_idx = static_cast<uint32_t*>(s.rlc_idx.p);   // [0..T] identity (g1 / tuple index) | [0..T-1, n_g2] (H_t, then S)
-        uint8_t* d_misc = static_cast<uint8_t*>(s.rlc_misc.p);    // [0,32) seed words | [32,36) bad flag | [64,68) final code
-        G1Pre* d_rg1 = static_cast<G1Pre*>(s.rlc_g1.p);
-        G2Jac* d_rq = static_cast<G2Jac*>(s.rlc_q.p);
-        B200_CUDA_TRY(cudaMemsetAsync(d_zero, 0, size_t(T + 8) * 4, sa));
-        B200_CUDA_TRY(cudaMemsetAsync(d_misc + 32, 0, 96, sa));
-        {   // seed words + index arrays through the pinned staging area (behind the small arrays and the code slots)
-            uint32_t* h = reinterpret_cast<uint32_t*>(h_x + ((size_t(rlc_world) * kPart + 63) & ~size_t(63)));
-            for (int i = 0; i < 8; i++)
-                h[i] = (uint32_t(rlc->seed32[4 * i]) << 24) | (uint32_t(rlc->seed32[4 * i + 1]) << 16) | (uint32_t(rlc->seed32[4 * i + 2]) << 8) | rlc->seed32[4 * i + 3];
-            uint32_t* hi = h + 8;
-            for (uint32_t t = 0; t <= T; t++) { hi[t] = t; hi[T + 1 + t] = t < T ? t : n_g2; }
-            B200_CUDA_TRY(cudaMemcpyAsync(d_misc, h, 32, cudaMemcpyHostToDevice, sa));
-            B200_CUDA_TRY(cudaMemcpyAsync(d_idx, hi, size_t(2 * (T + 1)) * 4, cudaMemcpyHostToDevice, sa));
+    if (s.chunk_alt)
+        for (uint32_t c = 1; c < n_chunks; c += 2) B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_ck[c], 0));
+    B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
+    B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_in, 0));   // the small index arrays
+    B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_b, 0));
+    B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_c, 0));
+    B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sd));
+    int32_t* d_pk = static_cast<int32_t*>(s.pk_code.p);
+    uint32_t* d_fl = static_cast<uint32_t*>(s.flags.p);
+    const int32_t* d_sc = static_cast<const int32_t*>(s.sig_code.p);
+    for (uint32_t c = 0; c < n_chunks; c++) {
+        const uint32_t t0 = tb[c], nt = tb[c + 1] - tb[c];
+        if (!nt) continue;
+        B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_ck[c], 0));
+        launch_g1_aggregate(static_cast<const G1Aff*>(s.key_aff.p), static_cast<const int32_t*>(s.key_code.p), nullptr, d_small + o_koff + t0,
+                            nt, nullptr, static_cast<G1Pre*>(s.g1pre.p) + t0, d_pk + t0, d_fl + t0, 0u, sd, nullptr);
+        // pair-indexed arrays start at 2 t0 (values are absolute); tuple-indexed code arrays are read through pair_tuple
+        launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i + 2 * t0, static_cast<const G2Aff*>(s.g2pts.p), d_g2i + 2 * t0,
+                         d_ptu + 2 * t0, d_pk, d_fl, d_sc, 2 * nt, static_cast<Fp12*>(s.f.p) + 2 * size_t(t0), sd);
+        // f BASE + absolute pair offsets; tuple-indexed arrays start at t0
+        launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff + t0, d_pk + t0, d_fl + t0, d_sc + t0, nt,
+                        static_cast<int32_t*>(s.out.p) + t0, sd);
+        e.launches += 3;
+    }
+    B200_CUDA_TRY(cudaEventRecord(s.ev_join, sd));
+    B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_join, 0));
+    if (s.trace) { cudaEventRecord(s.ev_t[0], sa); cudaEventRecord(s.ev_t[1], sa); cudaEventRecord(s.ev_t[2], sa); cudaEventRecord(s.ev_t[3], sa); }
+    return B200_SUCCESS;
+}
+
+// One key range: K1 (two launches when the key copy is split at k_split), the signature / message kernels, K2, and the join
+int32_t VerifyRun::keys_one_range(uint32_t k_split) {
+    const bool have_k1 = n_keys != 0;
+    G1Aff* d_g1 = static_cast<G1Aff*>(s.g1pts.p);
+    const G1Aff* key_aff = registry ? static_cast<const G1Aff*>(s.reg_aff.p) : static_cast<const G1Aff*>(s.key_aff.p);
+    const int32_t* key_code = registry ? static_cast<const int32_t*>(s.reg_code.p) : static_cast<const int32_t*>(s.key_code.p);
+    // where the per-key kernel writes: the call's own arrays, or (registry + extra keys) the tail behind the reg_n resident keys
+    G1Aff* k1_aff = registry ? static_cast<G1Aff*>(s.reg_aff.p) + s.reg_n : static_cast<G1Aff*>(s.key_aff.p);
+    int32_t* k1_code = registry ? static_cast<int32_t*>(s.reg_code.p) + s.reg_n : static_cast<int32_t*>(s.key_code.p);
+    if (have_k1) {
+        launch_g1_validate(static_cast<const uint8_t*>(s.keys.p), k_split, k1_aff, k1_code, sa, k_split < n_keys ? s.k1_first_cta : 0);
+        e.launches++;
+    }
+    if (!(have_k1 && s.small_order == 1)) {
+        if (have_k1 && s.small_order == 2) {  // strictly after the per-key kernel
+            B200_CUDA_TRY(cudaEventRecord(s.ev_in, sa));
         }
-        launch_rlc_scale(static_cast<const G1Jac*>(s.rlc_jac.p), d_g2 + n_msgs, static_cast<const int32_t*>(s.pk_code.p),
-                         static_cast<const uint32_t*>(s.flags.p), static_cast<const int32_t*>(s.sig_code.p),
-                         reinterpret_cast<const uint32_t*>(d_misc), rlc->t0, T, d_rg1, d_rq, reinterpret_cast<int32_t*>(d_misc + 32), sa);
-        B200_CUDA_TRY(cudaMemcpyAsync(d_rg1 + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
+        int32_t rc = launch_small();
+        if (rc) return rc;
+    }
+    if (k_split < n_keys) {   // the remaining keys: copy strictly after the first part's (one PCIe link), then their launch
+        B200_CUDA_TRY(cudaStreamWaitEvent(s.se, s.ev_k0, 0));
+        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(s.keys.p) + size_t(k_split) * 48, b.keys + size_t(k_split) * 48,
+                                      size_t(n_keys - k_split) * 48, cudaMemcpyHostToDevice, s.se));
+        launch_g1_validate(static_cast<const uint8_t*>(s.keys.p) + size_t(k_split) * 48, n_keys - k_split, k1_aff + k_split,
+                           k1_code + k_split, s.se, 384);
+        e.launches++;
+        B200_CUDA_TRY(cudaEventRecord(s.ev_ck[0], s.se));
+        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_ck[0], 0));
+    }
+    B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
+    if (s.trace) cudaEventRecord(s.ev_t[0], sa);
+    launch_g1_aggregate(key_aff, key_code, registry ? d_small + o_index : nullptr, d_small + o_koff, fa ? T : 1,
+                        (fa && !s.use_vm) ? d_g1 : nullptr, (fa && s.use_vm) ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
+                        static_cast<int32_t*>(s.pk_code.p), static_cast<uint32_t*>(s.flags.p),
+                        b.force_fail_shape ? uint32_t(TUPLE_FLAG_EMPTY) : 0u, sa, b.rlc ? static_cast<G1Jac*>(s.rlc_jac.p) : nullptr);
+    e.launches++;
+    if (fa) {
+        B200_CUDA_TRY(cudaMemcpyAsync(d_g1 + T, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
+        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
+    } else {   // the pairs read the key array itself (pairing_tail)
+        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Aff*>(s.key_aff.p) + n_keys, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
+    }
+    // ---- join, pairing
+    if (s.trace) cudaEventRecord(s.ev_t[1], sa);
+    B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_b, 0));
+    B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_c, 0));
+    if (s.trace) cudaEventRecord(s.ev_t[2], sa);
+    return B200_SUCCESS;
+}
+
+// signatures on stream B, messages on stream C, both behind the small arrays (ev_in); done: ev_b, ev_c
+int32_t VerifyRun::launch_small() {
+    cudaStream_t sb = s.sb, sc = s.sc;
+    B200_CUDA_TRY(cudaStreamWaitEvent(sb, s.ev_in, 0));
+    B200_CUDA_TRY(cudaStreamWaitEvent(sc, s.ev_in, 0));
+    if (T) B200_CUDA_TRY(cudaMemcpyAsync(s.sigs.p, b.sigs, size_t(T) * 96, cudaMemcpyHostToDevice, sb));
+    if (msg_bytes) B200_CUDA_TRY(cudaMemcpyAsync(s.msgs.p, b.msgs, msg_bytes, cudaMemcpyHostToDevice, sc));
+    launch_g2_sig_decode(static_cast<const uint8_t*>(s.sigs.p), T, static_cast<G2Aff*>(s.g2pts.p) + n_msgs, static_cast<int32_t*>(s.sig_code.p), sb);
+    launch_hash_to_g2(static_cast<const uint8_t*>(s.msgs.p), d_small + o_moff, n_msgs, static_cast<G2Aff*>(s.g2pts.p), s.h2c_tmp.p, sc);
+    e.launches += (T ? 1 : 0) + (n_msgs ? 2 : 0);
+    B200_CUDA_TRY(cudaEventRecord(s.ev_b, sb));
+    B200_CUDA_TRY(cudaEventRecord(s.ev_c, sc));
+    return B200_SUCCESS;
+}
+
+// Miller loops and final exponentiations per tuple on stream A: the lane-parallel VM, or one thread per pair
+void VerifyRun::pairing_tail() {
+    const G2Aff* d_g2 = static_cast<const G2Aff*>(s.g2pts.p);
+    const int32_t* d_pk = static_cast<const int32_t*>(s.pk_code.p);
+    const uint32_t* d_fl = static_cast<const uint32_t*>(s.flags.p);
+    const int32_t* d_sc = static_cast<const int32_t*>(s.sig_code.p);
+    if (fa && s.use_vm) {
+        launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
         if (s.trace) cudaEventRecord(s.ev_t[3], sa);
-        Fp12* fbuf[2] = {static_cast<Fp12*>(s.rlc_fa.p), static_cast<Fp12*>(s.rlc_fb.p)};
-        G2Jac* qbuf[2] = {static_cast<G2Jac*>(s.rlc_qa.p), static_cast<G2Jac*>(s.rlc_qb.p)};
-        // S = sum_t r_t sig_t first (warp-shuffle folds T -> T/32 -> ... -> 1): its pair (-g1, S) then rides in the SAME
-        // Miller launch as the T tuple pairs instead of costing a second, latency-bound launch of one team
-        const G2Jac* qi = d_rq;
-        uint32_t n_cur = T;
-        int pp = 0;
-        do {
-            n_cur = launch_rlc_reduce(nullptr, qi, n_cur, nullptr, qbuf[pp], sa);
-            e.launches++;
-            qi = qbuf[pp]; pp ^= 1;
-        } while (n_cur > 1);
-        launch_rlc_finish(qi, d_g2 + n_g2, sa);
-        // T + 1 Miller loops on the lane-parallel VM: (r_t agg_t, H_t) for every tuple and (-g1, S)
-        launch_vm_miller(d_rg1, d_idx, d_g2, d_idx + T + 1, d_zero, reinterpret_cast<const int32_t*>(d_zero), d_zero,
-                         reinterpret_cast<const int32_t*>(d_zero), T + 1, static_cast<Fp12*>(s.f.p), sa);
-        // Gt product of the T + 1 Miller values, again by warp-shuffle folds
-        const Fp12* fi = static_cast<const Fp12*>(s.f.p);
-        n_cur = T + 1;
-        pp = 0;
+        launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
+    } else {
+        // aggregate_verify pairs the keys themselves: len(msgs) != len(pks) or no keys was flagged EMPTY by K2 -> VERIFY_FAIL
+        // after the decoding checks
+        const G1Aff* pair_g1 = static_cast<const G1Aff*>(fa ? s.g1pts.p : s.key_aff.p);
+        launch_miller(pair_g1, d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
+        launch_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
+    }
+    e.launches += (n_pairs ? 1 : 0) + (T ? 1 : 0);
+}
+
+// `bytes` of results into the pinned area once every stream has finished; the call's kernel and per-key times
+int32_t VerifyRun::readback(void* h_dst, const void* d_src, size_t bytes) {
+    B200_CUDA_TRY(cudaEventRecord(s.ev_k1, sa));
+    B200_CUDA_TRY(cudaGetLastError());
+    B200_CUDA_TRY(cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, sa));
+    B200_CUDA_TRY(cudaStreamSynchronize(sa));
+    B200_CUDA_TRY(cudaStreamSynchronize(s.sb));
+    B200_CUDA_TRY(cudaStreamSynchronize(s.sc));
+    if (chunked) B200_CUDA_TRY(cudaStreamSynchronize(s.sd));
+    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, s.ev_k0, s.ev_k1));
+    B200_CUDA_TRY(cudaEventElapsedTime(&s.last_dominant_ms, s.ev_d0, s.ev_d1));
+    return B200_SUCCESS;
+}
+
+// ---- RLC whole-batch check (bls_rlc.cu): T Miller loops + ONE final exponentiation
+int32_t VerifyRun::rlc_tail() {
+    RlcReq* rlc = b.rlc;
+    G2Aff* d_g2 = static_cast<G2Aff*>(s.g2pts.p);
+    const size_t kPart = kRlcPart;
+    uint8_t* h_x = reinterpret_cast<uint8_t*>(h_out + 16);                    // gathered partials (their bad flags are read on the host)
+    uint32_t* d_zero = static_cast<uint32_t*>(s.rlc_zero.p);  // "every tuple alive" code arrays for the VM kernels
+    uint32_t* d_idx = static_cast<uint32_t*>(s.rlc_idx.p);   // [0..T] identity (g1 / tuple index) | [0..T-1, n_g2] (H_t, then S)
+    uint8_t* d_misc = static_cast<uint8_t*>(s.rlc_misc.p);    // [0,32) seed words | [32,36) bad flag | [64,68) final code
+    G1Pre* d_rg1 = static_cast<G1Pre*>(s.rlc_g1.p);
+    G2Jac* d_rq = static_cast<G2Jac*>(s.rlc_q.p);
+    B200_CUDA_TRY(cudaMemsetAsync(d_zero, 0, size_t(T + 8) * 4, sa));
+    B200_CUDA_TRY(cudaMemsetAsync(d_misc + 32, 0, 96, sa));
+    {   // seed words + index arrays through the pinned staging area (behind the small arrays and the code slots)
+        uint32_t* h = reinterpret_cast<uint32_t*>(h_x + ((size_t(rlc_world) * kPart + 63) & ~size_t(63)));
+        for (int i = 0; i < 8; i++)
+            h[i] = (uint32_t(rlc->seed32[4 * i]) << 24) | (uint32_t(rlc->seed32[4 * i + 1]) << 16) | (uint32_t(rlc->seed32[4 * i + 2]) << 8) | rlc->seed32[4 * i + 3];
+        uint32_t* hi = h + 8;
+        for (uint32_t t = 0; t <= T; t++) { hi[t] = t; hi[T + 1 + t] = t < T ? t : n_g2; }
+        B200_CUDA_TRY(cudaMemcpyAsync(d_misc, h, 32, cudaMemcpyHostToDevice, sa));
+        B200_CUDA_TRY(cudaMemcpyAsync(d_idx, hi, size_t(2 * (T + 1)) * 4, cudaMemcpyHostToDevice, sa));
+    }
+    launch_rlc_scale(static_cast<const G1Jac*>(s.rlc_jac.p), d_g2 + n_msgs, static_cast<const int32_t*>(s.pk_code.p),
+                     static_cast<const uint32_t*>(s.flags.p), static_cast<const int32_t*>(s.sig_code.p),
+                     reinterpret_cast<const uint32_t*>(d_misc), rlc->t0, T, d_rg1, d_rq, reinterpret_cast<int32_t*>(d_misc + 32), sa);
+    B200_CUDA_TRY(cudaMemcpyAsync(d_rg1 + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
+    if (s.trace) cudaEventRecord(s.ev_t[3], sa);
+    Fp12* fbuf[2] = {static_cast<Fp12*>(s.rlc_fa.p), static_cast<Fp12*>(s.rlc_fb.p)};
+    G2Jac* qbuf[2] = {static_cast<G2Jac*>(s.rlc_qa.p), static_cast<G2Jac*>(s.rlc_qb.p)};
+    // S = sum_t r_t sig_t first (warp-shuffle folds T -> T/32 -> ... -> 1): its pair (-g1, S) then rides in the SAME
+    // Miller launch as the T tuple pairs instead of costing a second, latency-bound launch of one team
+    const G2Jac* qi = d_rq;
+    uint32_t n_cur = T;
+    int pp = 0;
+    do {
+        n_cur = launch_rlc_reduce(nullptr, qi, n_cur, nullptr, qbuf[pp], sa);
+        e.launches++;
+        qi = qbuf[pp]; pp ^= 1;
+    } while (n_cur > 1);
+    launch_rlc_finish(qi, d_g2 + n_g2, sa);
+    // T + 1 Miller loops on the lane-parallel VM: (r_t agg_t, H_t) for every tuple and (-g1, S)
+    launch_vm_miller(d_rg1, d_idx, d_g2, d_idx + T + 1, d_zero, reinterpret_cast<const int32_t*>(d_zero), d_zero,
+                     reinterpret_cast<const int32_t*>(d_zero), T + 1, static_cast<Fp12*>(s.f.p), sa);
+    // Gt product of the T + 1 Miller values, again by warp-shuffle folds
+    const Fp12* fi = static_cast<const Fp12*>(s.f.p);
+    n_cur = T + 1;
+    pp = 0;
+    do {
+        n_cur = launch_rlc_reduce(fi, nullptr, n_cur, fbuf[pp], nullptr, sa);
+        e.launches++;
+        fi = fbuf[pp]; pp ^= 1;
+    } while (n_cur > 1);
+    if (rlc->exchange && rlc_world > 1) {
+        // the path's one exchange step: e(-g1, sum over ranks) = product over ranks, so every rank has already paired
+        // its own partial sum and only the Gt partial (576 B) and the bad flag travel; then the same fold on all ranks
+        uint8_t* x = static_cast<uint8_t*>(s.rlc_xch.p);
+        B200_CUDA_TRY(cudaMemcpyAsync(x, fi, sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
+        B200_CUDA_TRY(cudaMemcpyAsync(x + sizeof(Fp12) + sizeof(G2Jac), d_misc + 32, 16, cudaMemcpyDeviceToDevice, sa));
+        int32_t rcx = comm_all_gather(e, x, x + kPart, kPart, sa);
+        if (rcx) return rcx;
+        for (uint32_t r = 0; r < rlc_world; r++)   // unpack into the fold's input array (world <= a few dozen)
+            B200_CUDA_TRY(cudaMemcpyAsync(fbuf[pp] + r, x + kPart * (1 + r), sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
+        B200_CUDA_TRY(cudaMemcpyAsync(h_x, x + kPart, size_t(rlc_world) * kPart, cudaMemcpyDeviceToHost, sa));   // for the ranks' bad flags
+        fi = fbuf[pp]; pp ^= 1;
+        n_cur = rlc_world;
         do {
             n_cur = launch_rlc_reduce(fi, nullptr, n_cur, fbuf[pp], nullptr, sa);
             e.launches++;
             fi = fbuf[pp]; pp ^= 1;
         } while (n_cur > 1);
-        if (rlc->exchange && rlc_world > 1) {
-            // the path's one exchange step: e(-g1, sum over ranks) = product over ranks, so every rank has already paired
-            // its own partial sum and only the Gt partial (576 B) and the bad flag travel; then the same fold on all ranks
-            uint8_t* x = static_cast<uint8_t*>(s.rlc_xch.p);
-            B200_CUDA_TRY(cudaMemcpyAsync(x, fi, sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
-            B200_CUDA_TRY(cudaMemcpyAsync(x + sizeof(Fp12) + sizeof(G2Jac), d_misc + 32, 16, cudaMemcpyDeviceToDevice, sa));
-            int32_t rcx = comm_all_gather(e, x, x + kPart, kPart, sa);
-            if (rcx) return rcx;
-            for (uint32_t r = 0; r < rlc_world; r++)   // unpack into the fold's input array (world <= a few dozen)
-                B200_CUDA_TRY(cudaMemcpyAsync(fbuf[pp] + r, x + kPart * (1 + r), sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
-            B200_CUDA_TRY(cudaMemcpyAsync(h_x, x + kPart, size_t(rlc_world) * kPart, cudaMemcpyDeviceToHost, sa));   // for the ranks' bad flags
-            fi = fbuf[pp]; pp ^= 1;
-            n_cur = rlc_world;
-            do {
-                n_cur = launch_rlc_reduce(fi, nullptr, n_cur, fbuf[pp], nullptr, sa);
-                e.launches++;
-                fi = fbuf[pp]; pp ^= 1;
-            } while (n_cur > 1);
-        }
-        // the single final exponentiation: (Gt product) * 1
-        Fp12* d_fin = fbuf[pp];
-        B200_CUDA_TRY(cudaMemcpyAsync(d_fin, fi, sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
-        launch_fp12_one(d_fin + 1, sa);
-        launch_vm_final(d_fin, d_zero, reinterpret_cast<const int32_t*>(d_zero), d_zero, reinterpret_cast<const int32_t*>(d_zero), 1,
-                        reinterpret_cast<int32_t*>(d_misc + 64), sa);
-        e.launches += 5;
-        B200_CUDA_TRY(cudaEventRecord(s.ev_k1, sa));
-        B200_CUDA_TRY(cudaGetLastError());
-        B200_CUDA_TRY(cudaMemcpyAsync(h_out, d_misc + 32, 64, cudaMemcpyDeviceToHost, sa));   // [0] bad, [8] final code
-        B200_CUDA_TRY(cudaStreamSynchronize(sa));
-        B200_CUDA_TRY(cudaStreamSynchronize(sb));
-        B200_CUDA_TRY(cudaStreamSynchronize(sc));
-        B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, s.ev_k0, s.ev_k1));
-        B200_CUDA_TRY(cudaEventElapsedTime(&s.last_dominant_ms, s.ev_d0, s.ev_d1));
-        bool bad = h_out[0] != 0;
-        if (rlc->exchange && rlc_world > 1)
-            for (uint32_t r = 0; r < rlc_world; r++) {
-                int32_t flag;
-                memcpy(&flag, h_x + size_t(r) * kPart + sizeof(Fp12) + sizeof(G2Jac), 4);
-                bad = bad || flag != 0;
-            }
-        rlc->all_ok = (!bad && h_out[8] == BLS_SUCCESS) ? 1 : 0;
-        if (s.trace) {
-            float a = 0, g2 = 0;
-            cudaEventElapsedTime(&a, s.ev_t[2], s.ev_k1); cudaEventElapsedTime(&g2, s.ev_k0, s.ev_k1);
-            fprintf(stderr, "[b200 bls rlc] K1 %.2f | scale + T Miller loops + folds + 1 final exponentiation %.2f | total %.2f ms\n",
-                    s.last_dominant_ms, a, g2);
-        }
-        return B200_SUCCESS;
     }
-    if (chunked) {
-        // every range's Miller loops and final exponentiations are already queued on stream D (joined above)
-    } else if (mode == MODE_FAST_AGGREGATE && s.use_vm) {
-        launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, static_cast<const int32_t*>(s.pk_code.p),
-                         static_cast<const uint32_t*>(s.flags.p), static_cast<const int32_t*>(s.sig_code.p), n_pairs,
-                         static_cast<Fp12*>(s.f.p), sa);
-        if (s.trace) cudaEventRecord(s.ev_t[3], sa);
-        launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff, static_cast<const int32_t*>(s.pk_code.p),
-                        static_cast<const uint32_t*>(s.flags.p), static_cast<const int32_t*>(s.sig_code.p), T,
-                        static_cast<int32_t*>(s.out.p), sa);
-    } else {
-        launch_miller(pair_g1, d_g1i, d_g2, d_g2i, d_ptu, static_cast<const int32_t*>(s.pk_code.p),
-                      static_cast<const uint32_t*>(s.flags.p), static_cast<const int32_t*>(s.sig_code.p), n_pairs,
-                      static_cast<Fp12*>(s.f.p), sa);
-        launch_final(static_cast<const Fp12*>(s.f.p), d_poff, static_cast<const int32_t*>(s.pk_code.p),
-                     static_cast<const uint32_t*>(s.flags.p), static_cast<const int32_t*>(s.sig_code.p), T,
-                     static_cast<int32_t*>(s.out.p), sa);
-    }
-    if (!chunked) e.launches += (n_pairs ? 1 : 0) + (T ? 1 : 0);
-    B200_CUDA_TRY(cudaEventRecord(s.ev_k1, sa));
-    B200_CUDA_TRY(cudaGetLastError());
-    B200_CUDA_TRY(cudaMemcpyAsync(h_out + 4, s.out.p, size_t(T) * 4, cudaMemcpyDeviceToHost, sa));
-    B200_CUDA_TRY(cudaStreamSynchronize(sa));
-    B200_CUDA_TRY(cudaStreamSynchronize(sb));
-    B200_CUDA_TRY(cudaStreamSynchronize(sc));
-    if (chunked) B200_CUDA_TRY(cudaStreamSynchronize(s.sd));
-    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, s.ev_k0, s.ev_k1));
-    B200_CUDA_TRY(cudaEventElapsedTime(&s.last_dominant_ms, s.ev_d0, s.ev_d1));
+    // the single final exponentiation: (Gt product) * 1
+    Fp12* d_fin = fbuf[pp];
+    B200_CUDA_TRY(cudaMemcpyAsync(d_fin, fi, sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
+    launch_fp12_one(d_fin + 1, sa);
+    launch_vm_final(d_fin, d_zero, reinterpret_cast<const int32_t*>(d_zero), d_zero, reinterpret_cast<const int32_t*>(d_zero), 1,
+                    reinterpret_cast<int32_t*>(d_misc + 64), sa);
+    e.launches += 5;
+    int32_t rc = readback(h_out, d_misc + 32, 64);   // [0] bad, [8] final code
+    if (rc) return rc;
+    bool bad = h_out[0] != 0;
+    if (rlc->exchange && rlc_world > 1)
+        for (uint32_t r = 0; r < rlc_world; r++) {
+            int32_t flag;
+            memcpy(&flag, h_x + size_t(r) * kPart + sizeof(Fp12) + sizeof(G2Jac), 4);
+            bad = bad || flag != 0;
+        }
+    rlc->all_ok = (!bad && h_out[8] == BLS_SUCCESS) ? 1 : 0;
     if (s.trace) {
-        float a = 0, b = 0, c = 0, d = 0, f2 = 0, g2 = 0;
-        cudaEventElapsedTime(&a, s.ev_k0, s.ev_d0); cudaEventElapsedTime(&b, s.ev_t[0], s.ev_t[1]);
-        cudaEventElapsedTime(&c, s.ev_t[1], s.ev_t[2]); cudaEventElapsedTime(&d, s.ev_t[2], s.ev_t[3]);
-        cudaEventElapsedTime(&f2, s.ev_t[3], s.ev_k1); cudaEventElapsedTime(&g2, s.ev_k0, s.ev_k1);
-        fprintf(stderr, "[b200 bls] pre-K1 %.2f | K1 %.2f | K2 %.2f | wait(streamB) %.2f | miller %.2f | final %.2f | total %.2f ms\n",
-                a, s.last_dominant_ms, b, c, d, f2, g2);
+        float a = 0, g2 = 0;
+        cudaEventElapsedTime(&a, s.ev_t[2], s.ev_k1); cudaEventElapsedTime(&g2, s.ev_k0, s.ev_k1);
+        fprintf(stderr, "[b200 bls rlc] K1 %.2f | scale + T Miller loops + folds + 1 final exponentiation %.2f | total %.2f ms\n",
+                s.last_dominant_ms, a, g2);
     }
-    for (uint32_t t = 0; t < T; t++) out_codes[t] = h_out[4 + t];
+    return B200_SUCCESS;
+}
+
+// An early error return must not leave work queued on the side streams (they read the caller's host buffers and the
+// engine's grow-only device buffers): drain all of them before handing the error back.
+static int32_t run_verify(Engine& e, BlsState& s, const Batch& b, int32_t* out_codes) {
+    const int32_t rc = VerifyRun{e, s, b}.run(out_codes);
+    if (rc != B200_SUCCESS) {
+        cudaStreamSynchronize(e.stream);
+        cudaStreamSynchronize(s.sb);
+        cudaStreamSynchronize(s.sc);
+        cudaStreamSynchronize(s.sd);
+        cudaStreamSynchronize(s.se);
+        cudaGetLastError();
+    }
+    return rc;
+}
+
+// ---- argument checks and set-up shared by the batch entry points
+
+// T + 1 non-decreasing offsets; *count: the last one (keys, or registry indices, of the batch)
+static int32_t check_offsets(const uint32_t* off, size_t n_tuples, uint32_t* count) {
+    for (size_t t = 0; t < n_tuples; t++)
+        if (off[t] > off[t + 1]) return B200_ERR_BAD_ARG;
+    *count = off[n_tuples];
+    return B200_SUCCESS;
+}
+
+// offsets of T 32-byte messages
+static std::vector<uint32_t> msg32_offsets(size_t n_tuples) {
+    std::vector<uint32_t> moff(n_tuples + 1);
+    for (size_t t = 0; t <= n_tuples; t++) moff[t] = uint32_t(32 * t);
+    return moff;
+}
+
+// contiguous block of tuples per rank, balanced to within one (parallel.tuple_shard in the Python mirror)
+struct TupleRange {
+    size_t lo, cnt;
+};
+static TupleRange tuple_shard(size_t n_tuples, size_t world, size_t rank) {
+    const size_t base = n_tuples / world, rem = n_tuples % world;
+    return {rank * base + std::min(rank, rem), base + (rank < rem ? 1 : 0)};
+}
+
+// the rank's block of a strict batch as a batch of its own; koff / moff receive its rebased key and message offsets
+static Batch shard_batch(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs32, const uint8_t* sigs, TupleRange r,
+                         std::vector<uint32_t>& koff, std::vector<uint32_t>& moff) {
+    koff.resize(r.cnt + 1);
+    for (size_t t = 0; t <= r.cnt; t++) koff[t] = pk_offsets[r.lo + t] - pk_offsets[r.lo];
+    moff = msg32_offsets(r.cnt);
+    return {.keys = pks_flat ? pks_flat + size_t(pk_offsets[r.lo]) * 48 : nullptr, .n_keys = koff[r.cnt], .key_off = koff.data(),
+            .msgs = msgs32 + 32 * r.lo, .msg_off = moff.data(), .n_msgs = uint32_t(r.cnt), .sigs = sigs + 96 * r.lo, .T = uint32_t(r.cnt)};
+}
+
+// every validator index names a resident registry key or one of the call's n_extra extra keys
+static int32_t check_indices(Engine& e, const BlsState& s, const uint32_t* index, uint32_t n, size_t n_extra) {
+    for (uint32_t i = 0; i < n; i++)
+        if (index[i] >= s.reg_n + n_extra) {
+            e.last_error = n_extra ? "validator index outside the loaded registry (+ extra keys)" : "validator index outside the loaded registry";
+            return B200_ERR_BAD_ARG;
+        }
+    return B200_SUCCESS;
+}
+
+static void rlc_seed(const uint8_t* seed32, uint8_t out[32]) {
+    if (seed32) { memcpy(out, seed32, 32); return; }
+    std::random_device rd;   // the scalars must be unpredictable to whoever produced the signatures
+    for (int i = 0; i < 8; i++) { const uint32_t v = rd(); memcpy(out + 4 * i, &v, 4); }
+}
+
+// the whole-batch entry points after their checks: `b` as one RLC check, scalars from the caller's seed (or one from the OS)
+static int32_t verify_all(Engine& e, BlsState& s, Batch b, const uint8_t* seed32, uint64_t t0, bool exchange, int32_t* all_ok) {
+    uint8_t seed[32];
+    rlc_seed(seed32, seed);
+    RlcReq req{seed, t0, exchange, 0};
+    b.rlc = &req;
+    const int32_t rc = run_verify(e, s, b, nullptr);
+    if (rc) return rc;
+    *all_ok = req.all_ok;
     return B200_SUCCESS;
 }
 
@@ -541,6 +679,7 @@ using namespace b200;
 
 extern "C" {
 
+// Knobs are the rows of kKnobs; an environment value takes the same rule as b200_tune's (see the header).
 int32_t b200_tune(const char* knob, int64_t value) {
     Engine& e = engine();
     Guard g(e);
@@ -550,18 +689,9 @@ int32_t b200_tune(const char* knob, int64_t value) {
     rc = bls_state(e, &s);
     if (rc) return rc;
     if (!knob) return B200_ERR_BAD_ARG;
-    const std::string k(knob);
-    if (k == "bls_chunks") s->chunks = uint32_t(std::max<int64_t>(1, value));
-    else if (k == "bls_chunk_min_tuples") s->chunk_min_tuples = uint32_t(std::max<int64_t>(2, value));
-    else if (k == "bls_chunk_k1_cta") s->chunk_k1_cta = int(value);
-    else if (k == "bls_chunk_alt") s->chunk_alt = value != 0;
-    else if (k == "bls_key_split") s->key_split = value != 0;
-    else if (k == "bls_k1_first_cta") s->k1_first_cta = (value == 128) ? 128 : 384;
-    else if (k == "bls_small_cta") s->small_cta_override = int(value);
-    else if (k == "vm_team16_max") set_vm_team16_max(uint32_t(std::max<int64_t>(0, value)));
-    else if (k == "vm_cta") set_vm_cta(int(value));
-    else return B200_ERR_BAD_ARG;
-    return B200_SUCCESS;
+    for (const Knob& k : kKnobs)
+        if (strcmp(k.name, knob) == 0) { k.set(*s, value); return B200_SUCCESS; }
+    return B200_ERR_BAD_ARG;
 }
 
 int32_t b200_vm_load_programs(const uint32_t* blob, size_t n_words) {
@@ -636,17 +766,15 @@ int32_t b200_fast_aggregate_verify_batch(const uint8_t* pks_flat, const uint32_t
     if (rc) return rc;
     if (n_tuples == 0) return B200_SUCCESS;
     if (!pk_offsets || !msgs32 || !sigs || !out_codes || n_tuples > kMaxBatchTuples) return B200_ERR_BAD_ARG;
-    for (size_t t = 0; t < n_tuples; t++)
-        if (pk_offsets[t] > pk_offsets[t + 1]) return B200_ERR_BAD_ARG;
-    const uint32_t nk = pk_offsets[n_tuples];
+    uint32_t nk;
+    if ((rc = check_offsets(pk_offsets, n_tuples, &nk))) return rc;
     if (nk && !pks_flat) return B200_ERR_BAD_ARG;
     BlsState* s;
     rc = bls_state(e, &s);
     if (rc) return rc;
-    std::vector<uint32_t> moff(n_tuples + 1);
-    for (size_t t = 0; t <= n_tuples; t++) moff[t] = uint32_t(32 * t);
-    return run_verify(e, *s, MODE_FAST_AGGREGATE, pks_flat, nk, nullptr, 0, pk_offsets, msgs32, moff.data(),
-                      uint32_t(n_tuples), sigs, uint32_t(n_tuples), false, out_codes);
+    const std::vector<uint32_t> moff = msg32_offsets(n_tuples);
+    return run_verify(e, *s, {.keys = pks_flat, .n_keys = nk, .key_off = pk_offsets, .msgs = msgs32, .msg_off = moff.data(),
+                              .n_msgs = uint32_t(n_tuples), .sigs = sigs, .T = uint32_t(n_tuples)}, out_codes);
 }
 
 // BASELINE configs[4]: the batch sharded over the communicator's ranks; verdicts exchanged with one ncclAllGather.
@@ -660,31 +788,26 @@ int32_t b200_fast_aggregate_verify_batch_sharded(const uint8_t* pks_flat, const 
     if (!c.ready) { e.last_error = "b200_comm_init has not been called"; return B200_ERR_NOT_INITIALIZED; }
     if (n_tuples == 0) return B200_SUCCESS;
     if (!pk_offsets || !msgs32 || !sigs || !out_codes || n_tuples > kMaxBatchTuples) return B200_ERR_BAD_ARG;
-    for (size_t t = 0; t < n_tuples; t++)
-        if (pk_offsets[t] > pk_offsets[t + 1]) return B200_ERR_BAD_ARG;
-    if (pk_offsets[n_tuples] && !pks_flat) return B200_ERR_BAD_ARG;
+    uint32_t nk;
+    if ((rc = check_offsets(pk_offsets, n_tuples, &nk))) return rc;
+    if (nk && !pks_flat) return B200_ERR_BAD_ARG;
     BlsState* s;
     rc = bls_state(e, &s);
     if (rc) return rc;
-    // contiguous block of tuples per rank, balanced to within one (parallel.tuple_shard in the Python mirror)
-    const size_t world = size_t(c.world), rank = size_t(c.rank);
-    const size_t base = n_tuples / world, rem = n_tuples % world;
-    const size_t lo = rank * base + std::min(rank, rem), cnt = base + (rank < rem ? 1 : 0);
-    const size_t per = base + (rem ? 1 : 0);  // padded shard length: equal contributions to the all-gather
+    const size_t world = size_t(c.world);
+    const TupleRange mine = tuple_shard(n_tuples, world, size_t(c.rank));
+    const size_t per = (n_tuples + world - 1) / world;  // padded shard length: equal contributions to the all-gather
     B200_CUDA_TRY(s->out.reserve((per + 1) * 4));
     B200_CUDA_TRY(s->gath.reserve(world * per * 4 + 16));
-    if (cnt) {
-        std::vector<uint32_t> koff(cnt + 1), moff(cnt + 1);
-        for (size_t t = 0; t <= cnt; t++) { koff[t] = pk_offsets[lo + t] - pk_offsets[lo]; moff[t] = uint32_t(32 * t); }
-        std::vector<int32_t> local(cnt);
-        rc = run_verify(e, *s, MODE_FAST_AGGREGATE, pks_flat ? pks_flat + size_t(pk_offsets[lo]) * 48 : nullptr, koff[cnt], nullptr, 0,
-                        koff.data(), msgs32 + 32 * lo, moff.data(), uint32_t(cnt), sigs + 96 * lo, uint32_t(cnt), false,
-                        local.data());
+    if (mine.cnt) {
+        std::vector<uint32_t> koff, moff;
+        std::vector<int32_t> local(mine.cnt);
+        rc = run_verify(e, *s, shard_batch(pks_flat, pk_offsets, msgs32, sigs, mine, koff, moff), local.data());
         if (rc) return rc;
     }
     cudaStream_t sa = e.stream;
     int32_t* d_out = static_cast<int32_t*>(s->out.p);
-    if (per > cnt) B200_CUDA_TRY(cudaMemsetAsync(d_out + cnt, 0xff, (per - cnt) * 4, sa));
+    if (per > mine.cnt) B200_CUDA_TRY(cudaMemsetAsync(d_out + mine.cnt, 0xff, (per - mine.cnt) * 4, sa));
     rc = comm_all_gather(e, d_out, s->gath.p, per * 4, sa);   // the path's one exchange step
     if (rc) return rc;
     B200_CUDA_TRY(s->stage.reserve(world * per * 4 + 64));
@@ -692,19 +815,13 @@ int32_t b200_fast_aggregate_verify_batch_sharded(const uint8_t* pks_flat, const 
     B200_CUDA_TRY(cudaStreamSynchronize(sa));
     const int32_t* h = static_cast<const int32_t*>(s->stage.p);
     for (size_t r = 0; r < world; r++) {
-        const size_t rlo = r * base + std::min(r, rem), rcnt = base + (r < rem ? 1 : 0);
-        memcpy(out_codes + rlo, h + r * per, rcnt * 4);
+        const TupleRange theirs = tuple_shard(n_tuples, world, r);
+        memcpy(out_codes + theirs.lo, h + r * per, theirs.cnt * 4);
     }
     return B200_SUCCESS;
 }
 
 // ---- RLC whole-batch entry points (bls_rlc.cu) --------------------------------------------------------------------
-static void rlc_seed(const uint8_t* seed32, uint8_t out[32]) {
-    if (seed32) { memcpy(out, seed32, 32); return; }
-    std::random_device rd;   // the scalars must be unpredictable to whoever produced the signatures
-    for (int i = 0; i < 8; i++) { const uint32_t v = rd(); memcpy(out + 4 * i, &v, 4); }
-}
-
 int32_t b200_fast_aggregate_verify_batch_all(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs32,
                                              const uint8_t* sigs, size_t n_tuples, const uint8_t* seed32, int32_t* all_ok) {
     Engine& e = engine();
@@ -714,23 +831,15 @@ int32_t b200_fast_aggregate_verify_batch_all(const uint8_t* pks_flat, const uint
     if (!all_ok) return B200_ERR_BAD_ARG;
     if (n_tuples == 0) { *all_ok = 1; return B200_SUCCESS; }
     if (!pk_offsets || !msgs32 || !sigs || n_tuples > kMaxBatchTuples) return B200_ERR_BAD_ARG;
-    for (size_t t = 0; t < n_tuples; t++)
-        if (pk_offsets[t] > pk_offsets[t + 1]) return B200_ERR_BAD_ARG;
-    const uint32_t nk = pk_offsets[n_tuples];
+    uint32_t nk;
+    if ((rc = check_offsets(pk_offsets, n_tuples, &nk))) return rc;
     if (nk && !pks_flat) return B200_ERR_BAD_ARG;
     BlsState* s;
     rc = bls_state(e, &s);
     if (rc) return rc;
-    std::vector<uint32_t> moff(n_tuples + 1);
-    for (size_t t = 0; t <= n_tuples; t++) moff[t] = uint32_t(32 * t);
-    uint8_t seed[32];
-    rlc_seed(seed32, seed);
-    RlcReq req{seed, 0, false, 0};
-    rc = run_verify(e, *s, MODE_FAST_AGGREGATE, pks_flat, nk, nullptr, 0, pk_offsets, msgs32, moff.data(), uint32_t(n_tuples), sigs,
-                    uint32_t(n_tuples), false, nullptr, &req);
-    if (rc) return rc;
-    *all_ok = req.all_ok;
-    return B200_SUCCESS;
+    const std::vector<uint32_t> moff = msg32_offsets(n_tuples);
+    return verify_all(e, *s, {.keys = pks_flat, .n_keys = nk, .key_off = pk_offsets, .msgs = msgs32, .msg_off = moff.data(),
+                              .n_msgs = uint32_t(n_tuples), .sigs = sigs, .T = uint32_t(n_tuples)}, seed32, 0, false, all_ok);
 }
 
 int32_t b200_fast_aggregate_verify_batch_indexed_all(const uint32_t* indices, const uint32_t* offsets, const uint8_t* msgs32,
@@ -745,23 +854,14 @@ int32_t b200_fast_aggregate_verify_batch_indexed_all(const uint32_t* indices, co
     BlsState* s;
     rc = bls_state(e, &s);
     if (rc) return rc;
-    for (size_t t = 0; t < n_tuples; t++)
-        if (offsets[t] > offsets[t + 1]) return B200_ERR_BAD_ARG;
-    const uint32_t ni = offsets[n_tuples];
+    uint32_t ni;
+    if ((rc = check_offsets(offsets, n_tuples, &ni))) return rc;
     if (ni && !indices) return B200_ERR_BAD_ARG;
-    for (uint32_t i = 0; i < ni; i++)
-        if (indices[i] >= s->reg_n) { e.last_error = "validator index outside the loaded registry"; return B200_ERR_BAD_ARG; }
-    std::vector<uint32_t> moff(n_tuples + 1);
-    for (size_t t = 0; t <= n_tuples; t++) moff[t] = uint32_t(32 * t);
+    if ((rc = check_indices(e, *s, indices, ni, 0))) return rc;
+    const std::vector<uint32_t> moff = msg32_offsets(n_tuples);
     static const uint32_t dummy = 0;
-    uint8_t seed[32];
-    rlc_seed(seed32, seed);
-    RlcReq req{seed, 0, false, 0};
-    rc = run_verify(e, *s, MODE_FAST_AGGREGATE, nullptr, 0, indices ? indices : &dummy, ni, offsets, msgs32, moff.data(),
-                    uint32_t(n_tuples), sigs, uint32_t(n_tuples), false, nullptr, &req);
-    if (rc) return rc;
-    *all_ok = req.all_ok;
-    return B200_SUCCESS;
+    return verify_all(e, *s, {.index = indices ? indices : &dummy, .n_index = ni, .key_off = offsets, .msgs = msgs32, .msg_off = moff.data(),
+                              .n_msgs = uint32_t(n_tuples), .sigs = sigs, .T = uint32_t(n_tuples)}, seed32, 0, false, all_ok);
 }
 
 // every rank passes the same batch AND the same seed; each verifies its block, the (Gt, G2) partials are all-gathered and
@@ -778,23 +878,15 @@ int32_t b200_fast_aggregate_verify_batch_all_sharded(const uint8_t* pks_flat, co
     if (n_tuples == 0) { *all_ok = 1; return B200_SUCCESS; }
     if (!pk_offsets || !msgs32 || !sigs || n_tuples > kMaxBatchTuples) return B200_ERR_BAD_ARG;
     if (n_tuples < size_t(c.world)) { e.last_error = "fewer tuples than ranks"; return B200_ERR_BAD_ARG; }
-    for (size_t t = 0; t < n_tuples; t++)
-        if (pk_offsets[t] > pk_offsets[t + 1]) return B200_ERR_BAD_ARG;
-    if (pk_offsets[n_tuples] && !pks_flat) return B200_ERR_BAD_ARG;
+    uint32_t nk;
+    if ((rc = check_offsets(pk_offsets, n_tuples, &nk))) return rc;
+    if (nk && !pks_flat) return B200_ERR_BAD_ARG;
     BlsState* s;
     rc = bls_state(e, &s);
     if (rc) return rc;
-    const size_t world = size_t(c.world), rank = size_t(c.rank);
-    const size_t base = n_tuples / world, rem = n_tuples % world;
-    const size_t lo = rank * base + std::min(rank, rem), cnt = base + (rank < rem ? 1 : 0);
-    std::vector<uint32_t> koff(cnt + 1), moff(cnt + 1);
-    for (size_t t = 0; t <= cnt; t++) { koff[t] = pk_offsets[lo + t] - pk_offsets[lo]; moff[t] = uint32_t(32 * t); }
-    RlcReq req{seed32, uint64_t(lo), true, 0};
-    rc = run_verify(e, *s, MODE_FAST_AGGREGATE, pks_flat ? pks_flat + size_t(pk_offsets[lo]) * 48 : nullptr, koff[cnt], nullptr, 0,
-                    koff.data(), msgs32 + 32 * lo, moff.data(), uint32_t(cnt), sigs + 96 * lo, uint32_t(cnt), false, nullptr, &req);
-    if (rc) return rc;
-    *all_ok = req.all_ok;
-    return B200_SUCCESS;
+    const TupleRange mine = tuple_shard(n_tuples, size_t(c.world), size_t(c.rank));
+    std::vector<uint32_t> koff, moff;
+    return verify_all(e, *s, shard_batch(pks_flat, pk_offsets, msgs32, sigs, mine, koff, moff), seed32, uint64_t(mine.lo), true, all_ok);
 }
 
 int32_t b200_registry_load(const uint8_t* pks_flat, size_t n) {
@@ -849,17 +941,15 @@ static int32_t verify_batch_indexed(const uint8_t* extra_pks, size_t n_extra, co
     rc = bls_state(e, &s);
     if (rc) return rc;
     if (n_extra && !s->reg_aff.p) { e.last_error = "no registry loaded"; return B200_ERR_BAD_ARG; }
-    for (size_t t = 0; t < n_tuples; t++)
-        if (offsets[t] > offsets[t + 1]) return B200_ERR_BAD_ARG;
-    const uint32_t ni = offsets[n_tuples];
+    uint32_t ni;
+    if ((rc = check_offsets(offsets, n_tuples, &ni))) return rc;
     if (ni && !indices) return B200_ERR_BAD_ARG;
-    for (uint32_t i = 0; i < ni; i++)
-        if (indices[i] >= s->reg_n + n_extra) { e.last_error = "validator index outside the loaded registry (+ extra keys)"; return B200_ERR_BAD_ARG; }
-    std::vector<uint32_t> moff(n_tuples + 1);
-    for (size_t t = 0; t <= n_tuples; t++) moff[t] = uint32_t(32 * t);
+    if ((rc = check_indices(e, *s, indices, ni, n_extra))) return rc;
+    const std::vector<uint32_t> moff = msg32_offsets(n_tuples);
     static const uint32_t dummy = 0;
-    return run_verify(e, *s, MODE_FAST_AGGREGATE, n_extra ? extra_pks : nullptr, uint32_t(n_extra), indices ? indices : &dummy, ni, offsets,
-                      msgs32, moff.data(), uint32_t(n_tuples), sigs, uint32_t(n_tuples), false, out_codes);
+    return run_verify(e, *s, {.keys = n_extra ? extra_pks : nullptr, .n_keys = uint32_t(n_extra), .index = indices ? indices : &dummy,
+                              .n_index = ni, .key_off = offsets, .msgs = msgs32, .msg_off = moff.data(), .n_msgs = uint32_t(n_tuples),
+                              .sigs = sigs, .T = uint32_t(n_tuples)}, out_codes);
 }
 
 int32_t b200_fast_aggregate_verify_batch_indexed(const uint32_t* indices, const uint32_t* offsets, const uint8_t* msgs32,
@@ -888,7 +978,8 @@ int32_t b200_fast_aggregate_verify(const uint8_t* const* pks, size_t k, const ui
     for (size_t i = 0; i < k; i++) memcpy(flat.data() + 48 * i, pks[i], 48);
     const uint32_t koff[2] = {0, uint32_t(k)}, moff[2] = {0, uint32_t(msg_len)};
     int32_t code = B200_ERR_CUDA;
-    rc = run_verify(e, *s, MODE_FAST_AGGREGATE, flat.data(), uint32_t(k), nullptr, 0, koff, msg, moff, 1, sig, 1, false, &code);
+    rc = run_verify(e, *s, {.keys = flat.data(), .n_keys = uint32_t(k), .key_off = koff, .msgs = msg, .msg_off = moff, .n_msgs = 1,
+                            .sigs = sig, .T = 1}, &code);
     return rc ? rc : code;
 }
 
@@ -937,8 +1028,8 @@ int32_t b200_aggregate_verify(const uint8_t* pks_flat, size_t n_pks, const uint8
         }
     }
     int32_t code = B200_ERR_CUDA;
-    rc = run_verify(e, *s, MODE_AGGREGATE, pks_flat, uint32_t(n_pks), nullptr, 0, nullptr, flat.data(), moff.data(),
-                    uint32_t(moff.size() - 1), sig, 1, shape_fail, &code);
+    rc = run_verify(e, *s, {.mode = MODE_AGGREGATE, .keys = pks_flat, .n_keys = uint32_t(n_pks), .msgs = flat.data(), .msg_off = moff.data(),
+                            .n_msgs = uint32_t(moff.size() - 1), .sigs = sig, .T = 1, .force_fail_shape = shape_fail}, &code);
     return rc ? rc : code;
 }
 

@@ -44,18 +44,6 @@ __global__ void k_sha256_bytes(const uint8_t* data, size_t len, uint32_t* out_wo
     for (int i = 0; i < 8; i++) out_words[i] = st[i];
 }
 
-struct Guard {
-    std::unique_lock<std::mutex> lk;
-    explicit Guard(Engine& e) : lk(e.mu) {}
-};
-
-int32_t check_ready(Engine& e) {
-    if (!e.ready) { e.last_error = "b200_init has not been called (or failed)"; return B200_ERR_NOT_INITIALIZED; }
-    cudaError_t ce = cudaSetDevice(e.device);
-    if (ce != cudaSuccess) { e.last_error = cudaGetErrorString(ce); return B200_ERR_CUDA; }
-    return B200_SUCCESS;
-}
-
 int32_t run_oneshot(Engine& e, SszPlan& plan, const std::vector<uint32_t>& outputs, uint8_t* out) {
     return plan.run(e, e.arena, e.fields, e.planbuf, COPY_ALL, outputs, out);
 }

@@ -66,6 +66,20 @@ struct Engine {
 
 Engine& engine();
 
+// Every entry point holds the engine lock for the whole call.
+struct Guard {
+    std::unique_lock<std::mutex> lk;
+    explicit Guard(Engine& e) : lk(e.mu) {}
+};
+
+// B200_SUCCESS when b200_init succeeded; binds the calling thread to the engine's device
+inline int32_t check_ready(Engine& e) {
+    if (!e.ready) { e.last_error = "b200_init has not been called (or failed)"; return B200_ERR_NOT_INITIALIZED; }
+    cudaError_t ce = cudaSetDevice(e.device);
+    if (ce != cudaSuccess) { e.last_error = cudaGetErrorString(ce); return B200_ERR_CUDA; }
+    return B200_SUCCESS;
+}
+
 #define B200_CUDA_TRY(expr)                                                                   \
     do {                                                                                      \
         cudaError_t e__ = (expr);                                                             \

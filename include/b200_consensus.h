@@ -253,6 +253,8 @@ B200_API int32_t b200_measure_int_peak(int32_t kind, double* gops);
  *   of their keys under the first waves of the per-key kernel), "bls_k1_first_cta" (128 | 384: CTA size of those first waves),
  *   "bls_small_cta" (0 = by batch size | 32 | 64 | 128: CTA size of the signature / message kernels), "vm_team16_max",
  *   "vm_cta" (32 | 64 | 128).
+ * An environment value goes through the same rule as the value passed here: B200_BLS_K1_FIRST_CTA other than 128 means 384,
+ * a negative B200_VM_TEAM16_MAX means 0, and B200_BLS_SMALL_CTA is the only name of that knob.
  * Unknown knob -> B200_ERR_BAD_ARG. */
 B200_API int32_t b200_tune(const char* knob, int64_t value);
 /* Replaces the scheduled Miller-loop / final-exponentiation programs of one team size (8 or 16 lanes) of the lane-parallel

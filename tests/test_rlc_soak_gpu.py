@@ -1,4 +1,4 @@
-"""GPU: the RLC whole-batch check (bls_rlc.cu and the RLC branch of capi_bls.cu run_verify_impl) against its exact
+"""GPU: the RLC whole-batch check (bls_rlc.cu and the rlc_tail phase of capi_bls.cu) against its exact
 exponent model (tests/rlc_soak_cases.py), case by case, through every entry point.
 
 a. family A: every tuple invalid, defects cancelling under one seed: True under that seed, False under every other seed,
