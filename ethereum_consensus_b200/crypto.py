@@ -44,6 +44,7 @@ _lib.register_protos({
     "b200_last_dominant_kernel_ms": (C.c_float, []),
     "b200_fp_selftest": (C.c_int32, [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]),
     "b200_fp_eval": (C.c_int32, [C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200_curve_eval": (C.c_int32, [C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_measure_int_peak": (C.c_int32, [C.c_int32, C.POINTER(C.c_double)]),
 })
 
@@ -290,6 +291,26 @@ def fp_eval(op: str, a, b=None) -> np.ndarray:
         raise ValueError("operands must be uint32[n, 24]")
     out = np.zeros((max(a.shape[0], 1), 25), dtype=np.uint32)
     _lib.check(_lib.lib().b200_fp_eval(FP_EVAL_OPS[op], a.shape[0], _lib.ptr(a), _lib.ptr(b), _lib.ptr(out)), f"fp_eval({op})")
+    return out[:a.shape[0]]
+
+
+# operations of curve_eval (bls_kernels.cuh CURVE_G1L_* / CURVE_G2_*)
+CURVE_EVAL_OPS = {"g1l_add_mixed": 0, "g1l_add": 1, "g1l_in_subgroup": 2,
+                  "g2_add": 32, "g2_add_mixed": 33, "g2_double": 34, "g2_in_subgroup": 35, "g2_psi": 36,
+                  "g2_clear_cofactor": 37, "g2_sswu_iso": 38, "g2_h2c_finish": 39}
+
+
+def curve_eval(op: str, a, b=None) -> np.ndarray:
+    """Self-test: one device curve stage on raw limbs.  a, b: uint32[n, 73] (X, Y, Z as 24-word slots, Fp in the first 12
+    words, Fp2 c0 | c1, then the affine infinity flag); returns uint32[n, 73]: the result point, then the flag word
+    (subgroup verdict, or the infinity flag of an affine result)."""
+    a = np.ascontiguousarray(a, dtype=np.uint32)
+    b = np.zeros_like(a) if b is None else np.ascontiguousarray(b, dtype=np.uint32)
+    if a.ndim != 2 or a.shape[1] != 73 or b.shape != a.shape:
+        raise ValueError("operands must be uint32[n, 73]")
+    out = np.zeros((max(a.shape[0], 1), 73), dtype=np.uint32)
+    _lib.check(_lib.lib().b200_curve_eval(CURVE_EVAL_OPS[op], a.shape[0], _lib.ptr(a), _lib.ptr(b), _lib.ptr(out)),
+               f"curve_eval({op})")
     return out[:a.shape[0]]
 
 

@@ -245,6 +245,39 @@ __global__ void k_fp_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a
     o[24] = flag;
 }
 
+// Curve stages on FpL against the big-integer oracle (b200_curve_eval): the per-key kernel's Jacobian formulas and
+// subgroup check with this unit's products.  Operands are taken as given, any representative in [0, 2p), so that a test
+// can hand the exceptional branches a coordinate difference equal to p instead of 0.
+__global__ void k_curve_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
+                             uint32_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t* pa = a + size_t(i) * kCurveEvalWords;
+    const uint32_t* pb = b + size_t(i) * kCurveEvalWords;
+    Jac<FpL> p, q, r;
+    for (int k = 0; k < 12; k++) {
+        p.x.v.l[k] = pa[k]; p.y.v.l[k] = pa[24 + k]; p.z.v.l[k] = pa[48 + k];
+        q.x.v.l[k] = pb[k]; q.y.v.l[k] = pb[24 + k]; q.z.v.l[k] = pb[48 + k];
+    }
+    jac_set_inf(r);
+    uint32_t flag = 0;
+    switch (op) {
+    case CURVE_G1L_ADD_MIXED: jac_add_mixed(r, p, q.x, q.y); break;
+    case CURVE_G1L_ADD: jac_add(r, p, q); break;
+    case CURVE_G1L_IN_SUBGROUP: {
+        G1Aff s;
+        s.x = p.x.v; s.y = p.y.v; s.inf = pa[72];
+        flag = g1_in_subgroup_lazy(s) ? 1u : 0u;
+        break;
+    }
+    default: break;
+    }
+    uint32_t* o = out + size_t(i) * kCurveEvalWords;
+    for (int k = 0; k < 72; k++) o[k] = 0;
+    for (int k = 0; k < 12; k++) { o[k] = r.x.v.l[k]; o[24 + k] = r.y.v.l[k]; o[48 + k] = r.z.v.l[k]; }
+    o[72] = flag;
+}
+
 }  // namespace
 
 // dynamic shared memory for fp_pow's table; opts the kernel in to > 48 KiB once
@@ -303,6 +336,10 @@ void launch_fp_selftest(uint32_t n, uint32_t seed, uint32_t* out_mismatch, void*
 void launch_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream) {
     if (!n) return;
     k_fp_eval<<<(n + 127) / 128, 128, with_pow_tab(k_fp_eval, 128), static_cast<cudaStream_t>(stream)>>>(op, n, a, b, out);
+}
+void launch_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream) {
+    if (!n) return;
+    k_curve_eval<<<(n + 127) / 128, 128, with_pow_tab(k_curve_eval, 128), static_cast<cudaStream_t>(stream)>>>(op, n, a, b, out);
 }
 
 }  // namespace b200

@@ -133,6 +133,57 @@ __global__ void B200_G2_BOUNDS k_fp2_eval(int32_t op, uint32_t n, const uint32_t
     o[24] = flag;
 }
 
+// Curve stages of the signature / hash kernels against the big-integer oracle (b200_curve_eval), one per launch, as this
+// unit compiles them: the Jacobian formulas, the subgroup check, psi, cofactor clearing, the map and hash_to_G2's second
+// half on Jacobian inputs
+__device__ __forceinline__ void curve2_load(G2Jac& p, const uint32_t* w) {
+    for (int k = 0; k < 12; k++) {
+        p.x.c0.l[k] = w[k]; p.x.c1.l[k] = w[12 + k];
+        p.y.c0.l[k] = w[24 + k]; p.y.c1.l[k] = w[36 + k];
+        p.z.c0.l[k] = w[48 + k]; p.z.c1.l[k] = w[60 + k];
+    }
+}
+__global__ void B200_G2_BOUNDS k_curve2_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
+                                             uint32_t* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t* pa = a + size_t(i) * kCurveEvalWords;
+    G2Jac p, q, r;
+    curve2_load(p, pa);
+    curve2_load(q, b + size_t(i) * kCurveEvalWords);
+    jac_set_inf(r);
+    uint32_t flag = 0;
+    switch (op) {
+    case CURVE_G2_ADD: jac_add(r, p, q); break;
+    case CURVE_G2_ADD_MIXED: jac_add_mixed(r, p, q.x, q.y); break;
+    case CURVE_G2_DOUBLE: jac_double(r, p); break;
+    case CURVE_G2_IN_SUBGROUP: {
+        G2Aff s;
+        s.x = p.x; s.y = p.y; s.inf = pa[72];
+        flag = g2_in_subgroup(s) ? 1u : 0u;
+        break;
+    }
+    case CURVE_G2_PSI: g2_psi(r, p); break;
+    case CURVE_G2_CLEAR_COFACTOR: g2_clear_cofactor(r, p); break;
+    case CURVE_G2_SSWU_ISO: B200_SSWU_ISO(r, p.x); break;
+    case CURVE_G2_H2C_FINISH: {
+        G2Aff h;
+        hash_to_g2_finish(h, p, q);
+        r.x = h.x; r.y = h.y; r.z = h.inf ? fp2_zero() : fp2_one();
+        flag = h.inf;
+        break;
+    }
+    default: break;
+    }
+    uint32_t* o = out + size_t(i) * kCurveEvalWords;
+    for (int k = 0; k < 12; k++) {
+        o[k] = r.x.c0.l[k]; o[12 + k] = r.x.c1.l[k];
+        o[24 + k] = r.y.c0.l[k]; o[36 + k] = r.y.c1.l[k];
+        o[48 + k] = r.z.c0.l[k]; o[60 + k] = r.z.c1.l[k];
+    }
+    o[72] = flag;
+}
+
 }  // namespace
 
 constexpr size_t kPowTab = 0;  // thread-local table here (see above)
@@ -159,6 +210,10 @@ void launch_g2_sum_compress(const G2Aff* sigs, const int32_t* sig_code, uint32_t
 void launch_fp2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream) {
     if (!n) return;
     k_fp2_eval<<<(n + kSmallCta - 1) / kSmallCta, kSmallCta, kPowTab, static_cast<cudaStream_t>(stream)>>>(op, n, a, b, out);
+}
+void launch_curve2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream) {
+    if (!n) return;
+    k_curve2_eval<<<(n + kSmallCta - 1) / kSmallCta, kSmallCta, kPowTab, static_cast<cudaStream_t>(stream)>>>(op, n, a, b, out);
 }
 
 }  // namespace b200

@@ -86,5 +86,18 @@ enum : int32_t {
 constexpr uint32_t kFpEvalIn = 24, kFpEvalOut = 25;
 void launch_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
 void launch_fp2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
+// on-device self-test of single curve stages (b200_curve_eval).  Records of kCurveEvalWords words: X, Y, Z as 24-word
+// slots (Fp in the first 12 words, Fp2 as c0 then c1), then a flag word: in, the affine infinity flag of operand a; out,
+// the subgroup verdict or the infinity flag of an affine result.  Affine operands are (X, Y) with Z ignored.
+enum : int32_t {
+    CURVE_G1L_ADD_MIXED = 0, CURVE_G1L_ADD = 1, CURVE_G1L_IN_SUBGROUP = 2,
+    CURVE_G1_N_OPS = 3,                                              // bls_g1.cu on FpL: the per-key kernel's formulas
+    CURVE_G2_ADD = 32, CURVE_G2_ADD_MIXED = 33, CURVE_G2_DOUBLE = 34, CURVE_G2_IN_SUBGROUP = 35, CURVE_G2_PSI = 36,
+    CURVE_G2_CLEAR_COFACTOR = 37, CURVE_G2_SSWU_ISO = 38, CURVE_G2_H2C_FINISH = 39,
+    CURVE_G2_END = 40                                                // bls_g2.cu: the signature / hash kernels' build
+};
+constexpr uint32_t kCurveEvalWords = 73;
+void launch_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
+void launch_curve2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
 
 }  // namespace b200

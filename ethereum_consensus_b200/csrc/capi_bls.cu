@@ -758,6 +758,34 @@ int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* 
     return B200_SUCCESS;
 }
 
+int32_t b200_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    const bool g2 = op >= CURVE_G2_ADD && op < CURVE_G2_END;
+    if (!(g2 || (op >= 0 && op < CURVE_G1_N_OPS)) || n > (1u << 24)) return B200_ERR_BAD_ARG;
+    if (n == 0) return B200_SUCCESS;
+    if (!a || !b || !out) return B200_ERR_BAD_ARG;
+    const size_t bytes = size_t(n) * kCurveEvalWords * 4;
+    uint32_t* d = nullptr;
+    B200_CUDA_TRY(cudaMalloc(&d, 3 * bytes));
+    uint32_t* da = d;
+    uint32_t* db = d + size_t(n) * kCurveEvalWords;
+    uint32_t* dout = db + size_t(n) * kCurveEvalWords;
+    cudaMemcpyAsync(da, a, bytes, cudaMemcpyHostToDevice, e.stream);
+    cudaMemcpyAsync(db, b, bytes, cudaMemcpyHostToDevice, e.stream);
+    if (g2) launch_curve2_eval(op, n, da, db, dout, e.stream);
+    else launch_curve_eval(op, n, da, db, dout, e.stream);
+    e.launches++;
+    cudaError_t ce = cudaGetLastError();
+    if (ce == cudaSuccess) ce = cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, e.stream);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(e.stream);
+    cudaFree(d);
+    if (ce != cudaSuccess) { e.last_error = cudaGetErrorString(ce); return B200_ERR_CUDA; }
+    return B200_SUCCESS;
+}
+
 int32_t b200_fast_aggregate_verify_batch(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs32,
                                          const uint8_t* sigs, size_t n_tuples, int32_t* out_codes) {
     Engine& e = engine();

@@ -268,6 +268,12 @@ B200_API int32_t b200_fp_selftest(uint32_t n, uint32_t seed, uint32_t* mismatche
  * FP2_EVAL_*) is applied to `n` operand pairs.  a, b: n x 24 raw little-endian 32-bit limbs (Fp in the first 12, Fp2 as
  * c0 then c1); out: n x 25 (the result's limbs, then a carry / borrow / square / sign flag).  Test use only. */
 B200_API int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
+/* On-device self-test of single curve stages, for comparison with a big-integer oracle: `op` (bls_kernels.cuh,
+ * CURVE_G1L_* on the per-key kernel's lazily reduced field, CURVE_G2_* in the signature / hash unit) is applied to `n`
+ * operand pairs.  a, b, out: n x 73 words: X, Y, Z as 24-word slots of raw little-endian 32-bit Montgomery limbs (Fp in
+ * the first 12 words of a slot, Fp2 as c0 then c1), then a flag word (in: the affine infinity flag; out: the subgroup
+ * verdict, or the infinity flag of an affine result).  Test use only. */
+B200_API int32_t b200_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
 
 #ifdef __cplusplus
 }
