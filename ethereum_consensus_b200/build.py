@@ -16,11 +16,12 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper)
 FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 # Per-TU ptxas optimisation level.  The three BLS translation units whose kernels are chains of inline-PTX Montgomery
-# products are assembled at -O1: at the default level ptxas interleaves more carry chains than it has predicate
+# products are assembled below the default level: at -O3 ptxas interleaves more carry chains than it has predicate
 # registers and spills the carries into a GPR bitmask (LOP3 / P2R / ISETP around every product); at -O1 the same
-# IMAD.WIDE remain, four chains stay interleaved and the spill code is gone.
+# IMAD.WIDE remain, four chains stay interleaved and the spill code is gone.  bls_g1.cu, whose per-key kernel has no
+# shared-memory table and spills to an L1-resident stack, is fastest at -O2 (DESIGN.md §4, K1's memory).
 # `B200_PTXAS_OPT=bls_g1.cu:3` restores the default level for a TU.  NVVM still runs at -O3.
-DEFAULT_PTXAS_OPT = {"bls_g1.cu": 1, "bls_g2.cu": 1, "bls_vm.cu": 1}
+DEFAULT_PTXAS_OPT = {"bls_g1.cu": 2, "bls_g2.cu": 1, "bls_vm.cu": 1}
 
 
 def _stale(target: Path, deps) -> bool:

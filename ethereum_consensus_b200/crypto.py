@@ -278,7 +278,7 @@ def fp_selftest(n: int = 1 << 16, seed: int = 1) -> int:
 # operations of fp_eval (bls_kernels.cuh FP_EVAL_* / FP2_EVAL_*)
 FP_EVAL_OPS = {"fp_mul": 0, "fp_sqr": 1, "fpl_mul": 2, "fpl_sqr": 3, "fp_add": 4, "fp_sub": 5, "fp_neg": 6, "fpl_add": 7,
                "fpl_sub": 8, "fpl_neg": 9, "fp_add_raw": 10, "fp_sub_raw": 11, "fp_inv_kaliski": 12, "fp_inv_fermat": 13,
-               "fp_sqrt": 14, "fpl_pow_sqrt": 15, "fp_is_lex_largest": 16,
+               "fp_sqrt": 14, "fpl_pow_sqrt": 15, "fp_is_lex_largest": 16, "fpl_sqrt_chain": 18,
                "fp2_mul": 32, "fp2_sqr": 33, "fp2_inv": 34, "fp2_sqrt": 35, "fp2_sgn0": 36}
 
 

@@ -237,6 +237,7 @@ __global__ void k_fp_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a
     case FP_EVAL_INV_FERMAT: fp_inv_fermat(r, x); break;
     case FP_EVAL_SQRT: flag = fp_sqrt(r, x) ? 1u : 0u; break;
     case FPL_EVAL_POW_SQRT: fpl_pow(rl, xl, B200_EXP_TABLE(exp_sqrt)); r = rl.v; break;
+    case FPL_EVAL_SQRT_CHAIN: fpl_sqrt_chain(rl, xl); r = rl.v; break;
     case FP_EVAL_IS_LEX_LARGEST: flag = fp_is_lex_largest(x) ? 1u : 0u; break;
     default: break;
     }
@@ -297,6 +298,25 @@ static size_t with_pow_tab(K kernel, unsigned threads) {
     if (n_seen < 16) { seen[n_seen] = key; granted[n_seen++] = bytes; }
     return bytes;
 }
+// Shared memory of a per-key kernel launch.  Its square root is a fixed chain in registers (fpl_sqrt_chain), so it reaches
+// no pow table: no dynamic shared memory, and the carve-out asks for all of the SM's unified L1 / shared array as L1,
+// where the 168-register kernel's stack frames (384 threads x 280 B at 12 warps per SM) have to stay.
+template <class K>
+static size_t k1_smem(K kernel, unsigned threads) {
+#if defined(B200_G1_CANONICAL_FP)
+    return with_pow_tab(kernel, threads);   // fp_sqrt -> fp_pow
+#else
+    (void)threads;
+    static const void* done[3];
+    static int n_done = 0;
+    const void* key = reinterpret_cast<const void*>(kernel);
+    for (int i = 0; i < n_done; i++)
+        if (done[i] == key) return 0;
+    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 0);
+    if (n_done < 3) done[n_done++] = key;
+    return 0;
+#endif
+}
 // tuning knob (B200_G1_VARIANT): 7: 384 threads, 168 registers (default); 0: 256 threads, 224 registers; 6: 512 threads, 128 registers
 static int g_g1_variant = 7;
 static uint32_t g_g1_small_n = 3u * 148u * 384u;   // B200_G1_SMALL_N overrides (0: always 384-thread CTAs)
@@ -306,15 +326,15 @@ void launch_g1_validate(const uint8_t* keys, uint32_t n, G1Aff* out, int32_t* co
     if (!n) return;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     switch (g_g1_variant) {
-    case 6: k_g1_validate_r128<<<(n + 511) / 512, 512, with_pow_tab(k_g1_validate_r128, 512), st>>>(keys, n, out, codes); break;
-    case 0: k_g1_validate_main<<<(n + 255) / 256, 256, with_pow_tab(k_g1_validate_main, 256), st>>>(keys, n, out, codes); break;
+    case 6: k_g1_validate_r128<<<(n + 511) / 512, 512, k1_smem(k_g1_validate_r128, 512), st>>>(keys, n, out, codes); break;
+    case 0: k_g1_validate_main<<<(n + 255) / 256, 256, k1_smem(k_g1_validate_main, 256), st>>>(keys, n, out, codes); break;
     default:
         // 12 warps per SM either way; below ~3 full waves of 384-thread CTAs the same kernel goes out as three 128-thread
         // CTAs per SM, so that the last, partial wave spreads over all SMs instead of leaving most of them idle
         if (cta == 128 || (cta != 384 && n <= g_g1_small_n))
-            k_g1_validate_r168<<<(n + 127) / 128, 128, with_pow_tab(k_g1_validate_r168, 128), st>>>(keys, n, out, codes);
+            k_g1_validate_r168<<<(n + 127) / 128, 128, k1_smem(k_g1_validate_r168, 128), st>>>(keys, n, out, codes);
         else
-            k_g1_validate_r168<<<(n + 383) / 384, 384, with_pow_tab(k_g1_validate_r168, 384), st>>>(keys, n, out, codes);
+            k_g1_validate_r168<<<(n + 383) / 384, 384, k1_smem(k_g1_validate_r168, 384), st>>>(keys, n, out, codes);
         break;
     }
 }

@@ -80,6 +80,7 @@ enum : int32_t {
     FP_EVAL_ADD_RAW = 10, FP_EVAL_SUB_RAW = 11, FP_EVAL_INV_KALISKI = 12, FP_EVAL_INV_FERMAT = 13,
     FP_EVAL_SQRT = 14, FPL_EVAL_POW_SQRT = 15, FP_EVAL_IS_LEX_LARGEST = 16,
     FP_EVAL_N_OPS = 17,                                              // bls_g1.cu: the per-key kernel's build
+    FPL_EVAL_SQRT_CHAIN = 18,                                        // bls_g1.cu as well; 17 stays unassigned
     FP2_EVAL_MUL = 32, FP2_EVAL_SQR = 33, FP2_EVAL_INV = 34, FP2_EVAL_SQRT = 35, FP2_EVAL_SGN0 = 36,
     FP2_EVAL_END = 37                                                // bls_g2.cu: the signature / hash kernels' build
 };

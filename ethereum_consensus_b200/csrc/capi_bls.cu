@@ -736,7 +736,7 @@ int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* 
     int32_t rc = check_ready(e);
     if (rc) return rc;
     const bool fp2 = op >= FP2_EVAL_MUL && op < FP2_EVAL_END;
-    if (!(fp2 || (op >= 0 && op < FP_EVAL_N_OPS)) || n > (1u << 24)) return B200_ERR_BAD_ARG;
+    if (!(fp2 || (op >= 0 && op < FP_EVAL_N_OPS) || op == FPL_EVAL_SQRT_CHAIN) || n > (1u << 24)) return B200_ERR_BAD_ARG;
     if (n == 0) return B200_SUCCESS;
     if (!a || !b || !out) return B200_ERR_BAD_ARG;
     const size_t in_bytes = size_t(n) * kFpEvalIn * 4, out_bytes = size_t(n) * kFpEvalOut * 4;

@@ -139,4 +139,13 @@ B200_BIG void fpl_pow(FpL& r, const FpL& a, const uint32_t* e) {
     r = acc;
 }
 
+// a = a^(2^n): the squaring runs of the fixed chains, one call site per run
+B200_HD void fpl_sqr_n(FpL& a, int n) {
+#pragma unroll 1
+    for (int k = 0; k < n; k++) f_sqr(a, a);
+}
+
 }  // namespace b200
+
+// fpl_sqrt_chain(r, a): r = a^((p+1)/4), no table (what the per-key kernel's decompression runs)
+#include "fpl_sqrt_chain.cuh"

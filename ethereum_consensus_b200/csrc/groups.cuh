@@ -70,7 +70,8 @@ B200_HD bool g1_in_subgroup(const G1Aff& p) {
 }
 
 // ---- the same two steps on lazily reduced field elements (fpl.cuh): what the per-key kernel runs ----------------
-// decompression: identical checks and codes as g1_uncompress; y = (x^3 + 4)^((p+1)/4) with no reduction inside the chain
+// decompression: identical checks and codes as g1_uncompress; y = (x^3 + 4)^((p+1)/4) with no reduction inside the chain,
+// a fixed addition chain whose temporaries are registers (no pow table: the kernel's L1 stays free for its stack)
 B200_HD int32_t g1_uncompress_lazy(G1Aff& out, const uint8_t b[48]) {
     const uint8_t f = b[0];
     out.inf = 0;
@@ -85,7 +86,7 @@ B200_HD int32_t g1_uncompress_lazy(G1Aff& out, const uint8_t b[48]) {
     f_sqr(y2, xl);
     f_mul(y2, y2, xl);
     f_add(y2, y2, curve_b<FpL>());
-    fpl_pow(yl, y2, B200_EXP_TABLE(exp_sqrt));
+    fpl_sqrt_chain(yl, y2);
     f_sqr(c, yl);
     if (!f_eq(c, y2)) return BLS_POINT_NOT_ON_CURVE;
     Fp y = fpl_canon(yl);
@@ -99,7 +100,7 @@ B200_HD bool g1_in_subgroup_lazy(const G1Aff& p) {
     const FpL px = fpl_from_fp(p.x), py = fpl_from_fp(p.y);
     Jac<FpL> t, t2;
     jac_mul_u64(t, px, py, B200_Z_ABS);
-    jac_mul_u64_jac(t2, t, B200_Z_ABS);
+    jac_mul_u64_jac_cached(t2, t, B200_Z_ABS);
     const Fp beta = B200_FP_BETA;
     FpL bx, ny;
     f_mul(bx, px, fpl_from_fp(beta));
