@@ -279,6 +279,7 @@ def fp_selftest(n: int = 1 << 16, seed: int = 1) -> int:
 FP_EVAL_OPS = {"fp_mul": 0, "fp_sqr": 1, "fpl_mul": 2, "fpl_sqr": 3, "fp_add": 4, "fp_sub": 5, "fp_neg": 6, "fpl_add": 7,
                "fpl_sub": 8, "fpl_neg": 9, "fp_add_raw": 10, "fp_sub_raw": 11, "fp_inv_kaliski": 12, "fp_inv_fermat": 13,
                "fp_sqrt": 14, "fpl_pow_sqrt": 15, "fp_is_lex_largest": 16, "fpl_sqrt_chain": 18,
+               "fpl_mul_sub_mul": 19, "fpl_mul_sub_8sqr": 20,
                "fp2_mul": 32, "fp2_sqr": 33, "fp2_inv": 34, "fp2_sqrt": 35, "fp2_sgn0": 36}
 
 
@@ -295,7 +296,7 @@ def fp_eval(op: str, a, b=None) -> np.ndarray:
 
 
 # operations of curve_eval (bls_kernels.cuh CURVE_G1L_* / CURVE_G2_*)
-CURVE_EVAL_OPS = {"g1l_add_mixed": 0, "g1l_add": 1, "g1l_in_subgroup": 2,
+CURVE_EVAL_OPS = {"g1l_add_mixed": 0, "g1l_add": 1, "g1l_in_subgroup": 2, "g1l_double": 4,
                   "g2_add": 32, "g2_add_mixed": 33, "g2_double": 34, "g2_in_subgroup": 35, "g2_psi": 36,
                   "g2_clear_cofactor": 37, "g2_sswu_iso": 38, "g2_h2c_finish": 39}
 

@@ -215,9 +215,10 @@ __global__ void k_fp_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a
                           uint32_t* __restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    Fp x, y, r = fp_zero();
+    Fp x, y, x1, y1, r = fp_zero();
     for (int k = 0; k < 12; k++) { x.l[k] = a[size_t(i) * kFpEvalIn + k]; y.l[k] = b[size_t(i) * kFpEvalIn + k]; }
-    const FpL xl = fpl_from_fp(x), yl = fpl_from_fp(y);
+    for (int k = 0; k < 12; k++) { x1.l[k] = a[size_t(i) * kFpEvalIn + 12 + k]; y1.l[k] = b[size_t(i) * kFpEvalIn + 12 + k]; }
+    const FpL xl = fpl_from_fp(x), yl = fpl_from_fp(y), x1l = fpl_from_fp(x1), y1l = fpl_from_fp(y1);
     FpL rl;
     uint32_t flag = 0;
     switch (op) {
@@ -238,6 +239,8 @@ __global__ void k_fp_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a
     case FP_EVAL_SQRT: flag = fp_sqrt(r, x) ? 1u : 0u; break;
     case FPL_EVAL_POW_SQRT: fpl_pow(rl, xl, B200_EXP_TABLE(exp_sqrt)); r = rl.v; break;
     case FPL_EVAL_SQRT_CHAIN: fpl_sqrt_chain(rl, xl); r = rl.v; break;
+    case FPL_EVAL_MUL_SUB_MUL: f_mul_sub_mul(rl, xl, x1l, yl, y1l); r = rl.v; break;
+    case FPL_EVAL_MUL_SUB_8SQR: f_mul_sub_8sqr(rl, xl, x1l, yl); r = rl.v; break;
     case FP_EVAL_IS_LEX_LARGEST: flag = fp_is_lex_largest(x) ? 1u : 0u; break;
     default: break;
     }
@@ -265,6 +268,7 @@ __global__ void k_curve_eval(int32_t op, uint32_t n, const uint32_t* __restrict_
     switch (op) {
     case CURVE_G1L_ADD_MIXED: jac_add_mixed(r, p, q.x, q.y); break;
     case CURVE_G1L_ADD: jac_add(r, p, q); break;
+    case CURVE_G1L_DOUBLE: jac_double(r, p); break;
     case CURVE_G1L_IN_SUBGROUP: {
         G1Aff s;
         s.x = p.x.v; s.y = p.y.v; s.inf = pa[72];

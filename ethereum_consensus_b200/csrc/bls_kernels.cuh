@@ -81,6 +81,8 @@ enum : int32_t {
     FP_EVAL_SQRT = 14, FPL_EVAL_POW_SQRT = 15, FP_EVAL_IS_LEX_LARGEST = 16,
     FP_EVAL_N_OPS = 17,                                              // bls_g1.cu: the per-key kernel's build
     FPL_EVAL_SQRT_CHAIN = 18,                                        // bls_g1.cu as well; 17 stays unassigned
+    FPL_EVAL_MUL_SUB_MUL = 19, FPL_EVAL_MUL_SUB_8SQR = 20,            // bls_g1.cu: (a0 a1 - b0 b1)/R, (a0 a1 - 8 b0^2)/R
+    FPL_EVAL_END = 21,                                               //   (a0 / a1: words 0..11 / 12..23 of operand a)
     FP2_EVAL_MUL = 32, FP2_EVAL_SQR = 33, FP2_EVAL_INV = 34, FP2_EVAL_SQRT = 35, FP2_EVAL_SGN0 = 36,
     FP2_EVAL_END = 37                                                // bls_g2.cu: the signature / hash kernels' build
 };
@@ -93,6 +95,7 @@ void launch_fp2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* 
 enum : int32_t {
     CURVE_G1L_ADD_MIXED = 0, CURVE_G1L_ADD = 1, CURVE_G1L_IN_SUBGROUP = 2,
     CURVE_G1_N_OPS = 3,                                              // bls_g1.cu on FpL: the per-key kernel's formulas
+    CURVE_G1L_DOUBLE = 4,                                            // bls_g1.cu as well; 3 stays unassigned
     CURVE_G2_ADD = 32, CURVE_G2_ADD_MIXED = 33, CURVE_G2_DOUBLE = 34, CURVE_G2_IN_SUBGROUP = 35, CURVE_G2_PSI = 36,
     CURVE_G2_CLEAR_COFACTOR = 37, CURVE_G2_SSWU_ISO = 38, CURVE_G2_H2C_FINISH = 39,
     CURVE_G2_END = 40                                                // bls_g2.cu: the signature / hash kernels' build

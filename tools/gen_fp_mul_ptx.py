@@ -11,6 +11,11 @@ fuses each mad.lo.cc / madc.hi.cc pair into one IMAD.WIDE.U32(.X) with carry-in/
 * square: off-diagonal products a_i a_j (i<j) into TE (even columns) / TO (odd columns), doubled with funnel shifts,
   diagonal squares added, then 12 reduction rounds that fold one column per round; chain carry-outs are collected
   lazily in a side array (they only affect columns >= 12).                              66 + 12 + 144 = 222 wide MADs.
+* fused reductions for the per-key kernel's Jacobian formulas (fpl.cuh), built from the same pieces — schoolbook rows into
+  the square's even / odd accumulators, the square's body, and its 12-round reduction as the standalone REDC:
+  REDC(a*b + x*y)                                                                       144 + 144 + 144 = 432 wide MADs;
+  REDC(a*b + 32p^2 - 8x^2)                                                              144 + 78 + 144 = 366 wide MADs.
+  Their emulations are checked against big-ints in tests/test_fpl_fused.py.
 """
 from pathlib import Path
 
@@ -69,28 +74,35 @@ def build_mul():
 
 
 # ------------------------------------------------------------------------------------------------ square
-def build_sqr():
-    ops = []
-    live = set()          # registers that hold a defined value
+class Prog:
+    """One instruction list; `live` = registers that hold a defined value (others read as literal zero)."""
+    def __init__(self):
+        self.ops, self.live = [], set()
 
-    def emit(op, d, a, b=None, c=None):
-        ops.append((op, d, a, b, c))
-        live.add(d)
+    def emit(self, op, d, a, b=None, c=None):
+        self.ops.append((op, d, a, b, c))
+        self.live.add(d)
 
-    def val(r):           # operand: register if defined else literal zero
-        return r if r in live else "0"
+    def val(self, r):
+        return r if r in self.live else "0"
 
-    TE = [f"te{k}" for k in range(26)]   # TE[k] <-> column k
-    TO = [f"to{k}" for k in range(26)]   # TO[k] <-> column k + 1
-    CY = [f"c{k}" for k in range(26)]    # lazy carries, CY[k] <-> column k
+    def regs(self):
+        return sorted(self.live, key=lambda r: (r.rstrip("0123456789"), int("".join(ch for ch in r if ch.isdigit()) or 0)))
 
-    def lane(col):
-        """(array, index) of the even-aligned lane whose low word is column `col`."""
-        return (TE, col) if col % 2 == 0 else (TO, col - 1)
 
-    def word(col, arr):
-        return arr[col] if arr is TE else arr[col - 1]
+def wide_arrays(e, o):
+    """even / odd column accumulators of a 24-word value: E[k] <-> column k, O[k] <-> column k + 1"""
+    return [f"{e}{k}" for k in range(26)], [f"{o}{k}" for k in range(26)]
 
+
+def lane(TE, TO, col):
+    """(array, index) of the even-aligned lane whose low word is column `col`."""
+    return (TE, col) if col % 2 == 0 else (TO, col - 1)
+
+
+def sqr_body(P, TE, TO, X):
+    """X^2 into fresh accumulators: off-diagonal products, doubled with funnel shifts, plus the diagonal.  66 + 12 wide MADs."""
+    emit, val = P.emit, P.val
     # ---- off-diagonal products
     for i in range(N - 1):
         for parity in (0, 1):  # parity 0: j = i+2, i+4..  (even columns -> TE); parity 1: j = i+1, i+3.. (odd columns -> TO)
@@ -98,11 +110,11 @@ def build_sqr():
             if not js:
                 continue
             for n_, j in enumerate(js):
-                arr, idx = lane(i + j)
+                arr, idx = lane(TE, TO, i + j)
                 lo, hi = arr[idx], arr[idx + 1]
-                emit("mad.lo.cc" if n_ == 0 else "madc.lo.cc", lo, A(i), A(j), val(lo))
-                emit("madc.hi.cc", hi, A(i), A(j), val(hi))
-            arr, idx = lane(i + js[-1])
+                emit("mad.lo.cc" if n_ == 0 else "madc.lo.cc", lo, X(i), X(j), val(lo))
+                emit("madc.hi.cc", hi, X(i), X(j), val(hi))
+            arr, idx = lane(TE, TO, i + js[-1])
             top = arr[idx + 2]
             emit("addc", top, val(top), "0")
     # ---- double both arrays with funnel shifts (independent ops, high word first so sources are still intact)
@@ -110,17 +122,48 @@ def build_sqr():
         for k in range(23, -1, -1):
             hi_w = arr[k]
             lo_w = arr[k - 1] if k > 0 else None
-            if hi_w not in live and (lo_w is None or lo_w not in live):
+            if hi_w not in P.live and (lo_w is None or lo_w not in P.live):
                 continue
             emit("shf.l.wrap", hi_w, val(lo_w) if lo_w else "0", val(hi_w), "1")
     # ---- diagonal squares at even columns: one chain over the TE lanes
     for i in range(N):
         lo, hi = TE[2 * i], TE[2 * i + 1]
-        emit("mad.lo.cc" if i == 0 else "madc.lo.cc", lo, A(i), A(i), val(lo))
-        emit("madc.hi.cc", hi, A(i), A(i), val(hi))
+        emit("mad.lo.cc" if i == 0 else "madc.lo.cc", lo, X(i), X(i), val(lo))
+        emit("madc.hi.cc", hi, X(i), X(i), val(hi))
+
+
+def mul_body(P, TE, TO, pairs):
+    """sum of x*y over `pairs` into fresh accumulators, schoolbook: per row i and pair, one carry chain over the even-j
+    lanes and one over the odd-j lanes; a chain's carry-out lands in the word above its last lane, which no earlier chain
+    has carried into more than a few times (rows go up one column at a time).  144 wide MADs per pair."""
+    emit, val = P.emit, P.val
+    for i in range(N):
+        for X, Y in pairs:
+            for parity in (0, 1):
+                js = list(range(parity, N, 2))
+                for n_, j in enumerate(js):
+                    arr, idx = lane(TE, TO, i + j)
+                    lo, hi = arr[idx], arr[idx + 1]
+                    emit("mad.lo.cc" if n_ == 0 else "madc.lo.cc", lo, X(i), Y(j), val(lo))
+                    emit("madc.hi.cc", hi, X(i), Y(j), val(hi))
+                arr, idx = lane(TE, TO, i + js[-1])
+                top = arr[idx + 2]
+                emit("addc", top, val(top), "0")
+
+
+def redc(P, TE, TO):
+    """Montgomery reduction of the 24-column value TE + TO (+ lazy carries): 12 rounds that fold one column each; chain
+    carry-outs are collected lazily in a side array (they only affect columns >= 12).  144 wide MADs.  The value must
+    be below 2^768 and its reduction below 2^384; returns the 12 result registers."""
+    emit, val, live = P.emit, P.val, P.live
+    CY = [f"c{k}" for k in range(26)]    # lazy carries, CY[k] <-> column k
+
+    def word(col, arr):
+        return arr[col] if arr is TE else arr[col - 1]
+
     # ---- 12 reduction rounds; cy = pending carry into the current column
     for i in range(N):
-        X, xi = lane(i)                       # lane starting at column i
+        X, xi = lane(TE, TO, i)               # lane starting at column i
         Y = TO if X is TE else TE
         xlo = X[xi]
         yw = word(i, Y) if i > 0 or Y is TE else None
@@ -141,13 +184,13 @@ def build_sqr():
         emit("mul.lo", "m", xlo, "n0")
         # even-j products: lanes at columns i, i+2, .., i+10 (array X)
         for j in range(0, N, 2):
-            arr, idx = lane(i + j)
+            arr, idx = lane(TE, TO, i + j)
             emit("mad.lo.cc" if j == 0 else "madc.lo.cc", arr[idx], Pm(j), "m", val(arr[idx]))
             emit("madc.hi.cc", arr[idx + 1], Pm(j), "m", val(arr[idx + 1]))
         emit("addc", CY[i + 12], val(CY[i + 12]), "0")
         # odd-j products: lanes at columns i+1, .., i+11 (array Y)
         for j in range(1, N, 2):
-            arr, idx = lane(i + j)
+            arr, idx = lane(TE, TO, i + j)
             emit("mad.lo.cc" if j == 1 else "madc.lo.cc", arr[idx], Pm(j), "m", val(arr[idx]))
             emit("madc.hi.cc", arr[idx + 1], Pm(j), "m", val(arr[idx + 1]))
         emit("addc", CY[i + 13], val(CY[i + 13]), "0")
@@ -164,22 +207,74 @@ def build_sqr():
         emit("add.cc", res[0], res[0], "cy")
         for k in range(1, N):
             emit("addc.cc", res[k], res[k], "0")
-    regs = sorted(live, key=lambda r: (r.rstrip("0123456789"), int("".join(ch for ch in r if ch.isdigit()) or 0)))
-    return ops, regs, res
+    return res
+
+
+def build_sqr():
+    P = Prog()
+    TE, TO = wide_arrays("te", "to")
+    sqr_body(P, TE, TO, A)
+    res = redc(P, TE, TO)
+    return P.ops, P.regs(), res
+
+
+# ------------------------------------------------------------------------------------------------ fused reductions
+def X_(j): return f"x{j}"  # noqa: E302
+def Y_(j): return f"y{j}"  # noqa: E302
+
+
+def build_mul_add_mul():
+    """REDC(a*b + x*y): both schoolbook products into one 24-word accumulator, then ONE reduction.  432 wide MADs (two
+    separate products: 576).  Needs a*b + x*y < 2^768 and a result below 2^384: operands below 2p give < 8p^2, REDC < 1.82p."""
+    P = Prog()
+    TE, TO = wide_arrays("te", "to")
+    mul_body(P, TE, TO, [(A, B), (X_, Y_)])
+    res = redc(P, TE, TO)
+    return P.ops, P.regs(), res
+
+
+K32PP = 32 * P_INT * P_INT
+
+
+def build_mul_sub_8sqr():
+    """REDC(a*b + 32p^2 - 8x^2) for a, b, x < 2p: a*b into (TE, TO), x^2 into a second pair (UE, UO) by the square's
+    body, then TE += 32p^2 - 8 UE - 8 UO 2^32 (shifts by 3 on the way), then ONE reduction of (TE, TO).
+    144 + 78 + 144 = 366 wide MADs (product + square + product: 798).  Every partial sum stays in [0, 36p^2) < 2^767:
+    8 UE <= 8x^2 < 32p^2 and 8 UE + 8 UO 2^32 = 8x^2."""
+    P = Prog()
+    emit, val = P.emit, P.val
+    TE, TO = wide_arrays("te", "to")
+    UE, UO = wide_arrays("ue", "uo")
+    mul_body(P, TE, TO, [(A, B)])
+    sqr_body(P, UE, UO, X_)
+    kw = [f"0x{(K32PP >> (32 * k)) & 0xffffffff:08x}" for k in range(24)]
+    for k in range(24):
+        emit("add.cc" if k == 0 else "addc.cc", TE[k], val(TE[k]), kw[k])
+    for k in range(24):       # TE -= 8 UE
+        emit("shf.l.wrap", "s", val(UE[k - 1]) if k > 0 else "0", val(UE[k]), "3")
+        emit("sub.cc" if k == 0 else "subc.cc", TE[k], TE[k], "s")
+    for k in range(23):       # TE -= 8 UO 2^32  (UO[k] <-> column k + 1)
+        emit("shf.l.wrap", "s", val(UO[k - 1]) if k > 0 else "0", val(UO[k]), "3")
+        emit("sub.cc" if k == 0 else "subc.cc", TE[k + 1], TE[k + 1], "s")
+    res = redc(P, TE, TO)
+    return P.ops, P.regs(), res
 
 
 # ------------------------------------------------------------------------------------------------ emitters
-def emit_c(name, ops, regs, res, two_inputs):
+def _sig(name, inputs, qual):
+    return f"{qual} void {name}(uint32_t r[12], " + ", ".join(f"const uint32_t {x}[12]" for x in inputs) + ") {\n"
+
+
+def emit_c(name, ops, regs, res, inputs):
     c = []
-    c.append(f"B200_HD void {name}(uint32_t r[12], const uint32_t a[12]" + (", const uint32_t b[12]" if two_inputs else "") + ") {\n")
+    c.append(_sig(name, inputs, "B200_HD"))
     c.append("    const uint32_t n0 = B200_FP_N0;\n")
     c.append("    " + " ".join(f"const uint32_t p{j} = 0x{P_LIMBS[j]:08x}u;" for j in range(12)) + "\n")
-    c.append("    " + " ".join(f"const uint32_t a{j} = a[{j}];" for j in range(12)) + "\n")
-    if two_inputs:
-        c.append("    " + " ".join(f"const uint32_t b{j} = b[{j}];" for j in range(12)) + "\n")
+    for x in inputs:
+        c.append("    " + " ".join(f"const uint32_t {x}{j} = {x}[{j}];" for j in range(12)) + "\n")
     c.append("    uint32_t cc = 0; uint64_t w; (void)cc; (void)n0;\n")
     c.append("    uint32_t " + ", ".join(f"{r} = 0" for r in regs) + ";\n")
-    def lit(x): return "0u" if x == "0" else ("1u" if x == "1" else x)
+    def lit(x): return "0u" if x == "0" else ("1u" if x == "1" else (x + "u" if x.startswith("0x") else x))
     for op, d, x, y, z in ops:
         x, y, z = (lit(x) if x is not None else None, lit(y) if y is not None else None, lit(z) if z is not None else None)
         if op == "mul.lo": c.append(f"    {d} = {x} * {y};\n")
@@ -192,37 +287,39 @@ def emit_c(name, ops, regs, res, two_inputs):
         elif op == "addc.cc": c.append(f"    w = uint64_t({x}) + {y} + cc; {d} = uint32_t(w); cc = uint32_t(w >> 32);\n")
         elif op == "addc": c.append(f"    {d} = {x} + {y} + cc;\n")
         elif op == "add": c.append(f"    {d} = {x} + {y};\n")
+        elif op == "sub.cc": c.append(f"    w = uint64_t({x}) - {y}; {d} = uint32_t(w); cc = uint32_t(w >> 63);\n")
+        elif op == "subc.cc": c.append(f"    w = uint64_t({x}) - {y} - cc; {d} = uint32_t(w); cc = uint32_t(w >> 63);\n")
         elif op == "mov": c.append(f"    {d} = {x};\n")
-        elif op == "shf.l.wrap": c.append(f"    {d} = ({y} << 1) | ({x} >> 31);\n")
+        elif op == "shf.l.wrap" and z == "1u": c.append(f"    {d} = ({y} << 1) | ({x} >> 31);\n")
+        elif op == "shf.l.wrap": c.append(f"    {d} = ({y} << {z}) | ({x} >> (32 - {z}));\n")
         else: raise ValueError(op)
     c.append("    " + " ".join(f"r[{k}] = {res[k]};" for k in range(12)) + "\n}\n\n")
     return c
 
 
-def emit_ptx(name, ops, regs, res, two_inputs):
+def emit_ptx(name, ops, regs, res, inputs):
     names = {}
     temps = [r for r in regs if r not in res]
     for k, nme in enumerate(res): names[nme] = f"%{k}"
-    ins = [f"a{j}" for j in range(12)] + ([f"b{j}" for j in range(12)] if two_inputs else [])
+    ins = [f"{x}{j}" for x in inputs for j in range(12)]
     for k, nme in enumerate(ins): names[nme] = f"%{len(res) + k}"
     for k, nme in enumerate(temps): names[nme] = f"t{k}"
     for j in range(12): names[f"p{j}"] = f"0x{P_LIMBS[j]:08x}"
-    names["n0"] = "0xfffcfffd"; names["0"] = "0"; names["1"] = "1"
+    names["n0"] = "0xfffcfffd"; names["0"] = "0"; names["1"] = "1"; names["3"] = "3"
     lines = ["{", f".reg .u32 t<{len(temps)}>;"]
     for op, d, x, y, z in ops:
-        args = [names[d], names[x]] + ([names[y]] if y is not None else []) + ([names[z]] if z is not None else [])
+        args = [names.get(v, v) for v in (d, x, y, z) if v is not None]
         suffix = ".b32" if op in ("shf.l.wrap", "mov") else ".u32"
         lines.append(f"{op}{suffix} {', '.join(args)};")
     lines.append("}")
     c = []
-    c.append(f"__device__ __forceinline__ void {name}(uint32_t r[12], const uint32_t a[12]" + (", const uint32_t b[12]" if two_inputs else "") + ") {\n")
+    c.append(_sig(name, inputs, "__device__ __forceinline__"))
     c.append("    uint32_t " + ", ".join(res) + ";\n")
     c.append("    asm(\n")
     for ln in lines:
         c.append(f'        "{ln}\\n\\t"\n')
     c.append("        : " + ", ".join(f'"=&r"({n})' for n in res) + "\n")
-    srcs = ["a"] + (["b"] if two_inputs else [])
-    c.append("        : " + ", ".join(f'"r"({n}[{j}])' for n in srcs for j in range(12)) + ");\n")
+    c.append("        : " + ", ".join(f'"r"({n}[{j}])' for n in inputs for j in range(12)) + ");\n")
     c.append("    " + " ".join(f"r[{k}] = {res[k]};" for k in range(12)) + "\n}\n\n")
     return c
 
@@ -242,25 +339,38 @@ def split_carry_captures(ops, regs):
     return out, (regs + ["ct"] if "ct" not in regs else regs)
 
 
+def wide_macs(ops):
+    return sum(1 for o in ops if o[0] in ("mul.lo", "mad.lo.cc", "madc.lo.cc") and o[3] != "n0")
+
+
 def main():
     import sys
     mul_ops, mul_regs, mul_res = build_mul()
     sqr_ops, sqr_regs, sqr_res = build_sqr()
+    mam_ops, mam_regs, mam_res = build_mul_add_mul()
+    m8s_ops, m8s_regs, m8s_res = build_mul_sub_8sqr()
     if "--split-carry" in sys.argv:
         mul_ops, mul_regs = split_carry_captures(mul_ops, mul_regs)
         sqr_ops, sqr_regs = split_carry_captures(sqr_ops, sqr_regs)
     out = ["// GENERATED by tools/gen_fp_mul_ptx.py — do not edit.  Included from fp.cuh (needs B200_HD, B200_FP_N0).\n#pragma once\n\nnamespace b200 {\n\n"]
     out.append("// C emulations of the PTX instruction lists below (same order, explicit carry flag `cc`).  Results in [0, 2p).\n")
-    out += emit_c("fp_mul_emul_core", mul_ops, mul_regs, mul_res, True)
-    out += emit_c("fp_sqr_emul_core", sqr_ops, sqr_regs, sqr_res, False)
+    out += emit_c("fp_mul_emul_core", mul_ops, mul_regs, mul_res, ["a", "b"])
+    out += emit_c("fp_sqr_emul_core", sqr_ops, sqr_regs, sqr_res, ["a"])
+    out.append("// fused reductions (fpl.cuh): r = REDC(a b + x y) and r = REDC(a b + 32 p^2 - 8 x^2), operands in [0, 2p);\n"
+               "// results below 1.82 p and 4.66 p.\n")
+    out += emit_c("fp_mul_add_mul_emul_core", mam_ops, mam_regs, mam_res, ["a", "b", "x", "y"])
+    out += emit_c("fp_mul_sub_8sqr_emul_core", m8s_ops, m8s_regs, m8s_res, ["a", "b", "x"])
     out.append("#if defined(__CUDA_ARCH__)\n// r = a*b/R mod p and r = a*a/R mod p, results in [0, 2p); inputs < p.\n")
-    out += emit_ptx("fp_mul_ptx_core", mul_ops, mul_regs, mul_res, True)
-    out += emit_ptx("fp_sqr_ptx_core", sqr_ops, sqr_regs, sqr_res, False)
+    out += emit_ptx("fp_mul_ptx_core", mul_ops, mul_regs, mul_res, ["a", "b"])
+    out += emit_ptx("fp_sqr_ptx_core", sqr_ops, sqr_regs, sqr_res, ["a"])
+    out.append("// the fused reductions, as above\n")
+    out += emit_ptx("fp_mul_add_mul_ptx_core", mam_ops, mam_regs, mam_res, ["a", "b", "x", "y"])
+    out += emit_ptx("fp_mul_sub_8sqr_ptx_core", m8s_ops, m8s_regs, m8s_res, ["a", "b", "x"])
     out.append("#endif\n\n}  // namespace b200\n")
     path = Path(__file__).resolve().parent.parent / "ethereum_consensus_b200" / "csrc" / "fp_mul_ptx.cuh"
     path.write_text("".join(out))
-    wide = lambda ops: sum(1 for o in ops if o[0] in ("mul.lo", "mad.lo.cc", "madc.lo.cc") and o[3] != "n0")  # noqa: E731
-    print("wrote", path, "mul ops:", len(mul_ops), "wide:", wide(mul_ops), "| sqr ops:", len(sqr_ops), "wide:", wide(sqr_ops))
+    print("wrote", path, "wide MADs: mul", wide_macs(mul_ops), "| sqr", wide_macs(sqr_ops), "| mul_add_mul", wide_macs(mam_ops),
+          "| mul_sub_8sqr", wide_macs(m8s_ops))
 
 
 if __name__ == "__main__":
