@@ -54,6 +54,8 @@ _PROTOS = {
     "b200_state_update_elements": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t]),
     "b200_state_update_bytes": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t]),
     "b200_state_root_incremental": (C.c_int32, [C.c_void_p, C.c_void_p]),
+    "b200_state_append_elements": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t]),
+    "b200_state_set_field": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t]),
     "b200_htr_beacon_state_deneb_shard": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "b200_htr_beacon_state_deneb_combine": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "b200_compute_shuffled_indices": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_void_p]),

@@ -59,22 +59,27 @@ struct b200_state {
     DevBuf arena, fields, planbuf, selbuf, scatter;
     bool uploaded = false;
     // ---- incremental re-hash (b200_state_update_* / b200_state_root_incremental) ----
-    // Host shadow of the serialization with everything EXCEPT the five big lists filled in (their byte ranges stay
-    // untouched zero pages of an anonymous mapping): small-field updates patch it and the plan is rebuilt from it.
+    // Host shadow of the serialization with everything EXCEPT the five big lists filled in (their byte ranges are never
+    // written or read: untouched zero pages of an anonymous mapping): small-field updates patch it and the plan is
+    // rebuilt from it.  `shadow_cap` bytes are allocated, so that a reshape (b200_state_append_elements /
+    // b200_state_set_field) moves the bytes after the changed field in place; past that it is re-allocated.
     uint8_t* shadow = nullptr;
-    size_t len = 0;
+    size_t len = 0, shadow_cap = 0;
     int preset = 0;
     StateOffsets so;
+    uint64_t cap[5] = {0, 0, 0, 0, 0};   // elements each big list's device regions are reserved for
     // per chain (5 big lists, then block_roots / state_roots / randao_mixes / slashings): changed first-job inputs
     // (Validator records / 32-byte chunks), unsorted
     std::vector<uint32_t> dirty[9];
+    std::vector<char> rehash = std::vector<char>(9, 0);  // chains to re-hash in full at the next root
     bool small_dirty = false;
     std::vector<std::pair<const uint8_t*, const uint8_t*>> small_ranges;  // patched shadow bytes since the last root
-    bool pinned_head = false, pinned_tail = false;
+    uint8_t* pinned_head = nullptr;   // page-locked ranges of the shadow (registration is an optimisation)
+    uint8_t* pinned_tail = nullptr;
     bool sharded = false;   // b200_state_upload_deneb_sharded: this rank's slices only; root is a collective, no updates
     ~b200_state() {  // callers hold the engine lock and have selected the device
-        if (pinned_head) cudaHostUnregister(shadow);
-        if (pinned_tail) cudaHostUnregister(shadow + so.var[7]);
+        if (pinned_head) cudaHostUnregister(pinned_head);
+        if (pinned_tail) cudaHostUnregister(pinned_tail);
         free(shadow);
         arena.release(); fields.release(); planbuf.release(); selbuf.release(); scatter.release();
     }
@@ -87,6 +92,145 @@ constexpr uint32_t kBigElem[5] = {121, 8, 1, 1, 8};  // element size in bytes
 inline uint32_t big_input_of(int f, uint64_t i) { return uint32_t(f == 0 ? i : (i * kBigElem[f]) / 32); }
 inline uint64_t big_count(const b200_state* h, int f) {
     return uint64_t(h->so.var[kBigVar[f] + 1] - h->so.var[kBigVar[f]]) / kBigElem[f];
+}
+// Elements reserved beyond a big list's length when its device regions are (re)allocated: 2^16 (one 8 MB slab of
+// Validator records) or a sixteenth of the list, whichever is larger.  Deposits then append in place for many blocks;
+// crossing the capacity relocates the list on the device.
+inline uint64_t headroom(uint64_t n) { return std::max<uint64_t>(uint64_t(1) << 16, n / 16); }
+constexpr size_t kShadowSlack = 64 << 10;   // shadow bytes beyond the reserved lists: header / summaries growth
+constexpr uint64_t kRegistryLimit = uint64_t(1) << 40;   // VALIDATOR_REGISTRY_LIMIT (both presets)
+
+size_t shadow_bytes_for(const b200_state* h) {
+    size_t b = h->len + kShadowSlack;
+    for (int f = 0; f < 5; f++) b += size_t(h->cap[f] - big_count(h, f)) * kBigElem[f];
+    const size_t votes = h->so.var[2] - h->so.var[1];
+    return b + size_t(eth1_data_votes_bound(h->preset) * 72) - votes;
+}
+
+// Page-lock the head of the shadow up to eth1_data_votes (the fixed part and historical_roots: it never changes size),
+// and the tail (latest_execution_payload_header, the two withdrawal indices, historical_summaries) while it stays where
+// it is.  A staged copy lies wholly inside or wholly outside each range (eth1_data_votes starts where the head ends).
+void pin_shadow(b200_state* h, bool tail) {
+    if (cudaHostRegister(h->shadow, h->so.var[1], cudaHostRegisterDefault) == cudaSuccess) h->pinned_head = h->shadow;
+    if (tail && cudaHostRegister(h->shadow + h->so.var[7], h->len - h->so.var[7], cudaHostRegisterDefault) == cudaSuccess)
+        h->pinned_tail = h->shadow + h->so.var[7];
+    cudaGetLastError();  // pageable copies work too
+}
+void unpin_tail(b200_state* h) {
+    if (h->pinned_tail) cudaHostUnregister(h->pinned_tail);
+    h->pinned_tail = nullptr;
+}
+
+// Resize variable-size field k (StateOffsets::var index) of the shadow to `new_size` bytes: the shadow's bytes after it
+// move, the offset words after it are rewritten, h->len follows.  The field's own bytes are the caller's to fill; call
+// reparse() after.  Refuses (leaving everything as it was) a serialization beyond the 32-bit offsets' reach.
+int32_t reshape_shadow(Engine& e, b200_state* h, int k, size_t new_size) {
+    const size_t old_size = h->so.var[k + 1] - h->so.var[k];
+    if (new_size == old_size) return B200_SUCCESS;
+    const uint64_t new_len = uint64_t(h->len) - old_size + new_size;
+    if (new_len > 0xffffffffull) { e.last_error = "state reshape: the serialization would exceed 4 GiB"; return B200_ERR_LIMIT; }
+    if (new_len > h->shadow_cap) {
+        const size_t want = shadow_bytes_for(h) + (new_len - h->len);
+        uint8_t* ns = static_cast<uint8_t*>(calloc(want, 1));
+        if (!ns) { e.last_error = "out of host memory for the state shadow"; return B200_ERR_CUDA; }
+        memcpy(ns, h->shadow, h->so.var[2]);
+        memcpy(ns + h->so.var[7], h->shadow + h->so.var[7], h->len - h->so.var[7]);
+        if (h->pinned_head) cudaHostUnregister(h->pinned_head);
+        h->pinned_head = nullptr;
+        unpin_tail(h);
+        free(h->shadow);
+        h->shadow = ns; h->shadow_cap = want;
+        pin_shadow(h, false);
+    }
+    // the shadow holds nothing of the big lists: what moves is [max(end of field k, start of the header), len)
+    const size_t from = std::max<size_t>(h->so.var[k + 1], h->so.var[7]);
+    unpin_tail(h);   // the tail moves or changes size: it stays pageable from now on (a few KB to copy)
+    if (from < h->len) memmove(h->shadow + (from + new_size - old_size), h->shadow + from, h->len - from);
+    for (int i = k + 1; i < 9; i++) {
+        const uint32_t v = uint32_t(h->so.var[i] + new_size - old_size);
+        uint8_t* w = h->shadow + h->so.var_word[i];
+        w[0] = uint8_t(v); w[1] = uint8_t(v >> 8); w[2] = uint8_t(v >> 16); w[3] = uint8_t(v >> 24);
+    }
+    for (int i = k + 1; i < 10; i++) h->so.var[i] = uint32_t(h->so.var[i] + new_size - old_size);
+    h->len = size_t(new_len);
+    return B200_SUCCESS;
+}
+bool reparse(b200_state* h) { return parse_beacon_state(h->shadow, h->len, h->preset, h->so); }
+
+// every small staged field: re-copied and re-hashed at the next root (their field-buffer and arena places follow the
+// sizes of eth1_data_votes / the header / historical_summaries)
+void mark_all_small(b200_state* h) {
+    h->small_dirty = true;
+    h->small_ranges.emplace_back(h->shadow, h->shadow + h->so.var[2]);
+    h->small_ranges.emplace_back(h->shadow + h->so.var[7], h->shadow + h->len);
+}
+
+// grow a device buffer keeping its contents
+int32_t grow_keep(Engine& e, DevBuf& b, size_t n) {
+    if (n <= b.cap) return B200_SUCCESS;
+    DevBuf nb;
+    B200_CUDA_TRY(nb.reserve(n));
+    if (b.p) {
+        cudaError_t ce = cudaMemcpyAsync(nb.p, b.p, b.cap, cudaMemcpyDeviceToDevice, e.stream);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(e.stream);
+        if (ce != cudaSuccess) { nb.release(); e.last_error = cudaGetErrorString(ce); return B200_ERR_CUDA; }
+    }
+    b.release();
+    b = nb;
+    return B200_SUCCESS;
+}
+
+// Make `np` (planned from the shadow as it is now) the handle's plan.  Chains whose job sequence changed are re-hashed in
+// full at the next root.  When a chain's regions moved (a big list outgrew its capacity), the nine chains are copied into
+// new device buffers on the device — field bytes and every arena level — except the arena of a chain whose capacity
+// changed, which is re-hashed in full from its copied bytes; the small fields are re-staged.
+int32_t adopt_plan(Engine& e, b200_state* h, SszPlan& np, std::vector<uint32_t>& outs) {
+    bool moved = false;
+    for (int c = 0; c < 9; c++) moved = moved || !np.same_chain_layout(h->plan, c);
+    const size_t need_arena = np.arena_nodes() * 32, need_fields = np.field_bytes() + 256;
+    if (!moved) {
+        int32_t rc = grow_keep(e, h->arena, need_arena);
+        if (rc) return rc;
+        rc = grow_keep(e, h->fields, need_fields);
+        if (rc) return rc;
+    } else {
+        DevBuf na, nf;
+        cudaError_t ce = na.reserve(need_arena);
+        if (ce == cudaSuccess) ce = nf.reserve(need_fields);
+        std::vector<char> full(9, 0);
+        for (int c = 0; c < 9 && ce == cudaSuccess; c++) {
+            uint64_t fo = 0, fn = 0; size_t nb = 0;
+            h->plan.chain_field(c, &fo, &nb);
+            np.chain_field(c, &fn, &nb);
+            const size_t ro = h->plan.chain_region_bytes(c), rn = np.chain_region_bytes(c);
+            uint8_t* nfp = static_cast<uint8_t*>(nf.p);
+            ce = cudaMemcpyAsync(nfp + fn, static_cast<uint8_t*>(h->fields.p) + fo, std::min(ro, rn), cudaMemcpyDeviceToDevice, e.stream);
+            if (ce == cudaSuccess && rn > ro) ce = cudaMemsetAsync(nfp + fn + ro, 0, rn - ro, e.stream);
+            const auto& ao = h->plan.chain_arena(c);
+            const auto& an = np.chain_arena(c);
+            bool same_shape = ao.size() == an.size();
+            for (size_t i = 0; same_shape && i < ao.size(); i++) same_shape = ao[i].second == an[i].second;
+            if (!same_shape) { full[size_t(c)] = 1; continue; }
+            for (size_t i = 0; ce == cudaSuccess && i < ao.size(); i++)
+                ce = cudaMemcpyAsync(static_cast<uint32_t*>(na.p) + an[i].first * 8, static_cast<uint32_t*>(h->arena.p) + ao[i].first * 8,
+                                     ao[i].second * 32, cudaMemcpyDeviceToDevice, e.stream);
+        }
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(e.stream);
+        if (ce != cudaSuccess) {
+            na.release(); nf.release();
+            e.last_error = std::string("state relocation: ") + cudaGetErrorString(ce);
+            return B200_ERR_CUDA;
+        }
+        h->arena.release(); h->fields.release();
+        h->arena = na; h->fields = nf;
+        for (int c = 0; c < 9; c++) if (full[size_t(c)]) h->rehash[size_t(c)] = 1;
+        mark_all_small(h);
+    }
+    for (int c = 0; c < 9; c++)
+        if (!np.same_chain_jobs(h->plan, c)) h->rehash[size_t(c)] = 1;
+    h->plan = std::move(np);
+    h->outputs = outs;
+    return B200_SUCCESS;
 }
 }  // namespace
 
@@ -258,46 +402,42 @@ int32_t b200_state_upload_deneb(const uint8_t* ssz, size_t len, int32_t preset, 
     if (rc) return rc;
     if (!ssz || !out_handle) return B200_ERR_BAD_ARG;
     std::unique_ptr<b200_state> h(new b200_state());
+    if (!parse_beacon_state(ssz, len, preset, h->so)) { e.last_error = "malformed deneb BeaconState SSZ"; return B200_ERR_SSZ_MALFORMED; }
+    h->len = len; h->preset = preset;
+    for (int f = 0; f < 5; f++) h->cap[f] = big_count(h.get(), f) + headroom(big_count(h.get(), f));
     {
         SszPlan first;  // reads the caller's buffer
         std::vector<uint32_t> outs;
-        rc = build_beacon_state_plan(first, ssz, len, preset, outs);
+        rc = build_beacon_state_plan(first, ssz, len, preset, outs, h->cap);
         if (rc) { e.last_error = "malformed deneb BeaconState SSZ"; return rc; }
         uint8_t root[32];
         rc = first.run(e, h->arena, h->fields, h->planbuf, COPY_ALL, outs, root);  // uploads + first hash
         if (rc) return rc;  // ~b200_state releases the device buffers
     }
     // keep what is needed to re-plan without the caller's buffer: the serialization minus the big lists
-    if (!parse_beacon_state(ssz, len, preset, h->so)) return B200_ERR_SSZ_MALFORMED;
-    h->len = len; h->preset = preset;
-    h->shadow = static_cast<uint8_t*>(calloc(len ? len : 1, 1));
+    h->shadow_cap = shadow_bytes_for(h.get());
+    h->shadow = static_cast<uint8_t*>(calloc(h->shadow_cap, 1));
     if (!h->shadow) { e.last_error = "out of host memory for the state shadow"; return B200_ERR_CUDA; }
     memcpy(h->shadow, ssz, h->so.var[2]);
     memcpy(h->shadow + h->so.var[7], ssz + h->so.var[7], len - h->so.var[7]);
-    // page-lock the two populated ranges (a few MB) so that re-staging a patched small field is a real async DMA
-    h->pinned_head = cudaHostRegister(h->shadow, h->so.var[2], cudaHostRegisterDefault) == cudaSuccess;
-    h->pinned_tail = cudaHostRegister(h->shadow + h->so.var[7], len - h->so.var[7], cudaHostRegisterDefault) == cudaSuccess;
-    cudaGetLastError();  // registration is an optimisation: pageable copies work too
-    rc = build_beacon_state_plan(h->plan, h->shadow, len, preset, h->outputs);  // same layout: it depends on lengths only
+    // page-lock the populated ranges (a few MB) so that re-staging a patched small field is a real async DMA
+    pin_shadow(h.get(), true);
+    rc = build_beacon_state_plan(h->plan, h->shadow, len, preset, h->outputs, h->cap);  // same layout: lengths and caps
     if (rc) return rc;
     h->uploaded = true;
     *out_handle = h.release();
     return B200_SUCCESS;
 }
 
-// pending small-field updates: re-plan from the shadow (same arena / field layout, fresh small leaves)
+// pending small-field updates or reshapes: re-plan from the shadow (the chains stay where they are; fresh small leaves,
+// lengths and finisher ops)
 static int32_t replan_if_small_dirty(Engine& e, b200_state* h) {
     if (!h->small_dirty) return B200_SUCCESS;
     SszPlan np;
     std::vector<uint32_t> outs;
-    int32_t rc = build_beacon_state_plan(np, h->shadow, h->len, h->preset, outs);
+    int32_t rc = build_beacon_state_plan(np, h->shadow, h->len, h->preset, outs, h->cap);
     if (rc) return rc;
-    if (np.arena_nodes() != h->plan.arena_nodes() || np.field_bytes() != h->plan.field_bytes() || outs != h->outputs) {
-        e.last_error = "state root: plan layout changed";
-        return B200_ERR_BAD_ARG;
-    }
-    h->plan = std::move(np);
-    return B200_SUCCESS;
+    return adopt_plan(e, h, np, outs);
 }
 
 int32_t b200_state_root(b200_state* h, uint8_t out[32]) {
@@ -314,6 +454,7 @@ int32_t b200_state_root(b200_state* h, uint8_t out[32]) {
                      nullptr, nullptr, &h->small_ranges);
     if (rc) return rc;
     for (auto& d : h->dirty) d.clear();  // a full re-hash covers every dirty path
+    std::fill(h->rehash.begin(), h->rehash.end(), 0);
     h->small_dirty = false;
     h->small_ranges.clear();
     return B200_SUCCESS;
@@ -391,7 +532,7 @@ int32_t b200_state_update_bytes(b200_state* h, uint64_t ssz_offset, const uint8_
             restore_small(0, h->so.var[2], pos);
             restore_small(h->so.var[7], h->len, pos);
             // (the ranges stay recorded: re-copying unchanged bytes is harmless)
-            e.last_error = "state_update_bytes: the update changes a variable-size field's offset or length; re-upload instead";
+            e.last_error = "state_update_bytes: the update changes a variable-size field's offset or length; use state_append_elements / state_set_field";
             return B200_ERR_BAD_ARG;
         }
         h->small_dirty = true;
@@ -419,6 +560,105 @@ int32_t b200_state_update_bytes(b200_state* h, uint64_t ssz_offset, const uint8_
     return B200_SUCCESS;
 }
 
+// Field ids of the reshaping calls beyond the five big lists (include/b200_consensus.h)
+static constexpr int32_t kFieldVotes = B200_FIELD_ETH1_DATA_VOTES, kFieldSummaries = B200_FIELD_HISTORICAL_SUMMARIES,
+                         kFieldHeader = B200_FIELD_LATEST_EXECUTION_PAYLOAD_HEADER;
+
+// append to a big list: shadow offsets, then (past the capacity) relocation on the device, then the appended bytes H2D
+static int32_t append_big(Engine& e, b200_state* h, int f, const uint8_t* values, size_t n) {
+    const uint64_t old_n = big_count(h, f), new_n = old_n + n;
+    if (n > kRegistryLimit || new_n > kRegistryLimit) { e.last_error = "state_append_elements: beyond the list limit"; return B200_ERR_LIMIT; }
+    const uint32_t elem = kBigElem[f];
+    if (uint64_t(n) * elem > 0xffffffffull) { e.last_error = "state_append_elements: the serialization would exceed 4 GiB"; return B200_ERR_LIMIT; }
+    const size_t old_bytes = size_t(old_n) * elem, new_bytes = size_t(new_n) * elem;
+    int32_t rc = reshape_shadow(e, h, kBigVar[f], new_bytes);
+    if (rc) return rc;
+    auto undo = [&]() { reshape_shadow(e, h, kBigVar[f], old_bytes); reparse(h); };
+    if (!reparse(h)) { undo(); return B200_ERR_SSZ_MALFORMED; }
+    if (new_n > h->cap[f]) {   // relocate the list (and re-place the chains after it) with fresh headroom
+        const uint64_t old_cap = h->cap[f];
+        h->cap[f] = new_n + headroom(new_n);
+        SszPlan np;
+        std::vector<uint32_t> outs;
+        rc = build_beacon_state_plan(np, h->shadow, h->len, h->preset, outs, h->cap);
+        if (!rc) rc = adopt_plan(e, h, np, outs);
+        if (rc) { h->cap[f] = old_cap; undo(); return rc; }
+    }
+    uint64_t field_off = 0; size_t staged = 0;
+    if (!h->plan.chain_field(f, &field_off, &staged)) { undo(); return B200_ERR_BAD_ARG; }
+    B200_CUDA_TRY(e.staging.reserve(n * elem));
+    memcpy(e.staging.p, values, n * elem);
+    B200_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(h->fields.p) + field_off + old_bytes, e.staging.p, n * elem,
+                                  cudaMemcpyHostToDevice, e.stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+    // appended inputs are dirty; the old ragged last chunk is among them when the first appended element shares it
+    for (uint64_t u = big_input_of(f, old_n); u <= big_input_of(f, new_n - 1); u++) h->dirty[f].push_back(uint32_t(u));
+    // new length mix-in and finisher ops; the finisher nodes of the lists' tops are allocated ahead of the small fields'
+    // arena levels, so those move with them and are re-hashed
+    mark_all_small(h);
+    return B200_SUCCESS;
+}
+
+// replace small variable-size field k (StateOffsets::var index) of the shadow with `len` bytes
+static int32_t set_small(Engine& e, b200_state* h, int k, const uint8_t* data, size_t len) {
+    const std::vector<uint8_t> saved(h->shadow + h->so.var[k], h->shadow + h->so.var[k + 1]);
+    int32_t rc = reshape_shadow(e, h, k, len);
+    if (rc) return rc;
+    if (len) memcpy(h->shadow + h->so.var[k], data, len);
+    if (!reparse(h)) {
+        reshape_shadow(e, h, k, saved.size());
+        if (!saved.empty()) memcpy(h->shadow + h->so.var[k], saved.data(), saved.size());
+        reparse(h);
+        e.last_error = "state_set_field: malformed encoding";
+        return B200_ERR_SSZ_MALFORMED;
+    }
+    mark_all_small(h);
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_append_elements(b200_state* h, int32_t field, const uint8_t* values, size_t n) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!h || !h->uploaded || h->sharded || (n && !values)) return B200_ERR_BAD_ARG;
+    if (field >= 0 && field <= 4) return n ? append_big(e, h, field, values, n) : B200_SUCCESS;
+    if (field != kFieldVotes && field != kFieldSummaries) { e.last_error = "state_append_elements: unknown field"; return B200_ERR_BAD_ARG; }
+    if (!n) return B200_SUCCESS;
+    const int k = field == kFieldVotes ? 1 : 8;
+    const size_t elem = field == kFieldVotes ? 72 : 64;
+    const uint64_t limit = field == kFieldVotes ? eth1_data_votes_bound(h->preset) : historical_roots_limit(h->preset);
+    const size_t old_bytes = h->so.var[k + 1] - h->so.var[k];
+    if (n > limit || old_bytes / elem + n > limit) { e.last_error = "state_append_elements: beyond the list limit"; return B200_ERR_LIMIT; }
+    std::vector<uint8_t> buf(old_bytes + n * elem);
+    memcpy(buf.data(), h->shadow + h->so.var[k], old_bytes);
+    memcpy(buf.data() + old_bytes, values, n * elem);
+    return set_small(e, h, k, buf.data(), buf.size());
+}
+
+int32_t b200_state_set_field(b200_state* h, int32_t field, const uint8_t* ssz, size_t len) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!h || !h->uploaded || h->sharded || (len && !ssz)) return B200_ERR_BAD_ARG;
+    if (field == kFieldVotes) {
+        if (len % 72) { e.last_error = "state_set_field: eth1_data_votes not a multiple of 72 bytes"; return B200_ERR_SSZ_MALFORMED; }
+        if (len / 72 > eth1_data_votes_bound(h->preset)) { e.last_error = "state_set_field: beyond ETH1_DATA_VOTES_BOUND"; return B200_ERR_LIMIT; }
+        return set_small(e, h, 1, ssz, len);
+    }
+    if (field == kFieldHeader) {
+        // 584 fixed bytes whose only offset (extra_data, at byte 436) is 584, then 0..32 bytes of extra_data
+        if (len < 584 || len > 584 + 32 || (uint32_t(ssz[436]) | uint32_t(ssz[437]) << 8 | uint32_t(ssz[438]) << 16 | uint32_t(ssz[439]) << 24) != 584) {
+            e.last_error = "state_set_field: malformed ExecutionPayloadHeader";
+            return B200_ERR_SSZ_MALFORMED;
+        }
+        return set_small(e, h, 7, ssz, len);
+    }
+    e.last_error = "state_set_field: unknown field";
+    return B200_ERR_BAD_ARG;
+}
+
 int32_t b200_state_root_incremental(b200_state* h, uint8_t out[32]) {
     Engine& e = engine();
     Guard g(e);
@@ -434,9 +674,10 @@ int32_t b200_state_root_incremental(b200_state* h, uint8_t out[32]) {
         dirty[size_t(f)].erase(std::unique(dirty[size_t(f)].begin(), dirty[size_t(f)].end()), dirty[size_t(f)].end());
     }
     rc = h->plan.run(e, h->arena, h->fields, h->planbuf, h->small_dirty ? COPY_SMALL_ONLY : COPY_NONE, h->outputs, out,
-                     &dirty, &h->selbuf, &h->small_ranges);
+                     &dirty, &h->selbuf, &h->small_ranges, &h->rehash);
     if (rc) return rc;
     for (auto& d : h->dirty) d.clear();
+    std::fill(h->rehash.begin(), h->rehash.end(), 0);
     h->small_dirty = false;
     h->small_ranges.clear();
     return B200_SUCCESS;

@@ -78,12 +78,12 @@ uint32_t SszPlan::merkle_small(std::vector<uint32_t> nodes, int level, int depth
 uint32_t SszPlan::container(const std::vector<uint32_t>& field_roots) {
     return merkle_small(field_roots, 0, depth_for(field_roots.size()));
 }
-uint64_t SszPlan::stage_field(const uint8_t* src, size_t nbytes) {
+uint64_t SszPlan::stage_field(const uint8_t* src, size_t nbytes, size_t reserve_bytes) {
     uint64_t off = (field_next_ + 255) & ~uint64_t(255);
-    size_t padded = ((nbytes + 31) & ~size_t(31)) + 32;
+    size_t padded = ((std::max(nbytes, reserve_bytes) + 31) & ~size_t(31)) + 32;
     field_next_ = off + padded;
-    if (nbytes) {
-        copies_.push_back(HostCopy{src, nbytes, off, padded - nbytes, false, cur_chain_});
+    if (nbytes || reserve_bytes) {
+        copies_.push_back(HostCopy{src, nbytes, off, padded - nbytes, false, cur_chain_, reserve_bytes != 0});
         if (cur_chain_ >= 0) chains_[size_t(cur_chain_)].copy = int(copies_.size()) - 1;
     }
     return off;
@@ -106,54 +106,116 @@ bool SszPlan::chain_field(int c, uint64_t* field_off, size_t* nbytes) const {
     *field_off = hc.field_off; *nbytes = hc.nbytes;
     return true;
 }
-
-uint32_t SszPlan::wide_nodes(PSrc src, bool raw, uint64_t n, int level, int depth_target, size_t s) {
-    if (n == 0) return zero(depth_target);
-    while (n > kHandoff && level < depth_target) {
-        uint32_t nlev = uint32_t(std::min(3, depth_target - level));
-        uint64_t n_out = (n + (uint64_t(1) << nlev) - 1) >> nlev;
-        PJob j;
-        j.type = JOB_REDUCE; j.src = src; j.dst = arena_alloc(n_out); j.n_in = n;
-        j.level = uint32_t(level); j.nlev = nlev; j.raw = raw ? 1 : 0;
-        add_job(s++, j);
-        src.in_arena = true; src.off = j.dst; raw = false;
-        n = n_out; level += int(nlev);
+size_t SszPlan::chain_region_bytes(int c) const {
+    if (c < 0 || size_t(c) >= chains_.size() || chains_[size_t(c)].copy < 0) return 0;
+    const HostCopy& hc = copies_[size_t(chains_[size_t(c)].copy)];
+    return hc.nbytes + hc.zero_tail;
+}
+bool SszPlan::same_chain_layout(const SszPlan& o, int c) const {
+    if (size_t(c) >= chains_.size() || size_t(c) >= o.chains_.size()) return false;
+    uint64_t a = 0, b = 0; size_t na = 0, nb = 0;
+    const bool sa = chain_field(c, &a, &na), sb = o.chain_field(c, &b, &nb);
+    return sa == sb && a == b && chain_region_bytes(c) == o.chain_region_bytes(c) && chain_arena(c) == o.chain_arena(c);
+}
+bool SszPlan::same_chain_jobs(const SszPlan& o, int c) const {
+    if (size_t(c) >= chains_.size() || size_t(c) >= o.chains_.size()) return false;
+    const auto& x = chains_[size_t(c)].jobs;
+    const auto& y = o.chains_[size_t(c)].jobs;
+    if (x.size() != y.size()) return false;
+    // places relative to the chain's own field region and first arena range: a relocated chain compares equal
+    auto bases = [c](const SszPlan& p, uint64_t* fb, uint64_t* ab) {
+        size_t nb = 0;
+        *fb = 0; p.chain_field(c, fb, &nb);
+        *ab = p.chains_[size_t(c)].arena.empty() ? 0 : p.chains_[size_t(c)].arena[0].first;
+    };
+    uint64_t fa, aa, fb, ab;
+    bases(*this, &fa, &aa);
+    bases(o, &fb, &ab);
+    for (size_t k = 0; k < x.size(); k++) {
+        const PJob& a = chain_job(c, k);
+        const PJob& b = o.chain_job(c, k);
+        const uint64_t sa = a.src.off - (a.src.in_arena ? aa : fa), sb = b.src.off - (b.src.in_arena ? ab : fb);
+        if (x[k].first != y[k].first || a.type != b.type || a.src.in_arena != b.src.in_arena || sa != sb ||
+            a.dst - aa != b.dst - ab || a.level != b.level || a.nlev != b.nlev || a.raw != b.raw)
+            return false;
     }
-    if (!src.in_arena) {  // small raw input: convert to word form on the device
+    return true;
+}
+
+Handoff SszPlan::reduce_to_handoff(PSrc src, bool raw, uint64_t n, int level, int depth_target, size_t s, uint64_t cap) {
+    Handoff h;
+    h.depth = depth_target;
+    const bool reserve = cap != 0;
+    if (!reserve) cap = n;
+    if (n == 0 && !reserve) return h;
+    const bool raw_src = !src.in_arena;
+    // levels are sized for `cap` inputs; the jobs reduce the n actual ones (a prefix of the same level sequence, since
+    // the levels folded per job depend on the tree level only)
+    uint64_t c = cap;
+    int lc = level;
+    while (c > kHandoff && lc < depth_target) {
+        const uint32_t nlev = uint32_t(std::min(3, depth_target - lc));
+        const uint64_t c_out = (c + (uint64_t(1) << nlev) - 1) >> nlev;
+        const uint64_t dst = arena_alloc(c_out);
+        if (n > kHandoff) {
+            PJob j;
+            j.type = JOB_REDUCE; j.src = src; j.dst = dst; j.n_in = n;
+            j.level = uint32_t(lc); j.nlev = nlev; j.raw = raw ? 1 : 0;
+            add_job(s++, j);
+            src.in_arena = true; src.off = dst; raw = false;
+            n = (n + (uint64_t(1) << nlev) - 1) >> nlev;
+            level = lc + int(nlev);
+        }
+        c = c_out; lc += int(nlev);
+    }
+    const uint64_t conv = (reserve && raw_src) ? arena_alloc(kHandoff) : 0;
+    if (!src.in_arena && n) {  // small raw input: convert to word form on the device
         PJob j;
-        j.type = JOB_REDUCE; j.src = src; j.dst = arena_alloc(n); j.n_in = n;
+        j.type = JOB_REDUCE; j.src = src; j.dst = reserve ? conv : arena_alloc(n); j.n_in = n;
         j.level = uint32_t(level); j.nlev = 0; j.raw = raw ? 1 : 0;
         add_job(s++, j);
         src.in_arena = true; src.off = j.dst;
     }
     // n > kHandoff can only remain if level == depth_target, which means n == 1 by the limit check upstream
-    std::vector<uint32_t> nodes;
-    for (uint64_t i = 0; i < n; i++) nodes.push_back(uint32_t(src.off + i));
-    return merkle_small(nodes, level, depth_target);
+    for (uint64_t i = 0; i < n; i++) h.nodes.push_back(uint32_t(src.off + i));
+    h.level = level;
+    return h;
 }
-uint32_t SszPlan::wide_chunks(uint64_t field_off, uint64_t n_chunks, int depth_target) {
+uint32_t SszPlan::wide_nodes(PSrc src, bool raw, uint64_t n, int level, int depth_target, size_t s) {
+    return finish(reduce_to_handoff(src, raw, n, level, depth_target, s, 0));
+}
+Handoff SszPlan::chunks_to_handoff(uint64_t field_off, uint64_t n_chunks, int depth_target, uint64_t cap_chunks) {
     PSrc s; s.in_arena = false; s.off = field_off;
     cur_copy_ = copy_of(field_off);
-    const uint32_t r = wide_nodes(s, true, n_chunks, 0, depth_target, 0);
+    Handoff h = reduce_to_handoff(s, true, n_chunks, 0, depth_target, 0, cap_chunks);
     cur_copy_ = -1;
-    return r;
+    return h;
+}
+uint32_t SszPlan::wide_chunks(uint64_t field_off, uint64_t n_chunks, int depth_target) {
+    return finish(chunks_to_handoff(field_off, n_chunks, depth_target));
+}
+Handoff SszPlan::records_to_handoff(uint32_t type, uint64_t field_off, uint64_t n, int depth_target, uint64_t cap) {
+    if (n == 0 && cap == 0) { Handoff h; h.depth = depth_target; return h; }
+    cur_copy_ = copy_of(field_off);
+    const uint64_t dst = arena_alloc(cap ? cap : n);
+    if (n) {
+        PJob j;
+        j.type = type; j.src.in_arena = false; j.src.off = field_off; j.dst = dst; j.n_in = n;
+        j.copy = cur_copy_;
+        if (type == JOB_VALIDATORS) {
+            j.chain = cur_chain_;
+            validator_jobs_.push_back(j);
+            if (cur_chain_ >= 0) chains_[size_t(cur_chain_)].jobs.emplace_back(-1, validator_jobs_.size() - 1);
+            for (auto& c : copies_) if (c.field_off == field_off) c.validators = true;
+        } else add_job(0, j);
+    }
+    PSrc s; s.in_arena = true; s.off = dst;
+    Handoff h = reduce_to_handoff(s, false, n, 0, depth_target, 1, cap);
+    cur_copy_ = -1;
+    return h;
 }
 uint32_t SszPlan::wide_records(uint32_t type, uint64_t field_off, uint64_t n, int depth_target) {
-    if (n == 0) return zero(depth_target);
-    cur_copy_ = copy_of(field_off);
-    PJob j;
-    j.type = type; j.src.in_arena = false; j.src.off = field_off; j.dst = arena_alloc(n); j.n_in = n;
-    j.copy = cur_copy_;
-    if (type == JOB_VALIDATORS) {
-        j.chain = cur_chain_;
-        validator_jobs_.push_back(j);
-        if (cur_chain_ >= 0) chains_[size_t(cur_chain_)].jobs.emplace_back(-1, validator_jobs_.size() - 1);
-        for (auto& c : copies_) if (c.field_off == field_off) c.validators = true;
-    } else add_job(0, j);
-    PSrc s; s.in_arena = true; s.off = j.dst;
-    const uint32_t r = wide_nodes(s, false, n, 0, depth_target, 1);
-    cur_copy_ = -1;
-    return r;
+    return finish(records_to_handoff(type, field_off, n, depth_target));
 }
 uint32_t SszPlan::wide_pubkeys_with_extra(uint64_t field_off, uint64_t n, int depth_target, uint32_t* extra) {
     cur_copy_ = copy_of(field_off);
@@ -199,8 +261,10 @@ int32_t ensure_zero_nodes(Engine& e) {
 int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, CopyMode copy,
                      const std::vector<uint32_t>& outputs, uint8_t* out,
                      const std::vector<std::vector<uint32_t>>* dirty, DevBuf* selbuf,
-                     const std::vector<std::pair<const uint8_t*, const uint8_t*>>* changed_host_ranges) {
+                     const std::vector<std::pair<const uint8_t*, const uint8_t*>>* changed_host_ranges,
+                     const std::vector<char>* rehash) {
     const bool sparse = dirty != nullptr;
+    auto full_chain = [&](int c) { return rehash && c >= 0 && size_t(c) < rehash->size() && (*rehash)[size_t(c)]; };
     if (sparse && (dirty->size() != chains_.size() || !selbuf || copy == COPY_ALL)) return B200_ERR_BAD_ARG;
     if (small_words_.size() / 8 > kSmallCap) { e.last_error = "ssz plan: too many small leaves"; return B200_ERR_BAD_ARG; }
     int32_t rc = ensure_zero_nodes(e);
@@ -235,6 +299,7 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
     std::vector<Launch> launches;
     if (sparse) {
         for (size_t c = 0; c < chains_.size(); c++) {
+            if (full_chain(int(c))) continue;   // dense below
             std::vector<uint32_t> cur = (*dirty)[c];
             size_t level = 0;
             for (auto& ref : chains_[c].jobs) {
@@ -385,8 +450,8 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
                 for (auto& r : *changed_host_ranges) hit = hit || (r.first < c.src + c.nbytes && c.src < r.second);
                 if (!hit) continue;
             }
-            B200_CUDA_TRY(cudaMemcpyAsync(d_fields + c.field_off, c.src, c.nbytes, cudaMemcpyHostToDevice, cs));
-            if (c.nbytes % 32)
+            if (c.nbytes) B200_CUDA_TRY(cudaMemcpyAsync(d_fields + c.field_off, c.src, c.nbytes, cudaMemcpyHostToDevice, cs));
+            if (c.nbytes % 32 || c.reserved)
                 B200_CUDA_TRY(cudaMemsetAsync(d_fields + c.field_off + c.nbytes, 0, c.zero_tail, cs));
         }
         B200_CUDA_TRY(cudaEventRecord(e.ev_copy[16], cs));
@@ -414,7 +479,7 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
                     launch_validators(j, s);
                     e.launches++;
                 }
-                if (c.nbytes % 32) {
+                if (c.nbytes % 32 || c.reserved) {
                     B200_CUDA_TRY(cudaMemsetAsync(d_fields + c.field_off + c.nbytes, 0, c.zero_tail, cs));
                     B200_CUDA_TRY(cudaEventRecord(e.ev_copy[16], cs));
                     B200_CUDA_TRY(cudaStreamWaitEvent(s, e.ev_copy[16], 0));
@@ -463,7 +528,7 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
     // is the critical path, and the join adds two event waits.)
     if (!validators_launched)
         for (auto& pj : validator_jobs_) {
-            if (sparse && pj.chain >= 0) continue;
+            if (sparse && pj.chain >= 0 && !full_chain(pj.chain)) continue;
             launch_validators(materialize(pj), s); e.launches++;
         }
     // incremental mode: the arena is the resident state's own, so the outputs of a dense job whose staged field did not
@@ -474,7 +539,7 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
             for (auto& r : *changed_host_ranges)
                 if (r.first < copies_[ci].src + copies_[ci].nbytes && copies_[ci].src < r.second) copy_changed[ci] = 1;
     launch_stages([&](const PJob& pj) {
-        if (sparse && pj.chain >= 0) return false;
+        if (sparse && pj.chain >= 0) return full_chain(pj.chain);
         if (sparse && pj.copy >= 0 && !copy_changed[size_t(pj.copy)]) return false;
         if (pipelined && !from_validators(pj)) return false;   // already launched, under the Validator list's transfer
         return true;
@@ -536,6 +601,9 @@ inline uint32_t le32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16
 inline uint64_t le64(const uint8_t* p) { return uint64_t(le32(p)) | (uint64_t(le32(p + 4)) << 32); }
 }  // namespace
 
+uint64_t eth1_data_votes_bound(int preset) { return kPresets[preset ? 1 : 0].eth1_data_votes_bound; }
+uint64_t historical_roots_limit(int preset) { return kPresets[preset ? 1 : 0].historical_roots_limit; }
+
 bool parse_beacon_state(const uint8_t* s, size_t len, int preset, StateOffsets& so) {
     if (preset < 0 || preset > 1) return false;
     const Preset& P = kPresets[preset];
@@ -546,25 +614,25 @@ bool parse_beacon_state(const uint8_t* s, size_t len, int preset, StateOffsets& 
     size_t o = 8 + 32 + 8 + 16 + 112;
     so.block_roots = o; o += 32 * P.slots_per_historical_root;
     so.state_roots = o; o += 32 * P.slots_per_historical_root;
-    so.var[0] = le32(s + o); o += 4;  // historical_roots
+    so.var_word[0] = uint32_t(o); so.var[0] = le32(s + o); o += 4;  // historical_roots
     so.eth1_data = o; o += 72;
-    so.var[1] = le32(s + o); o += 4;  // eth1_data_votes
+    so.var_word[1] = uint32_t(o); so.var[1] = le32(s + o); o += 4;  // eth1_data_votes
     so.eth1_deposit_index = o; o += 8;
-    so.var[2] = le32(s + o); o += 4;  // validators
-    so.var[3] = le32(s + o); o += 4;  // balances
+    so.var_word[2] = uint32_t(o); so.var[2] = le32(s + o); o += 4;  // validators
+    so.var_word[3] = uint32_t(o); so.var[3] = le32(s + o); o += 4;  // balances
     so.randao_mixes = o; o += 32 * P.epochs_per_historical_vector;
     so.slashings = o; o += 8 * P.epochs_per_slashings_vector;
-    so.var[4] = le32(s + o); o += 4;  // previous_epoch_participation
-    so.var[5] = le32(s + o); o += 4;  // current_epoch_participation
+    so.var_word[4] = uint32_t(o); so.var[4] = le32(s + o); o += 4;  // previous_epoch_participation
+    so.var_word[5] = uint32_t(o); so.var[5] = le32(s + o); o += 4;  // current_epoch_participation
     so.justification_bits = o; o += 1;
     so.checkpoints = o; o += 120;
-    so.var[6] = le32(s + o); o += 4;  // inactivity_scores
+    so.var_word[6] = uint32_t(o); so.var[6] = le32(s + o); o += 4;  // inactivity_scores
     so.current_sync_committee = o; o += 48 * P.sync_committee_size + 48;
     so.next_sync_committee = o; o += 48 * P.sync_committee_size + 48;
-    so.var[7] = le32(s + o); o += 4;  // latest_execution_payload_header
+    so.var_word[7] = uint32_t(o); so.var[7] = le32(s + o); o += 4;  // latest_execution_payload_header
     so.next_withdrawal_index = o; o += 8;
     so.next_withdrawal_validator_index = o; o += 8;
-    so.var[8] = le32(s + o); o += 4;  // historical_summaries
+    so.var_word[8] = uint32_t(o); so.var[8] = le32(s + o); o += 4;  // historical_summaries
     so.var[9] = uint32_t(len);
     so.fixed = fixed;
     if (o != fixed || so.var[0] != fixed) return false;
@@ -581,10 +649,10 @@ bool parse_beacon_state(const uint8_t* s, size_t len, int preset, StateOffsets& 
 }
 
 // Everything except the five big lists; `big[5]` = their roots (already length-mixed).
-// `chain_vectors`: the four big fixed-size vectors become chains 5..8 (in this order: block_roots, state_roots,
-// randao_mixes, slashings) so that a resident state can re-hash only their dirty paths too.
+// `vec` (optional): roots of the four big fixed-size vectors (block_roots, state_roots, randao_mixes, slashings), planned
+// by the caller as chains 5..8; without it they are staged and reduced here (as chains 5..8 when `chain_vectors`).
 static uint32_t assemble_state(SszPlan& p, const uint8_t* s, const StateOffsets& so, const Preset& P,
-                               const uint32_t big[5], bool chain_vectors = false) {
+                               const uint32_t big[5], const uint32_t* vec = nullptr, bool chain_vectors = false) {
     std::vector<uint32_t> f(28);
     auto sz = [&](int i) { return size_t(so.var[i + 1] - so.var[i]); };
     f[0] = p.leaf_bytes(s + 0, 8);
@@ -593,11 +661,15 @@ static uint32_t assemble_state(SszPlan& p, const uint8_t* s, const StateOffsets&
     f[3] = p.container({p.leaf_bytes(s + 48, 4), p.leaf_bytes(s + 52, 4), p.leaf_bytes(s + 56, 8)});
     f[4] = p.container({p.leaf_bytes(s + 64, 8), p.leaf_bytes(s + 72, 8), p.leaf(s + 80), p.leaf(s + 112), p.leaf(s + 144)});
     int d_hist = depth_for(P.slots_per_historical_root);
-    if (chain_vectors) p.begin_chain();
-    f[5] = p.wide_chunks(p.stage_field(s + so.block_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
-    if (chain_vectors) p.begin_chain();
-    f[6] = p.wide_chunks(p.stage_field(s + so.state_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
-    if (chain_vectors) p.end_chain();
+    if (vec) {
+        f[5] = vec[0]; f[6] = vec[1]; f[13] = vec[2]; f[14] = vec[3];
+    } else {
+        if (chain_vectors) p.begin_chain();
+        f[5] = p.wide_chunks(p.stage_field(s + so.block_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
+        if (chain_vectors) p.begin_chain();
+        f[6] = p.wide_chunks(p.stage_field(s + so.state_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
+        if (chain_vectors) p.end_chain();
+    }
     f[7] = p.mix_in_length(p.wide_chunks(p.stage_field(s + so.var[0], sz(0)), sz(0) / 32, depth_for(P.historical_roots_limit)), sz(0) / 32);
     {
         const uint8_t* e = s + so.eth1_data;
@@ -607,11 +679,13 @@ static uint32_t assemble_state(SszPlan& p, const uint8_t* s, const StateOffsets&
     f[10] = p.leaf_bytes(s + so.eth1_deposit_index, 8);
     f[11] = big[0];
     f[12] = big[1];
-    if (chain_vectors) p.begin_chain();
-    f[13] = p.wide_chunks(p.stage_field(s + so.randao_mixes, 32 * P.epochs_per_historical_vector), P.epochs_per_historical_vector, depth_for(P.epochs_per_historical_vector));
-    if (chain_vectors) p.begin_chain();
-    f[14] = p.wide_chunks(p.stage_field(s + so.slashings, 8 * P.epochs_per_slashings_vector), P.epochs_per_slashings_vector / 4, depth_for(P.epochs_per_slashings_vector / 4));
-    if (chain_vectors) p.end_chain();
+    if (!vec) {
+        if (chain_vectors) p.begin_chain();
+        f[13] = p.wide_chunks(p.stage_field(s + so.randao_mixes, 32 * P.epochs_per_historical_vector), P.epochs_per_historical_vector, depth_for(P.epochs_per_historical_vector));
+        if (chain_vectors) p.begin_chain();
+        f[14] = p.wide_chunks(p.stage_field(s + so.slashings, 8 * P.epochs_per_slashings_vector), P.epochs_per_slashings_vector / 4, depth_for(P.epochs_per_slashings_vector / 4));
+        if (chain_vectors) p.end_chain();
+    }
     f[15] = big[2];
     f[16] = big[3];
     f[17] = p.leaf_bytes(s + so.justification_bits, 1);
@@ -669,26 +743,59 @@ static void slice_of(uint64_t n, int world, int rank, uint64_t* first, uint64_t*
     *first = lo; *count = hi - lo; *k = kk;
 }
 
-int32_t build_beacon_state_plan(SszPlan& p, const uint8_t* s, size_t len, int preset, std::vector<uint32_t>& outputs) {
+int32_t build_beacon_state_plan(SszPlan& p, const uint8_t* s, size_t len, int preset, std::vector<uint32_t>& outputs,
+                                const uint64_t* caps) {
     StateOffsets so;
     if (!parse_beacon_state(s, len, preset, so)) return B200_ERR_SSZ_MALFORMED;
     const Preset& P = kPresets[preset];
     auto sz = [&](int i) { return size_t(so.var[i + 1] - so.var[i]); };
-    uint32_t big[5];
-    int d_reg = depth_for(P.validator_registry_limit);
-    // the five big lists are chains 0..4 (B200_FIELD_* in the C ABI): their jobs can re-hash dirty paths only
+    const int d_reg = depth_for(P.validator_registry_limit);
+    constexpr uint64_t kElem[5] = {121, 8, 1, 1, 8};
+    const int depth[5] = {d_reg, d_reg - 2, d_reg - 5, d_reg - 5, d_reg - 2};
+    if (!caps) {   // one-shot: the staging order the pipelined Validator upload is tuned with (same chains, same root)
+        uint32_t big[5];
+        for (int q = 0; q < 5; q++) {
+            const size_t nb = sz(2 + q);
+            p.begin_chain();
+            const uint64_t off = p.stage_field(s + so.var[2 + q], nb);
+            const uint32_t r = q == 0 ? p.wide_records(JOB_VALIDATORS, off, nb / 121, depth[0]) : p.wide_chunks(off, (nb + 31) / 32, depth[q]);
+            big[q] = p.mix_in_length(r, nb / kElem[q]);
+        }
+        p.end_chain();
+        outputs.assign(1, assemble_state(p, s, so, P, big, nullptr, true));
+        return B200_SUCCESS;
+    }
+    // the five big lists are chains 0..4 (B200_FIELD_* in the C ABI), the four big vectors chains 5..8 (block_roots,
+    // state_roots, randao_mixes, slashings): their jobs can re-hash dirty paths only.  All nine are staged and given their
+    // arena levels first, so that their places do not depend on any small variable-size field.
+    Handoff hb[5], hv[4];
+    uint64_t len_of[5];
+    for (int q = 0; q < 5; q++) {
+        const size_t nb = sz(2 + q);
+        len_of[q] = nb / kElem[q];
+        if (caps && caps[q] < len_of[q]) return B200_ERR_BAD_ARG;
+        const uint64_t cap = caps ? caps[q] : 0;
+        p.begin_chain();
+        const uint64_t off = p.stage_field(s + so.var[2 + q], nb, size_t(cap * kElem[q]));
+        if (q == 0) hb[q] = p.records_to_handoff(JOB_VALIDATORS, off, len_of[q], depth[q], cap);
+        else hb[q] = p.chunks_to_handoff(off, (nb + 31) / 32, depth[q], (cap * kElem[q] + 31) / 32);
+    }
+    const int d_hist = depth_for(P.slots_per_historical_root);
     p.begin_chain();
-    big[0] = p.mix_in_length(p.wide_records(JOB_VALIDATORS, p.stage_field(s + so.var[2], sz(2)), sz(2) / 121, d_reg), sz(2) / 121);
+    hv[0] = p.chunks_to_handoff(p.stage_field(s + so.block_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
     p.begin_chain();
-    big[1] = p.mix_in_length(p.wide_chunks(p.stage_field(s + so.var[3], sz(3)), (sz(3) + 31) / 32, d_reg - 2), sz(3) / 8);
+    hv[1] = p.chunks_to_handoff(p.stage_field(s + so.state_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
     p.begin_chain();
-    big[2] = p.mix_in_length(p.wide_chunks(p.stage_field(s + so.var[4], sz(4)), (sz(4) + 31) / 32, d_reg - 5), sz(4));
+    hv[2] = p.chunks_to_handoff(p.stage_field(s + so.randao_mixes, 32 * P.epochs_per_historical_vector), P.epochs_per_historical_vector,
+                                depth_for(P.epochs_per_historical_vector));
     p.begin_chain();
-    big[3] = p.mix_in_length(p.wide_chunks(p.stage_field(s + so.var[5], sz(5)), (sz(5) + 31) / 32, d_reg - 5), sz(5));
-    p.begin_chain();
-    big[4] = p.mix_in_length(p.wide_chunks(p.stage_field(s + so.var[6], sz(6)), (sz(6) + 31) / 32, d_reg - 2), sz(6) / 8);
+    hv[3] = p.chunks_to_handoff(p.stage_field(s + so.slashings, 8 * P.epochs_per_slashings_vector), P.epochs_per_slashings_vector / 4,
+                                depth_for(P.epochs_per_slashings_vector / 4));
     p.end_chain();
-    outputs.assign(1, assemble_state(p, s, so, P, big, true));
+    uint32_t big[5], vec[4];
+    for (int q = 0; q < 5; q++) big[q] = p.mix_in_length(p.finish(hb[q]), len_of[q]);
+    for (int k = 0; k < 4; k++) vec[k] = p.finish(hv[k]);
+    outputs.assign(1, assemble_state(p, s, so, P, big, vec));
     return B200_SUCCESS;
 }
 

@@ -37,13 +37,22 @@ struct HostCopy {
     size_t zero_tail;  // bytes to clear after the copy (keeps the last partial chunk zero-padded)
     bool validators = false;  // the big Validator list: copied in slices so hashing overlaps the PCIe transfer
     int chain = -1;
+    bool reserved = false;    // region sized for a capacity beyond nbytes: the whole tail is cleared on upload
 };
 
 // One big list of a device-resident state: its staged bytes and the sequence of jobs that reduces them to <= kHandoff
 // nodes.  `jobs[k]` = (stage, index in that stage), stage -1 = validator_jobs_.  Job k+1 reads exactly job k's output.
+// `arena` = every node range allocated for the chain (all levels, at capacity when the list was planned with one).
 struct PChain {
     int copy = -1;
     std::vector<std::pair<int, size_t>> jobs;
+    std::vector<std::pair<uint64_t, uint64_t>> arena;  // (first node, node count)
+};
+
+// A wide list reduced to <= kHandoff nodes at `level`; SszPlan::finish() adds the finisher ops up to `depth`.
+struct Handoff {
+    std::vector<uint32_t> nodes;
+    int level = 0, depth = 0;
 };
 
 enum CopyMode { COPY_ALL = 0, COPY_NONE = 1, COPY_SMALL_ONLY = 2 };
@@ -70,13 +79,22 @@ public:
     uint32_t merkle_small(std::vector<uint32_t> nodes, int level, int depth_target);
     // container of small field roots
     uint32_t container(const std::vector<uint32_t>& field_roots);
-    // stage a host region into the field buffer (16-byte padded, 256-byte aligned)
-    uint64_t stage_field(const uint8_t* src, size_t nbytes);
+    // stage a host region into the field buffer (16-byte padded, 256-byte aligned); `reserve_bytes` > nbytes sizes the
+    // region for a list that may grow in place (the tail is zeroed when the region is uploaded)
+    uint64_t stage_field(const uint8_t* src, size_t nbytes, size_t reserve_bytes = 0);
     // root at depth_target of `n` chunks/records living in the field buffer
     uint32_t wide_chunks(uint64_t field_off, uint64_t n_chunks, int depth_target);
     uint32_t wide_records(uint32_t type, uint64_t field_off, uint64_t n, int depth_target);
     // generic: n nodes at `level`, located at src, reduced to depth_target starting at stage `s`
     uint32_t wide_nodes(PSrc src, bool raw, uint64_t n, int level, int depth_target, size_t s);
+
+    // The same two reductions without their finisher ops, so that a resident plan can allocate every chain's arena
+    // levels before any finisher node.  `cap` (> 0): inputs the arena levels are sized for (>= n, every level of a
+    // cap-input tree is allocated, plus a kHandoff-node region for the word-form conversion of a short raw list): the
+    // positions then depend on `cap` only, and a list that grows up to `cap` keeps them.
+    Handoff chunks_to_handoff(uint64_t field_off, uint64_t n_chunks, int depth_target, uint64_t cap_chunks = 0);
+    Handoff records_to_handoff(uint32_t type, uint64_t field_off, uint64_t n, int depth_target, uint64_t cap = 0);
+    uint32_t finish(const Handoff& h) { return merkle_small(h.nodes, h.level, h.depth); }
 
     // n+1 48-byte records (n vector elements + 1 extra key) hashed by one job; returns the vector root
     uint32_t wide_pubkeys_with_extra(uint64_t field_off, uint64_t n, int depth_target, uint32_t* extra);
@@ -87,6 +105,13 @@ public:
     size_t n_chains() const { return chains_.size(); }
     // device byte offset (in the field buffer) and byte length of chain c's staged list; false if the list is empty
     bool chain_field(int c, uint64_t* field_off, size_t* nbytes) const;
+    // byte size of chain c's field-buffer region (reserved capacity included) and its arena node ranges
+    size_t chain_region_bytes(int c) const;
+    const std::vector<std::pair<uint64_t, uint64_t>>& chain_arena(int c) const { return chains_[size_t(c)].arena; }
+    // chain c sits at the same field-buffer region and arena ranges in both plans
+    bool same_chain_layout(const SszPlan& o, int c) const;
+    // chain c runs the same job sequence (stages, levels, sources, destinations) in both plans; input counts may differ
+    bool same_chain_jobs(const SszPlan& o, int c) const;
 
     // ---- execution ----
     // Uploads fields (+plan) and runs; `copy`: which staged fields to copy H2D first (COPY_NONE: device-resident state,
@@ -95,10 +120,13 @@ public:
     // 32-byte chunks of a packed list): the chains' jobs then only recompute the paths above those inputs.
     // `changed_host_ranges` (COPY_SMALL_ONLY): copy only the staged fields whose host bytes intersect one of these ranges.
     // `outputs`: arena nodes to read back (32 bytes each, SSZ byte order) into `out`.
+    // `rehash` (with `dirty`, one flag per chain): these chains are re-hashed in full from their resident data instead
+    // of along dirty paths (their job sequence changed, or they were relocated).
     int32_t run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, CopyMode copy,
                 const std::vector<uint32_t>& outputs, uint8_t* out,
                 const std::vector<std::vector<uint32_t>>* dirty = nullptr, DevBuf* selbuf = nullptr,
-                const std::vector<std::pair<const uint8_t*, const uint8_t*>>* changed_host_ranges = nullptr);
+                const std::vector<std::pair<const uint8_t*, const uint8_t*>>* changed_host_ranges = nullptr,
+                const std::vector<char>* rehash = nullptr);
     bool has_exchange() const { return xch_n_ != 0; }
 
     size_t field_bytes() const { return field_next_; }
@@ -106,8 +134,17 @@ public:
     uint64_t h2d_bytes() const;
 
 private:
-    uint64_t arena_alloc(uint64_t n) { uint64_t r = arena_next_; arena_next_ += n; return r; }
+    uint64_t arena_alloc(uint64_t n) {
+        uint64_t r = arena_next_; arena_next_ += n;
+        if (cur_chain_ >= 0) chains_[size_t(cur_chain_)].arena.emplace_back(r, n);
+        return r;
+    }
     void add_job(size_t stage, const PJob& j);
+    Handoff reduce_to_handoff(PSrc src, bool raw, uint64_t n, int level, int depth_target, size_t s, uint64_t cap);
+    const PJob& chain_job(int c, size_t k) const {
+        const auto& ref = chains_[size_t(c)].jobs[k];
+        return ref.first < 0 ? validator_jobs_[ref.second] : stages_[size_t(ref.first)][ref.second];
+    }
 
     std::vector<PJob> validator_jobs_;
     std::vector<std::vector<PJob>> stages_;
@@ -143,9 +180,17 @@ struct StateOffsets {
     // historical_roots, eth1_data_votes, validators, balances, previous/current participation, inactivity_scores,
     // latest_execution_payload_header, historical_summaries, end
     uint32_t var[10] = {0};
+    uint32_t var_word[9] = {0};  // byte position of each offset word in the fixed part
 };
 bool parse_beacon_state(const uint8_t* ssz, size_t len, int preset, StateOffsets& so);
-int32_t build_beacon_state_plan(SszPlan& plan, const uint8_t* ssz, size_t len, int preset, std::vector<uint32_t>& outputs);
+// `caps` (optional, element counts of the five big lists, each >= the list's length): the lists' field regions and arena
+// levels are reserved for that many elements and are laid out, with the four big vectors, ahead of everything whose size
+// depends on a small variable-size field — a device-resident state can then grow or reshape without moving them.
+int32_t build_beacon_state_plan(SszPlan& plan, const uint8_t* ssz, size_t len, int preset, std::vector<uint32_t>& outputs,
+                                const uint64_t* caps = nullptr);
+// ETH1_DATA_VOTES_BOUND / HISTORICAL_ROOTS_LIMIT of a preset (0 mainnet, 1 minimal)
+uint64_t eth1_data_votes_bound(int preset);
+uint64_t historical_roots_limit(int preset);
 int32_t build_beacon_state_shard_plan(SszPlan& plan, const uint8_t* ssz, size_t len, int preset, int rank, int world,
                                       std::vector<uint32_t>& outputs);
 int32_t build_beacon_state_sharded_plan(SszPlan& plan, const uint8_t* ssz, size_t len, int preset, int rank, int world,

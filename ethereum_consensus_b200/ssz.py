@@ -111,6 +111,12 @@ def _count_validators(ssz, preset: str) -> int:
     return (b_off - v_off) // 121
 
 
+def _as_u8(values) -> np.ndarray:
+    if isinstance(values, (bytes, bytearray, memoryview)):
+        return np.frombuffer(bytes(values), dtype=np.uint8)
+    return np.ascontiguousarray(values).view(np.uint8).reshape(-1)
+
+
 class DeviceBeaconState:
     """A deneb BeaconState resident in HBM: upload once, `hash_tree_root()` costs kernels only."""
 
@@ -146,6 +152,41 @@ class DeviceBeaconState:
         """Overwrite bytes [ssz_offset, ssz_offset+len(data)) of the uploaded serialization (any field, same layout)."""
         buf = np.frombuffer(bytes(data), dtype=np.uint8)
         _rc(_lib.lib().b200_state_update_bytes(self._h, ssz_offset, _lib.ptr(buf), buf.size), "state_update_bytes")
+
+    # ---- shape changes: list appends, the eth1-vote reset, a new payload header (then re-hashed incrementally) ----
+    RESHAPE_FIELDS = {**FIELDS, "eth1_data_votes": (5, 72), "historical_summaries": (6, 64)}
+    SET_FIELDS = {"eth1_data_votes": 5, "latest_execution_payload_header": 7}
+
+    def append_elements(self, field: str, values) -> None:
+        """The spec's `.push`: append SSZ-encoded elements (back to back) to one of the five big lists,
+        `eth1_data_votes` (72-byte Eth1Data) or `historical_summaries` (64-byte HistoricalSummary)."""
+        fid, elem = self.RESHAPE_FIELDS[field]
+        vals = _as_u8(values)
+        if vals.size % elem:
+            raise MerkleizationError(f"{field}: {vals.size} bytes is not a multiple of the {elem}-byte element")
+        _rc(_lib.lib().b200_state_append_elements(self._h, fid, _lib.ptr(vals), vals.size // elem), "state_append_elements")
+        if fid == 0:
+            self.n_validators += vals.size // elem
+
+    def set_field(self, field: str, data) -> None:
+        """Replace `eth1_data_votes` (n x 72 bytes; empty = the voting-period reset) or
+        `latest_execution_payload_header` (its SSZ: 584 fixed bytes, then 0..32 bytes of extra_data)."""
+        vals = _as_u8(data)
+        _rc(_lib.lib().b200_state_set_field(self._h, self.SET_FIELDS[field], _lib.ptr(vals), vals.size), "state_set_field")
+
+    def add_validators(self, records, balances) -> None:
+        """A deposit batch (`add_validator_to_registry` for each): append the Validator records and their balances, and
+        zero participation flags and inactivity scores, to the five big lists."""
+        recs = _as_u8(records)
+        bal = np.ascontiguousarray(balances, dtype="<u8")
+        n = recs.size // 121
+        if recs.size % 121 or bal.size != n:
+            raise ValueError(f"add_validators: {recs.size} record bytes and {bal.size} balances do not match")
+        self.append_elements("validators", recs)
+        self.append_elements("balances", bal)
+        self.append_elements("previous_epoch_participation", np.zeros(n, np.uint8))
+        self.append_elements("current_epoch_participation", np.zeros(n, np.uint8))
+        self.append_elements("inactivity_scores", np.zeros(n, "<u8"))
 
     def hash_tree_root_incremental(self) -> bytes:
         out = _out32()

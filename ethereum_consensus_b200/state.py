@@ -32,6 +32,21 @@ assert VALIDATOR_DTYPE.itemsize == 121
 FAR_FUTURE_EPOCH = (1 << 64) - 1
 
 
+class ReshapeRefused(ValueError):
+    """A reshaping step the library refuses: `kind` is "limit" (B200_ERR_LIMIT), "malformed" (B200_ERR_SSZ_MALFORMED) or
+    "bad_arg" (B200_ERR_BAD_ARG)."""
+
+    def __init__(self, kind: str, msg: str):
+        super().__init__(msg)
+        self.kind = kind
+
+
+# element sizes of the lists `SynthState.append_elements` (and DeviceBeaconState.append_elements) take
+APPEND_ELEM = {"validators": 121, "balances": 8, "previous_epoch_participation": 1, "current_epoch_participation": 1,
+               "inactivity_scores": 8, "eth1_data_votes": 72, "historical_summaries": 64}
+VALIDATOR_REGISTRY_LIMIT = 1 << 40
+
+
 @dataclass
 class SynthState:
     preset: str
@@ -52,6 +67,64 @@ class SynthState:
     payload_header_fixed: bytes = b""          # 584 bytes incl. the extra_data offset
     extra_data: bytes = b""
     historical_summaries: np.ndarray = None    # (n,64) u8
+
+    # ---- host mirror of the device-resident state's reshaping calls (ssz.DeviceBeaconState) ----
+    def append_elements(self, field: str, values) -> None:
+        """The spec's `.push` of SSZ-encoded elements onto a list; refused exactly where the library refuses."""
+        if field not in APPEND_ELEM:
+            raise ReshapeRefused("bad_arg", f"append_elements: unknown field {field}")
+        elem = APPEND_ELEM[field]
+        raw = np.frombuffer(bytes(values), dtype=np.uint8) if isinstance(values, (bytes, bytearray, memoryview)) \
+            else np.ascontiguousarray(values).view(np.uint8).reshape(-1)
+        if raw.size % elem:
+            raise ReshapeRefused("malformed", f"{field}: {raw.size} bytes is not a multiple of {elem}")
+        P = PRESETS[self.preset]
+        limit = {"eth1_data_votes": P["ETH1_DATA_VOTES_BOUND"], "historical_summaries": P["HISTORICAL_ROOTS_LIMIT"]}.get(
+            field, VALIDATOR_REGISTRY_LIMIT)
+        cur = getattr(self, field)
+        if len(cur) + raw.size // elem > limit:
+            raise ReshapeRefused("limit", f"{field}: beyond its limit {limit}")
+        if field == "validators":
+            new = np.frombuffer(raw.tobytes(), dtype=VALIDATOR_DTYPE)
+        elif elem in (72, 64):
+            new = raw.reshape(-1, elem)
+        else:
+            new = np.frombuffer(raw.tobytes(), dtype=cur.dtype)
+        setattr(self, field, np.concatenate([cur, new]))
+
+    def set_field(self, field: str, data: bytes) -> None:
+        """Replace `eth1_data_votes` (n x 72 bytes) or `latest_execution_payload_header` (584 + 0..32 bytes)."""
+        data = bytes(data)
+        if field == "eth1_data_votes":
+            if len(data) % 72:
+                raise ReshapeRefused("malformed", "eth1_data_votes: not a multiple of 72 bytes")
+            if len(data) // 72 > PRESETS[self.preset]["ETH1_DATA_VOTES_BOUND"]:
+                raise ReshapeRefused("limit", "eth1_data_votes: beyond ETH1_DATA_VOTES_BOUND")
+            self.eth1_data_votes = np.frombuffer(data, dtype=np.uint8).reshape(-1, 72).copy()
+        elif field == "latest_execution_payload_header":
+            if not 584 <= len(data) <= 584 + 32 or int.from_bytes(data[436:440], "little") != 584:
+                raise ReshapeRefused("malformed", "latest_execution_payload_header: malformed")
+            self.payload_header_fixed, self.extra_data = data[:584], data[584:]
+        else:
+            raise ReshapeRefused("bad_arg", f"set_field: unknown field {field}")
+
+    def add_validators(self, records, balances) -> None:
+        """A deposit batch (`add_validator_to_registry` for each): records and balances appended, flags and inactivity
+        scores zero."""
+        recs = np.ascontiguousarray(records).view(np.uint8).reshape(-1)
+        bal = np.ascontiguousarray(balances, dtype="<u8")
+        n = recs.size // 121
+        if recs.size % 121 or bal.size != n:
+            raise ValueError("add_validators: records and balances do not match")
+        self.append_elements("validators", recs)
+        self.append_elements("balances", bal)
+        self.append_elements("previous_epoch_participation", np.zeros(n, np.uint8))
+        self.append_elements("current_epoch_participation", np.zeros(n, np.uint8))
+        self.append_elements("inactivity_scores", np.zeros(n, "<u8"))
+
+    def payload_header(self) -> bytes:
+        """SSZ of latest_execution_payload_header (what `set_field` takes)."""
+        return self.payload_header_fixed + self.extra_data
 
 
 def _rand_bytes(rng: np.random.Generator, n: int, width: int) -> np.ndarray:

@@ -101,7 +101,8 @@ B200_API void b200_state_free(b200_state* handle);
  *    (n x 121 / 8 / 1 bytes, SSZ encoding of Validator / u64 / participation flags).  List lengths do not change;
  *    an index may appear more than once only with identical values (elements are written in parallel).
  *  - b200_state_update_bytes: overwrite bytes [ssz_offset, ssz_offset + n) of the serialization that was uploaded
- *    (any field; must not change a variable-size field's offset or length — re-upload for that).
+ *    (any field; must not change a variable-size field's offset or length — the two reshaping calls below do that).
+ *    Offsets refer to the serialization as it is now, after any reshape.
  *  - b200_state_root_incremental: root after the updates.  Dirty paths of the big lists only; everything small
  *    (~1 % of the hashes) is re-hashed in full.  b200_state_root stays the full O(N) re-hash. */
 #define B200_FIELD_VALIDATORS 0
@@ -109,9 +110,30 @@ B200_API void b200_state_free(b200_state* handle);
 #define B200_FIELD_PREVIOUS_EPOCH_PARTICIPATION 2
 #define B200_FIELD_CURRENT_EPOCH_PARTICIPATION 3
 #define B200_FIELD_INACTIVITY_SCORES 4
+#define B200_FIELD_ETH1_DATA_VOTES 5
+#define B200_FIELD_HISTORICAL_SUMMARIES 6
+#define B200_FIELD_LATEST_EXECUTION_PAYLOAD_HEADER 7
 B200_API int32_t b200_state_update_elements(b200_state* handle, int32_t field, const uint64_t* indices, const uint8_t* values, size_t n);
 B200_API int32_t b200_state_update_bytes(b200_state* handle, uint64_t ssz_offset, const uint8_t* data, size_t n);
 B200_API int32_t b200_state_root_incremental(b200_state* handle, uint8_t out[32]);
+
+/* Shape changes of a device-resident state (single-GPU handles; a sharded handle gets B200_ERR_BAD_ARG).  The library
+ * rewrites the offset words of the fixed part; b200_state_update_bytes, b200_state_update_elements,
+ * b200_state_shuffled_active_indices and both roots then see the state as reshaped.
+ *  - b200_state_append_elements: the spec's `.push` of `n` elements, SSZ-encoded back to back in `values`, onto one of
+ *    the five big lists (121 / 8 / 1 / 1 / 8-byte elements; the lists grow independently: a deposit appends to all five),
+ *    B200_FIELD_ETH1_DATA_VOTES (72-byte Eth1Data) or B200_FIELD_HISTORICAL_SUMMARIES (64-byte HistoricalSummary).
+ *    A big list's device regions hold its length plus max(2^16, length / 16) elements: an append within them copies
+ *    only the appended bytes; past them the list is relocated on the device (device-to-device copy) and re-hashed in
+ *    full from HBM at the next root.
+ *  - b200_state_set_field: replace a whole small variable-size value: B200_FIELD_ETH1_DATA_VOTES (`len` a multiple of
+ *    72; 0 is the voting-period reset) or B200_FIELD_LATEST_EXECUTION_PAYLOAD_HEADER (584 fixed bytes whose
+ *    extra_data offset, at byte 436, is 584, then 0..32 bytes of extra_data).
+ * Errors: beyond VALIDATOR_REGISTRY_LIMIT, ETH1_DATA_VOTES_BOUND or HISTORICAL_ROOTS_LIMIT (or a serialization past the
+ * 4 GiB its offsets can address) -> B200_ERR_LIMIT; a length that is not a multiple of the element size or a malformed
+ * header -> B200_ERR_SSZ_MALFORMED; any other field id -> B200_ERR_BAD_ARG.  A refused call leaves the handle as it was. */
+B200_API int32_t b200_state_append_elements(b200_state* handle, int32_t field, const uint8_t* values, size_t n);
+B200_API int32_t b200_state_set_field(b200_state* handle, int32_t field, const uint8_t* ssz, size_t len);
 
 /* Multi-GPU sharding of hash_tree_root(BeaconState) (SURVEY.md §8e): rank r of `world` hashes its contiguous
  * power-of-two-aligned slice of the five big lists and returns one subtree root per list
