@@ -45,6 +45,7 @@ _lib.register_protos({
     "b200_fp_selftest": (C.c_int32, [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]),
     "b200_fp_eval": (C.c_int32, [C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_curve_eval": (C.c_int32, [C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "b200_pairing_eval": (C.c_int32, [C.c_int32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "b200_measure_int_peak": (C.c_int32, [C.c_int32, C.POINTER(C.c_double)]),
 })
 
@@ -312,6 +313,28 @@ def curve_eval(op: str, a, b=None) -> np.ndarray:
     out = np.zeros((max(a.shape[0], 1), 73), dtype=np.uint32)
     _lib.check(_lib.lib().b200_curve_eval(CURVE_EVAL_OPS[op], a.shape[0], _lib.ptr(a), _lib.ptr(b), _lib.ptr(out)),
                f"curve_eval({op})")
+    return out[:a.shape[0]]
+
+
+# operations of pairing_eval (bls_kernels.cuh PAIRING_EVAL_*)
+PAIRING_EVAL_OPS = {"fp6_mul": 0, "fp6_inv": 1, "fp12_mul": 2, "fp12_sqr": 3, "fp12_inv": 4, "fp12_mul_by_line": 5,
+                    "fp12_frobenius1": 6, "fp12_frobenius2": 7, "fp12_cyclotomic_sqr": 8, "fp12_pow_z": 9,
+                    "miller_double_step": 10, "miller_add_step": 11, "miller_loop": 12, "final_exp": 13,
+                    "vm_miller8": 32, "vm_miller16": 33, "vm_final8": 34, "vm_final16": 35,
+                    "fold_fp12": 48, "fold_g2": 49}
+
+
+def pairing_eval(op: str, a, b=None) -> np.ndarray:
+    """Self-test: one device pairing operation on raw limbs.  a, b: uint32[n, 145] (twelve 12-word Fp slots in Fp12
+    memory order, then the infinity flag of a point); returns uint32[n, 145]: the result's slots, then the flag word (the
+    final exponentiation's verdict, or the infinity flag of the G2 fold's sum).  The folds return their one result in row 0."""
+    a = np.ascontiguousarray(a, dtype=np.uint32)
+    b = np.zeros_like(a) if b is None else np.ascontiguousarray(b, dtype=np.uint32)
+    if a.ndim != 2 or a.shape[1] != 145 or b.shape != a.shape:
+        raise ValueError("operands must be uint32[n, 145]")
+    out = np.zeros((max(a.shape[0], 1), 145), dtype=np.uint32)
+    _lib.check(_lib.lib().b200_pairing_eval(PAIRING_EVAL_OPS[op], a.shape[0], _lib.ptr(a), _lib.ptr(b), _lib.ptr(out)),
+               f"pairing_eval({op})")
     return out[:a.shape[0]]
 
 

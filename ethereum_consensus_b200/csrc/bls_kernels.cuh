@@ -103,5 +103,31 @@ enum : int32_t {
 constexpr uint32_t kCurveEvalWords = 73;
 void launch_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
 void launch_curve2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
+// on-device self-test of the pairing (b200_pairing_eval).  Records of kPairingEvalWords words: twelve 12-word Fp slots in
+// Fp12 memory order (c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1), raw Montgomery limbs, then a flag word.  Points and
+// lines use the leading slots: G1 affine x, y; G1Pre xz, y, z3; G2 affine x.c0, x.c1, y.c0, y.c1; G2 Jacobian x, y, z as
+// six slots; a line (A, B, C) as six slots.  The input flag is the infinity flag.
+enum : int32_t {
+    PAIRING_EVAL_FP6_MUL = 0, PAIRING_EVAL_FP6_INV = 1, PAIRING_EVAL_FP12_MUL = 2, PAIRING_EVAL_FP12_SQR = 3,
+    PAIRING_EVAL_FP12_INV = 4, PAIRING_EVAL_FP12_MUL_BY_LINE = 5, PAIRING_EVAL_FP12_FROB1 = 6, PAIRING_EVAL_FP12_FROB2 = 7,
+    PAIRING_EVAL_FP12_CYCLO_SQR = 8, PAIRING_EVAL_FP12_POW_Z = 9,
+    PAIRING_EVAL_MILLER_DOUBLE = 10, PAIRING_EVAL_MILLER_ADD = 11,   // a: T (Jacobian); b: Q affine (add), xP, yP in slots 4, 5
+                                                                     // out: T' in slots 0..5, A B C in 6..11
+    PAIRING_EVAL_MILLER_LOOP = 12, PAIRING_EVAL_FINAL_EXP = 13,      // final_exp: the value, flag = final_exp_is_one
+    PAIRING_EVAL_END = 14,                                           // bls_pairing.cu: the one-thread kernels' build
+    PAIRING_EVAL_VM_MILLER8 = 32, PAIRING_EVAL_VM_MILLER16 = 33,     // a: G1Pre, b: G2 affine -> the kernel's Fp12
+    PAIRING_EVAL_VM_FINAL8 = 34, PAIRING_EVAL_VM_FINAL16 = 35,       // a: f0, b: f1 -> the six program outputs, flag = verdict
+    PAIRING_EVAL_VM_END = 36,                                        // bls_vm.cu, teams of 8 / 16 lanes under vm_cta
+    PAIRING_EVAL_FOLD_FP12 = 48, PAIRING_EVAL_FOLD_G2 = 49,          // n inputs of a (Fp12 / G2 Jacobian) -> record 0: the
+    PAIRING_EVAL_FOLD_END = 50                                       // product / the affine sum (flag: infinity); bls_rlc.cu
+};
+constexpr uint32_t kPairingEvalWords = 145;
+void launch_pairing_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
+// the production VM kernels at an explicit team size, with identity indices and every tuple alive; pair_off: 0, 2, 4, ...;
+// f_out: the final program's six outputs per tuple (Fp12 memory order), next to its verdict in codes
+void launch_vm_miller_team(int team, const G1Pre* g1, const uint32_t* idx, const G2Aff* g2, const uint32_t* zeros, uint32_t n,
+                           Fp12* f, void* stream);
+void launch_vm_final_team(int team, const Fp12* f, const uint32_t* pair_off, const uint32_t* zeros, uint32_t n, Fp12* f_out,
+                          int32_t* codes, void* stream);
 
 }  // namespace b200

@@ -94,12 +94,14 @@ __global__ void __launch_bounds__(128) k_vm_miller(const uint32_t* __restrict__ 
 }
 
 // one team per tuple (two Miller values per tuple: pairs pair_off[t], pair_off[t]+1)
-template <int TEAM>
+// STORE (self-test only, b200_pairing_eval): also write the program's six outputs to f_out[t] in Fp12 memory order
+template <int TEAM, bool STORE = false>
 __global__ void __launch_bounds__(128) k_vm_final(const uint32_t* __restrict__ code, const Fp2* __restrict__ consts,
                                                   const Fp12* __restrict__ f, const uint32_t* __restrict__ pair_off,
                                                   const int32_t* __restrict__ pk_code, const uint32_t* __restrict__ flags,
                                                   const int32_t* __restrict__ sig_code, uint32_t n_tuples,
-                                                  int32_t* __restrict__ out_codes, int n_rounds, int n_slots, VmOuts outs6) {
+                                                  int32_t* __restrict__ out_codes, int n_rounds, int n_slots, VmOuts outs6,
+                                                  Fp12* __restrict__ f_out = nullptr) {
     extern __shared__ uint32_t smem[];
     const uint32_t team_in_block = threadIdx.x / TEAM, lane = threadIdx.x % TEAM;
     const uint32_t t = blockIdx.x * (blockDim.x / TEAM) + team_in_block;
@@ -121,6 +123,10 @@ __global__ void __launch_bounds__(128) k_vm_final(const uint32_t* __restrict__ c
     }
     __syncwarp();
     vm_run<TEAM>(code, n_rounds, consts, rf, lane, active);
+    if (STORE && active && lane < 6) {
+        const int tower_pos[6] = {0, 3, 1, 4, 2, 5};
+        reinterpret_cast<Fp2*>(f_out + t)[tower_pos[lane]] = rf.load(uint32_t(outs6.v[lane]));
+    }
     if (t < n_tuples && lane == 0) {
         if (active) {
             bool one = fp2_eq(rf.load(uint32_t(outs6.v[0])), fp2_one());
@@ -172,6 +178,7 @@ static int vm_upload(int slot, cudaStream_t st) {
     // any schedule that fits an SM's shared memory may be loaded later
     cudaFuncSetAttribute(k_vm_miller<TEAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kVmMaxSmemBytes);
     cudaFuncSetAttribute(k_vm_final<TEAM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kVmMaxSmemBytes);
+    cudaFuncSetAttribute(k_vm_final<TEAM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kVmMaxSmemBytes);
     return 0;
 }
 
@@ -236,16 +243,17 @@ static void launch_vm_miller_t(int slot, const G1Pre* g1, const uint32_t* g1_idx
     k_vm_miller<TEAM><<<(n_pairs + teams - 1) / teams, threads, smem, st>>>(
         p.d_code, g_d_consts, g1, g1_idx, g2, g2_idx, pair_tuple, pk_code, flags, sig_code, n_pairs, f, p.rounds, p.slots, p.outs);
 }
-template <int TEAM>
+template <int TEAM, bool STORE = false>
 static void launch_vm_final_t(int slot, const Fp12* f, const uint32_t* pair_off, const int32_t* pk_code, const uint32_t* flags,
-                              const int32_t* sig_code, uint32_t n_tuples, int32_t* out_codes, cudaStream_t st) {
+                              const int32_t* sig_code, uint32_t n_tuples, int32_t* out_codes, cudaStream_t st,
+                              Fp12* f_out = nullptr) {
     const VmProgramDev& p = g_final_prog[slot];
     int threads = g_vm_cta;
     while (threads > 32 && size_t(threads / TEAM) * vm_team_words(uint32_t(p.slots)) * 4 > size_t(kVmMaxSmemBytes)) threads >>= 1;
     const int teams = threads / TEAM;
     const size_t smem = size_t(teams) * vm_team_words(uint32_t(p.slots)) * 4;
-    k_vm_final<TEAM><<<(n_tuples + teams - 1) / teams, threads, smem, st>>>(
-        p.d_code, g_d_consts, f, pair_off, pk_code, flags, sig_code, n_tuples, out_codes, p.rounds, p.slots, p.outs);
+    k_vm_final<TEAM, STORE><<<(n_tuples + teams - 1) / teams, threads, smem, st>>>(
+        p.d_code, g_d_consts, f, pair_off, pk_code, flags, sig_code, n_tuples, out_codes, p.rounds, p.slots, p.outs, f_out);
 }
 
 void launch_vm_miller(const G1Pre* g1, const uint32_t* g1_idx, const G2Aff* g2, const uint32_t* g2_idx,
@@ -262,6 +270,23 @@ void launch_vm_final(const Fp12* f, const uint32_t* pair_off, const int32_t* pk_
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (n_tuples <= g_team16_max) launch_vm_final_t<16>(1, f, pair_off, pk_code, flags, sig_code, n_tuples, out_codes, st);
     else launch_vm_final_t<8>(0, f, pair_off, pk_code, flags, sig_code, n_tuples, out_codes, st);
+}
+
+void launch_vm_miller_team(int team, const G1Pre* g1, const uint32_t* idx, const G2Aff* g2, const uint32_t* zeros, uint32_t n,
+                           Fp12* f, void* stream) {
+    if (!n) return;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int32_t* z = reinterpret_cast<const int32_t*>(zeros);
+    if (team == 16) launch_vm_miller_t<16>(1, g1, idx, g2, idx, zeros, z, zeros, z, n, f, st);
+    else launch_vm_miller_t<8>(0, g1, idx, g2, idx, zeros, z, zeros, z, n, f, st);
+}
+void launch_vm_final_team(int team, const Fp12* f, const uint32_t* pair_off, const uint32_t* zeros, uint32_t n, Fp12* f_out,
+                          int32_t* codes, void* stream) {
+    if (!n) return;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int32_t* z = reinterpret_cast<const int32_t*>(zeros);
+    if (team == 16) launch_vm_final_t<16, true>(1, f, pair_off, z, zeros, z, n, codes, st, f_out);
+    else launch_vm_final_t<8, true>(0, f, pair_off, z, zeros, z, n, codes, st, f_out);
 }
 
 }  // namespace b200

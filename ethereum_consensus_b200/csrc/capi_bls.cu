@@ -24,6 +24,7 @@
 #include <memory>
 #include <random>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "bls_kernels.cuh"
@@ -497,6 +498,20 @@ int32_t VerifyRun::readback(void* h_dst, const void* d_src, size_t bytes) {
     return B200_SUCCESS;
 }
 
+// Warp-shuffle folds (k_rlc_reduce, 32 -> 1 per launch) until one value is left: the Gt product of n Fp12 values or the
+// sum of n G2 points.  The launches alternate between buf[pp] and buf[pp ^ 1] (each holding at least ceil(n / 32)
+// values); returns the buffer with the result, and pp then names the other one.
+template <class T>
+static const T* rlc_fold(Engine& e, const T* in, uint32_t n, T* const buf[2], int& pp, cudaStream_t st) {
+    do {
+        if constexpr (std::is_same_v<T, Fp12>) n = launch_rlc_reduce(in, nullptr, n, buf[pp], nullptr, st);
+        else n = launch_rlc_reduce(nullptr, in, n, nullptr, buf[pp], st);
+        e.launches++;
+        in = buf[pp]; pp ^= 1;
+    } while (n > 1);
+    return in;
+}
+
 // ---- RLC whole-batch check (bls_rlc.cu): T Miller loops + ONE final exponentiation
 int32_t VerifyRun::rlc_tail() {
     RlcReq* rlc = b.rlc;
@@ -528,27 +543,15 @@ int32_t VerifyRun::rlc_tail() {
     G2Jac* qbuf[2] = {static_cast<G2Jac*>(s.rlc_qa.p), static_cast<G2Jac*>(s.rlc_qb.p)};
     // S = sum_t r_t sig_t first (warp-shuffle folds T -> T/32 -> ... -> 1): its pair (-g1, S) then rides in the SAME
     // Miller launch as the T tuple pairs instead of costing a second, latency-bound launch of one team
-    const G2Jac* qi = d_rq;
-    uint32_t n_cur = T;
     int pp = 0;
-    do {
-        n_cur = launch_rlc_reduce(nullptr, qi, n_cur, nullptr, qbuf[pp], sa);
-        e.launches++;
-        qi = qbuf[pp]; pp ^= 1;
-    } while (n_cur > 1);
+    const G2Jac* qi = rlc_fold(e, d_rq, T, qbuf, pp, sa);
     launch_rlc_finish(qi, d_g2 + n_g2, sa);
     // T + 1 Miller loops on the lane-parallel VM: (r_t agg_t, H_t) for every tuple and (-g1, S)
     launch_vm_miller(d_rg1, d_idx, d_g2, d_idx + T + 1, d_zero, reinterpret_cast<const int32_t*>(d_zero), d_zero,
                      reinterpret_cast<const int32_t*>(d_zero), T + 1, static_cast<Fp12*>(s.f.p), sa);
     // Gt product of the T + 1 Miller values, again by warp-shuffle folds
-    const Fp12* fi = static_cast<const Fp12*>(s.f.p);
-    n_cur = T + 1;
     pp = 0;
-    do {
-        n_cur = launch_rlc_reduce(fi, nullptr, n_cur, fbuf[pp], nullptr, sa);
-        e.launches++;
-        fi = fbuf[pp]; pp ^= 1;
-    } while (n_cur > 1);
+    const Fp12* fi = rlc_fold(e, static_cast<const Fp12*>(s.f.p), T + 1, fbuf, pp, sa);
     if (rlc->exchange && rlc_world > 1) {
         // the path's one exchange step: e(-g1, sum over ranks) = product over ranks, so every rank has already paired
         // its own partial sum and only the Gt partial (576 B) and the bad flag travel; then the same fold on all ranks
@@ -561,12 +564,7 @@ int32_t VerifyRun::rlc_tail() {
             B200_CUDA_TRY(cudaMemcpyAsync(fbuf[pp] + r, x + kPart * (1 + r), sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
         B200_CUDA_TRY(cudaMemcpyAsync(h_x, x + kPart, size_t(rlc_world) * kPart, cudaMemcpyDeviceToHost, sa));   // for the ranks' bad flags
         fi = fbuf[pp]; pp ^= 1;
-        n_cur = rlc_world;
-        do {
-            n_cur = launch_rlc_reduce(fi, nullptr, n_cur, fbuf[pp], nullptr, sa);
-            e.launches++;
-            fi = fbuf[pp]; pp ^= 1;
-        } while (n_cur > 1);
+        fi = rlc_fold(e, fi, rlc_world, fbuf, pp, sa);
     }
     // the single final exponentiation: (Gt product) * 1
     Fp12* d_fin = fbuf[pp];
@@ -784,6 +782,129 @@ int32_t b200_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(e.stream);
     cudaFree(d);
     if (ce != cudaSuccess) { e.last_error = cudaGetErrorString(ce); return B200_ERR_CUDA; }
+    return B200_SUCCESS;
+}
+
+// The one-thread ops run on the records themselves (bls_pairing.cu); the VM kernels and the folds take the engine's structs,
+// packed here from the records' leading words, and run exactly as the batch paths launch them.
+int32_t b200_pairing_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    const bool vm = op >= PAIRING_EVAL_VM_MILLER8 && op < PAIRING_EVAL_VM_END;
+    const bool fold = op >= PAIRING_EVAL_FOLD_FP12 && op < PAIRING_EVAL_FOLD_END;
+    if (!(vm || fold || (op >= 0 && op < PAIRING_EVAL_END)) || n > (1u << 24)) return B200_ERR_BAD_ARG;
+    if (n == 0) return B200_SUCCESS;
+    if (!a || !b || !out) return B200_ERR_BAD_ARG;
+    BlsState* s;
+    if ((rc = bls_state(e, &s))) return rc;   // the VM's programs and constants
+    constexpr size_t W = kPairingEvalWords;
+    const size_t rec_bytes = size_t(n) * W * 4;
+    cudaStream_t st = e.stream;
+    std::vector<uint32_t> h_out(size_t(n) * W, 0);
+    const int team = (op == PAIRING_EVAL_VM_MILLER16 || op == PAIRING_EVAL_VM_FINAL16) ? 16 : 8;
+    // device scratch: records, or the structs and index arrays of the VM / fold launches
+    uint8_t* d = nullptr;
+    const size_t scratch = 3 * rec_bytes + size_t(n) * (sizeof(Fp12) * 3 + sizeof(G2Jac) + sizeof(G1Pre) + sizeof(G2Aff) + 12) + 4096;
+    B200_CUDA_TRY(cudaMalloc(&d, scratch));
+    auto carve = [&, off = size_t(0)](size_t bytes) mutable { uint8_t* p = d + off; off += (bytes + 255) & ~size_t(255); return p; };
+    auto fp12_of = [&](const uint32_t* rec) { Fp12 v; memcpy(&v, rec, sizeof(Fp12)); return v; };
+    auto put = [&](size_t i, const void* v, size_t bytes, uint32_t flag) {
+        memcpy(&h_out[i * W], v, bytes);
+        h_out[i * W + 144] = flag;
+    };
+    static_assert(sizeof(Fp12) == 144 * 4 && sizeof(G2Jac) == 72 * 4, "records hold the structs' words in order");
+    cudaError_t ce = cudaSuccess;
+    if (!vm && !fold) {
+        uint32_t* da = reinterpret_cast<uint32_t*>(carve(rec_bytes));
+        uint32_t* db = reinterpret_cast<uint32_t*>(carve(rec_bytes));
+        uint32_t* dout = reinterpret_cast<uint32_t*>(carve(rec_bytes));
+        cudaMemcpyAsync(da, a, rec_bytes, cudaMemcpyHostToDevice, st);
+        cudaMemcpyAsync(db, b, rec_bytes, cudaMemcpyHostToDevice, st);
+        launch_pairing_eval(op, n, da, db, dout, st);
+        e.launches++;
+        ce = cudaGetLastError();
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(h_out.data(), dout, rec_bytes, cudaMemcpyDeviceToHost, st);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    } else if (op == PAIRING_EVAL_VM_MILLER8 || op == PAIRING_EVAL_VM_MILLER16) {
+        std::vector<G1Pre> g1(n);
+        std::vector<G2Aff> g2(n);
+        std::vector<uint32_t> idx(n);
+        for (uint32_t i = 0; i < n; i++) {
+            memcpy(&g1[i], a + i * W, 3 * sizeof(Fp)); g1[i].inf = a[i * W + 144];
+            memcpy(&g2[i], b + i * W, 2 * sizeof(Fp2)); g2[i].inf = b[i * W + 144];
+            idx[i] = i;
+        }
+        G1Pre* dg1 = reinterpret_cast<G1Pre*>(carve(n * sizeof(G1Pre)));
+        G2Aff* dg2 = reinterpret_cast<G2Aff*>(carve(n * sizeof(G2Aff)));
+        uint32_t* didx = reinterpret_cast<uint32_t*>(carve(n * 4));
+        uint32_t* dzero = reinterpret_cast<uint32_t*>(carve(n * 4));
+        Fp12* df = reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12)));
+        std::vector<Fp12> f(n);
+        cudaMemcpyAsync(dg1, g1.data(), n * sizeof(G1Pre), cudaMemcpyHostToDevice, st);
+        cudaMemcpyAsync(dg2, g2.data(), n * sizeof(G2Aff), cudaMemcpyHostToDevice, st);
+        cudaMemcpyAsync(didx, idx.data(), n * 4, cudaMemcpyHostToDevice, st);
+        cudaMemsetAsync(dzero, 0, n * 4, st);
+        launch_vm_miller_team(team, dg1, didx, dg2, dzero, n, df, st);
+        e.launches++;
+        ce = cudaGetLastError();
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(f.data(), df, n * sizeof(Fp12), cudaMemcpyDeviceToHost, st);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        for (uint32_t i = 0; i < n; i++) put(i, &f[i], sizeof(Fp12), 0);
+    } else if (vm) {   // VM final: f0 from a, f1 from b -> one tuple each
+        std::vector<Fp12> f(2 * size_t(n));
+        std::vector<uint32_t> off(n);
+        for (uint32_t i = 0; i < n; i++) { f[2 * i] = fp12_of(a + i * W); f[2 * i + 1] = fp12_of(b + i * W); off[i] = 2 * i; }
+        Fp12* df = reinterpret_cast<Fp12*>(carve(2 * n * sizeof(Fp12)));
+        Fp12* dfo = reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12)));
+        uint32_t* doff = reinterpret_cast<uint32_t*>(carve(n * 4));
+        uint32_t* dzero = reinterpret_cast<uint32_t*>(carve(n * 4));
+        int32_t* dcodes = reinterpret_cast<int32_t*>(carve(n * 4));
+        std::vector<Fp12> fo(n);
+        std::vector<int32_t> codes(n);
+        cudaMemcpyAsync(df, f.data(), 2 * n * sizeof(Fp12), cudaMemcpyHostToDevice, st);
+        cudaMemcpyAsync(doff, off.data(), n * 4, cudaMemcpyHostToDevice, st);
+        cudaMemsetAsync(dzero, 0, n * 4, st);
+        launch_vm_final_team(team, df, doff, dzero, n, dfo, dcodes, st);
+        e.launches++;
+        ce = cudaGetLastError();
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(fo.data(), dfo, n * sizeof(Fp12), cudaMemcpyDeviceToHost, st);
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(codes.data(), dcodes, n * 4, cudaMemcpyDeviceToHost, st);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        for (uint32_t i = 0; i < n; i++) put(i, &fo[i], sizeof(Fp12), codes[i] == BLS_SUCCESS ? 1u : 0u);
+    } else if (op == PAIRING_EVAL_FOLD_FP12) {   // the product of the n values of a, through rlc_tail's fold
+        std::vector<Fp12> f(n);
+        for (uint32_t i = 0; i < n; i++) f[i] = fp12_of(a + i * W);
+        Fp12* df = reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12)));
+        Fp12* buf[2] = {reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12))), reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12)))};
+        cudaMemcpyAsync(df, f.data(), n * sizeof(Fp12), cudaMemcpyHostToDevice, st);
+        int pp = 0;
+        const Fp12* r = rlc_fold(e, static_cast<const Fp12*>(df), n, buf, pp, st);
+        Fp12 v;
+        ce = cudaGetLastError();
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&v, r, sizeof(Fp12), cudaMemcpyDeviceToHost, st);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        put(0, &v, sizeof(Fp12), 0);
+    } else {   // the sum of the n Jacobian points of a, through rlc_tail's fold and k_rlc_finish
+        std::vector<G2Jac> q(n);
+        for (uint32_t i = 0; i < n; i++) memcpy(&q[i], a + i * W, sizeof(G2Jac));
+        G2Jac* dq = reinterpret_cast<G2Jac*>(carve(n * sizeof(G2Jac)));
+        G2Jac* buf[2] = {reinterpret_cast<G2Jac*>(carve(n * sizeof(G2Jac))), reinterpret_cast<G2Jac*>(carve(n * sizeof(G2Jac)))};
+        G2Aff* daff = reinterpret_cast<G2Aff*>(carve(sizeof(G2Aff)));
+        cudaMemcpyAsync(dq, q.data(), n * sizeof(G2Jac), cudaMemcpyHostToDevice, st);
+        int pp = 0;
+        launch_rlc_finish(rlc_fold(e, static_cast<const G2Jac*>(dq), n, buf, pp, st), daff, st);
+        e.launches++;
+        G2Aff v;
+        ce = cudaGetLastError();
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(&v, daff, sizeof(G2Aff), cudaMemcpyDeviceToHost, st);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        put(0, &v, 2 * sizeof(Fp2), v.inf);
+    }
+    cudaFree(d);
+    if (ce != cudaSuccess) { e.last_error = cudaGetErrorString(ce); return B200_ERR_CUDA; }
+    memcpy(out, h_out.data(), rec_bytes);
     return B200_SUCCESS;
 }
 

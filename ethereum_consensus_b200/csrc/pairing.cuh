@@ -96,9 +96,9 @@ B200_BIG void fp12_pow_z(Fp12& r, const Fp12& g) {
     r = acc;
 }
 
-// f^((p^12-1)/r * 3) == 1 ?
-B200_BIG bool final_exp_is_one(const Fp12& f_in) {
-    Fp12 f, t0, t1, a, b, c;
+// c = f^((p^12-1)/r * 3); the inverse path maps 0 to 0
+B200_BIG void final_exp(Fp12& c, const Fp12& f_in) {
+    Fp12 f, t0, t1, a, b;
     // easy part: f^((p^6-1)(p^2+1))
     fp12_inv(t0, f_in);
     fp12_conj(t1, f_in);
@@ -118,6 +118,12 @@ B200_BIG bool final_exp_is_one(const Fp12& f_in) {
     fp12_mul(c, c, t1);                                               // b^(x^2+p^2-1)
     fp12_sqr(t0, f); fp12_mul(t0, t0, f);                             // f^3
     fp12_mul(c, c, t0);
+}
+
+// f^((p^12-1)/r * 3) == 1 ?
+B200_BIG bool final_exp_is_one(const Fp12& f_in) {
+    Fp12 c;
+    final_exp(c, f_in);
     return fp12_is_one(c);
 }
 

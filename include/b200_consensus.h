@@ -296,6 +296,13 @@ B200_API int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const u
  * the first 12 words of a slot, Fp2 as c0 then c1), then a flag word (in: the affine infinity flag; out: the subgroup
  * verdict, or the infinity flag of an affine result).  Test use only. */
 B200_API int32_t b200_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
+/* On-device self-test of the pairing, for comparison with a big-integer oracle: `op` (bls_kernels.cuh, PAIRING_EVAL_*) runs
+ * in the unit whose production kernel runs it: Fp6 / Fp12 operations, Miller steps and loop, the final exponentiation
+ * (one thread per record), the lane-parallel Miller and final programs at teams of 8 or 16 lanes, and the RLC folds.
+ * a, b, out: n x 145 words: twelve 12-word Fp slots in Fp12 memory order of raw little-endian 32-bit Montgomery limbs,
+ * then a flag word (in: the infinity flag of a point; out: the final exponentiation's verdict, or the infinity flag of the
+ * G2 fold's affine sum).  n = 0 .. 2^24.  Test use only. */
+B200_API int32_t b200_pairing_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
 
 #ifdef __cplusplus
 }

@@ -246,3 +246,80 @@ extern "C" HM int hm_vm_matches_direct(const uint8_t* g1a, const uint8_t* g2a, c
     const int r8 = vm_matches_direct<8>(g1a, g2a, g1b, g2b), r16 = vm_matches_direct<16>(g1a, g2a, g1b, g2b);
     return r8 == r16 ? r8 : 0;
 }
+
+// ---- b200_pairing_eval's operations on the host build of the same headers, on the same 145-word records (the folds
+// excepted): the one-thread ops, and the scheduled VM programs through vm_run_host with G1Pre inputs of any Z
+template <int TEAM>
+static void hm_vm_miller(Fp12& f, const Fp* pre, const Fp2* q) {
+    typedef VmProg<TEAM> P;
+    Fp2 consts[kVmConsts];
+    vm_consts(consts);
+    static Fp2 rf[256];
+    for (int k = 0; k < 3; k++) { rf[k].c0 = pre[k]; rf[k].c1 = fp_zero(); }
+    rf[3] = q[0]; rf[4] = q[1];
+    vm_run_host<TEAM>(P::miller_code(), P::miller_rounds, consts, rf);
+    Fp2* d = &f.c0.c0;
+    const int tower_pos[6] = {0, 3, 1, 4, 2, 5};
+    for (int k = 0; k < 6; k++) d[tower_pos[k]] = rf[P::miller_out[k]];
+}
+template <int TEAM>
+static uint32_t hm_vm_final(Fp12& f, const Fp12& f0, const Fp12& f1) {
+    typedef VmProg<TEAM> P;
+    Fp2 consts[kVmConsts];
+    vm_consts(consts);
+    static Fp2 rf[256];
+    const int tower_pos[6] = {0, 3, 1, 4, 2, 5};
+    for (int k = 0; k < 6; k++) { rf[k] = (&f0.c0.c0)[tower_pos[k]]; rf[6 + k] = (&f1.c0.c0)[tower_pos[k]]; }
+    vm_run_host<TEAM>(P::final_code(), P::final_rounds, consts, rf);
+    Fp2* d = &f.c0.c0;
+    for (int k = 0; k < 6; k++) d[tower_pos[k]] = rf[P::final_out[k]];
+    return fp12_is_one(f) ? 1u : 0u;
+}
+extern "C" HM void hm_pairing_eval(int op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out) {
+    const size_t W = 145;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t* pa = a + i * W;
+        const uint32_t* pb = b + i * W;
+        Fp12 x, y, r = fp12_one();
+        memcpy(&x, pa, sizeof(Fp12));
+        memcpy(&y, pb, sizeof(Fp12));
+        uint32_t flag = 0;
+        switch (op) {
+        case 0: fp6_mul(r.c0, x.c0, y.c0); r.c1 = x.c1; break;
+        case 1: fp6_inv(r.c0, x.c0); r.c1 = x.c1; break;
+        case 2: fp12_mul(r, x, y); break;
+        case 3: fp12_sqr(r, x); break;
+        case 4: fp12_inv(r, x); break;
+        case 5: fp12_mul_by_line(r, x, y.c0.c0, y.c0.c1, y.c0.c2); break;
+        case 6: fp12_frobenius<1>(r, x); break;
+        case 7: fp12_frobenius<2>(r, x); break;
+        case 8: fp12_cyclotomic_sqr(r, x); break;
+        case 9: fp12_pow_z(r, x); break;
+        case 10: case 11: {
+            G2Jac t; t.x = x.c0.c0; t.y = x.c0.c1; t.z = x.c0.c2;
+            G2Aff q; q.x = y.c0.c0; q.y = y.c0.c1; q.inf = 0;
+            if (op == 10) miller_double_step(t, r.c1.c0, r.c1.c1, r.c1.c2, y.c0.c2.c0, y.c0.c2.c1);
+            else miller_add_step(t, r.c1.c0, r.c1.c1, r.c1.c2, q, y.c0.c2.c0, y.c0.c2.c1);
+            r.c0.c0 = t.x; r.c0.c1 = t.y; r.c0.c2 = t.z;
+            break;
+        }
+        case 12: {
+            G1Aff p; p.x = x.c0.c0.c0; p.y = x.c0.c0.c1; p.inf = pa[144];
+            G2Aff q; q.x = y.c0.c0; q.y = y.c0.c1; q.inf = pb[144];
+            miller_loop(r, p, q);
+            break;
+        }
+        case 13: final_exp(r, x); flag = fp12_is_one(r) ? 1u : 0u; break;
+        case 32: case 33:   // the kernels bypass the program for a point at infinity: the pair contributes one
+            if (!pa[144] && !pb[144]) {
+                if (op == 32) hm_vm_miller<8>(r, &x.c0.c0.c0, &y.c0.c0); else hm_vm_miller<16>(r, &x.c0.c0.c0, &y.c0.c0);
+            }
+            break;
+        case 34: flag = hm_vm_final<8>(r, x, y); break;
+        case 35: flag = hm_vm_final<16>(r, x, y); break;
+        default: break;
+        }
+        memcpy(out + i * W, &r, sizeof(Fp12));
+        out[i * W + 144] = flag;
+    }
+}
