@@ -36,6 +36,9 @@ _lib.register_protos({
     "b200_eth_aggregate_public_keys": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200_fast_aggregate_verify_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200_registry_load": (C.c_int32, [C.c_void_p, C.c_size_t]),
+    "b200_registry_append": (C.c_int32, [C.c_void_p, C.c_size_t]),
+    "b200_registry_load_state": (C.c_int32, [C.c_void_p]),
+    "b200_registry_sync_state": (C.c_int32, [C.c_void_p]),
     "b200_registry_key_codes": (C.c_int32, [C.c_void_p, C.c_size_t]),
     "b200_fast_aggregate_verify_batch_indexed": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200_fast_aggregate_verify_batch_all": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int32)]),
@@ -221,12 +224,37 @@ def fast_aggregate_verify_batch_all(pks_flat, pk_offsets, msgs32, sigs, seed: by
 
 class Registry:
     """Validated validator public keys resident in HBM (`state.validators[i].public_key` is immutable,
-    phase0/validator.rs:10-13): `load` runs key_validate once per key, `verify_batch` names signers by index."""
+    phase0/validator.rs:10-13): `load` runs key_validate once per key, `verify_batch` names signers by index.
+    The list of keys grows with the validator set: `append` validates only the new keys, `from_state` / `sync` read them
+    from a resident `ssz.DeviceBeaconState` in HBM.  The library keeps one registry per process; `n` is its length."""
 
     def __init__(self, pks_flat):
         n = (pks_flat.nbytes if hasattr(pks_flat, "nbytes") else len(pks_flat)) // 48
         _lib.check(_lib.lib().b200_registry_load(_lib.ptr(pks_flat), n), "registry_load")
         self.n = n
+
+    @classmethod
+    def from_state(cls, state) -> "Registry":
+        """The registry of every validator's public key of a (single-GPU) resident state, read on the device."""
+        reg = cls.__new__(cls)
+        _lib.check(_lib.lib().b200_registry_load_state(state._h), "registry_load_state")
+        reg.n = state.n_validators
+        return reg
+
+    def append(self, pks_flat) -> None:
+        """Validate and append 48-byte keys: they become indices n, n + 1, ...; the keys already loaded are not
+        validated again."""
+        nbytes = _nbytes(pks_flat)
+        if nbytes % 48:
+            raise ValueError(f"registry keys must be 48 bytes each, got {nbytes} bytes")
+        _lib.check(_lib.lib().b200_registry_append(_lib.ptr(pks_flat), nbytes // 48), "registry_append")
+        self.n += nbytes // 48
+
+    def sync(self, state) -> None:
+        """Append the validators `state` gained since the registry last matched it (`add_validators`); the first n keys
+        are taken to be the state's first n public keys."""
+        _lib.check(_lib.lib().b200_registry_sync_state(state._h), "registry_sync_state")
+        self.n = state.n_validators
 
     def key_codes(self) -> np.ndarray:
         out = np.empty(max(self.n, 1), dtype=np.int32)

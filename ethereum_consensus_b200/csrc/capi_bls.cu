@@ -643,6 +643,61 @@ static Batch shard_batch(const uint8_t* pks_flat, const uint32_t* pk_offsets, co
             .msgs = msgs32 + 32 * r.lo, .msg_off = moff.data(), .n_msgs = uint32_t(r.cnt), .sigs = sigs + 96 * r.lo, .T = uint32_t(r.cnt)};
 }
 
+// Registry entries beyond reg_n reserved when its arrays are (re)allocated: the resident state lists' rule, 2^16 or a
+// sixteenth of the registry, so that appends of a block's deposits validate in place for many blocks
+static size_t registry_headroom(size_t n) { return std::max<size_t>(size_t(1) << 16, n / 16); }
+
+// Validate n keys into registry entries [at, at + n) and make the registry at + n keys long: at = 0 replaces it,
+// at = reg_n appends.  The keys come from the host (`host_keys`) or from n Validator records in HBM (`records`).  The
+// arrays always hold reg_n keys, then the extra-key tail `..._batch_mixed` validates into; an append past that grows them
+// (entries [0, at) copied on the device) before any key is validated.  last_kernel_ms: the gather and K1.
+static int32_t registry_fill(Engine& e, BlsState& s, size_t at, const uint8_t* host_keys, const uint8_t* records, size_t n) {
+    const size_t need = at + n + kRegistryExtraKeys + 1;
+    if (s.reg_aff.cap < need * sizeof(G1Aff) || s.reg_code.cap < need * 4) {
+        const size_t want = at + n + registry_headroom(at + n) + kRegistryExtraKeys + 1;
+        DevBuf na, nc;
+        cudaError_t ce = na.reserve(want * sizeof(G1Aff));
+        if (ce == cudaSuccess) ce = nc.reserve(want * 4);
+        if (ce == cudaSuccess && at) ce = cudaMemcpyAsync(na.p, s.reg_aff.p, at * sizeof(G1Aff), cudaMemcpyDeviceToDevice, e.stream);
+        if (ce == cudaSuccess && at) ce = cudaMemcpyAsync(nc.p, s.reg_code.p, at * 4, cudaMemcpyDeviceToDevice, e.stream);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(e.stream);
+        if (ce != cudaSuccess) {
+            na.release(); nc.release();
+            e.last_error = std::string("registry growth: ") + cudaGetErrorString(ce);
+            return B200_ERR_CUDA;
+        }
+        s.reg_aff.release(); s.reg_code.release();
+        s.reg_aff = na; s.reg_code = nc;
+    }
+    B200_CUDA_TRY(s.keys.reserve(n * 48 + 64));
+    if (host_keys && n) B200_CUDA_TRY(cudaMemcpyAsync(s.keys.p, host_keys, n * 48, cudaMemcpyHostToDevice, e.stream));
+    B200_CUDA_TRY(cudaEventRecord(s.ev_k0, e.stream));
+    if (records) {
+        launch_gather_validator_keys(records, uint32_t(n), static_cast<uint8_t*>(s.keys.p), e.stream);
+        e.launches += n ? 1 : 0;
+    }
+    launch_g1_validate(static_cast<const uint8_t*>(s.keys.p), uint32_t(n), static_cast<G1Aff*>(s.reg_aff.p) + at,
+                       static_cast<int32_t*>(s.reg_code.p) + at, e.stream);
+    e.launches += n ? 1 : 0;
+    B200_CUDA_TRY(cudaEventRecord(s.ev_k1, e.stream));
+    B200_CUDA_TRY(cudaGetLastError());
+    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, s.ev_k0, s.ev_k1));
+    s.last_dominant_ms = e.last_kernel_ms;
+    s.reg_n = at + n;
+    return B200_SUCCESS;
+}
+
+// the registry calls on a resident state: its Validator records in HBM and their count
+static int32_t registry_state_records(Engine& e, b200_state* h, const uint8_t** records, uint64_t* n) {
+    if (state_validator_records(h, records, n)) {
+        e.last_error = "registry: the state handle is NULL, not uploaded or sharded";
+        return B200_ERR_BAD_ARG;
+    }
+    if (*n > 0x7fffffffu) { e.last_error = "registry: more validators than the registry holds"; return B200_ERR_BAD_ARG; }
+    return B200_SUCCESS;
+}
+
 // every validator index names a resident registry key or one of the call's n_extra extra keys
 static int32_t check_indices(Engine& e, const BlsState& s, const uint32_t* index, uint32_t n, size_t n_extra) {
     for (uint32_t i = 0; i < n; i++)
@@ -1048,21 +1103,51 @@ int32_t b200_registry_load(const uint8_t* pks_flat, size_t n) {
     BlsState* s;
     rc = bls_state(e, &s);
     if (rc) return rc;
-    B200_CUDA_TRY(s->keys.reserve(n * 48 + 64));
-    B200_CUDA_TRY(s->reg_aff.reserve((n + kRegistryExtraKeys + 1) * sizeof(G1Aff)));   // + the tail `..._batch_mixed` validates into
-    B200_CUDA_TRY(s->reg_code.reserve((n + kRegistryExtraKeys + 1) * 4));
-    if (n) B200_CUDA_TRY(cudaMemcpyAsync(s->keys.p, pks_flat, n * 48, cudaMemcpyHostToDevice, e.stream));
-    B200_CUDA_TRY(cudaEventRecord(s->ev_k0, e.stream));
-    launch_g1_validate(static_cast<const uint8_t*>(s->keys.p), uint32_t(n), static_cast<G1Aff*>(s->reg_aff.p),
-                       static_cast<int32_t*>(s->reg_code.p), e.stream);
-    e.launches += n ? 1 : 0;
-    B200_CUDA_TRY(cudaEventRecord(s->ev_k1, e.stream));
-    B200_CUDA_TRY(cudaGetLastError());
-    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
-    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, s->ev_k0, s->ev_k1));
-    s->last_dominant_ms = e.last_kernel_ms;
-    s->reg_n = n;
-    return B200_SUCCESS;
+    return registry_fill(e, *s, 0, pks_flat, nullptr, n);
+}
+
+int32_t b200_registry_append(const uint8_t* pks_flat, size_t n) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!pks_flat && n) return B200_ERR_BAD_ARG;
+    BlsState* s;
+    rc = bls_state(e, &s);
+    if (rc) return rc;
+    if (n > 0x7fffffffu - s->reg_n) { e.last_error = "registry_append: more than 2^31 - 1 keys"; return B200_ERR_BAD_ARG; }
+    if (n == 0) { e.last_kernel_ms = 0.f; return B200_SUCCESS; }
+    return registry_fill(e, *s, s->reg_n, pks_flat, nullptr, n);
+}
+
+int32_t b200_registry_load_state(b200_state* h) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    const uint8_t* records;
+    uint64_t n;
+    if ((rc = registry_state_records(e, h, &records, &n))) return rc;
+    BlsState* s;
+    rc = bls_state(e, &s);
+    if (rc) return rc;
+    return registry_fill(e, *s, 0, nullptr, records, size_t(n));
+}
+
+int32_t b200_registry_sync_state(b200_state* h) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    const uint8_t* records;
+    uint64_t n;
+    if ((rc = registry_state_records(e, h, &records, &n))) return rc;
+    BlsState* s;
+    rc = bls_state(e, &s);
+    if (rc) return rc;
+    if (n < s->reg_n) { e.last_error = "registry_sync_state: the state has fewer validators than the registry"; return B200_ERR_BAD_ARG; }
+    if (n == s->reg_n) { e.last_kernel_ms = 0.f; return B200_SUCCESS; }
+    return registry_fill(e, *s, s->reg_n, nullptr, records + s->reg_n * 121, size_t(n) - s->reg_n);
 }
 
 int32_t b200_registry_key_codes(int32_t* out_codes, size_t n) {

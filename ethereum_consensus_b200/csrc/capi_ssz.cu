@@ -234,6 +234,18 @@ int32_t adopt_plan(Engine& e, b200_state* h, SszPlan& np, std::vector<uint32_t>&
 }
 }  // namespace
 
+// the registry's view of a resident state (capi_bls.cu: b200_registry_load_state / b200_registry_sync_state)
+int32_t b200::state_validator_records(const b200_state* h, const uint8_t** records, uint64_t* n) {
+    if (!h || !h->uploaded || h->sharded) return B200_ERR_BAD_ARG;
+    *records = nullptr;
+    *n = big_count(h, 0);
+    if (*n == 0) return B200_SUCCESS;
+    uint64_t field_off = 0; size_t nbytes = 0;
+    if (!h->plan.chain_field(0, &field_off, &nbytes)) return B200_ERR_BAD_ARG;
+    *records = static_cast<const uint8_t*>(h->fields.p) + field_off;
+    return B200_SUCCESS;
+}
+
 extern "C" {
 
 int32_t b200_init(int32_t device) {

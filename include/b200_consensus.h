@@ -240,6 +240,26 @@ B200_API int32_t b200_fast_aggregate_verify_batch_all(const uint8_t* pks_flat, c
 /* Registry mode: validate the (append-only, immutable-pubkey) validator registry once, keep the affine keys in
  * HBM, then verify tuples that name their signers by validator index.  Same per-tuple codes as the strict path. */
 B200_API int32_t b200_registry_load(const uint8_t* pks_flat, size_t n);
+/* The registry follows the growing validator list (deposits, phase0/block_processing.rs:394-401).  Registry indices are
+ * validator indices, and keys are never validated twice: each key keeps the code and point it was given, so the key codes
+ * and every verdict are exactly those of b200_registry_load over the concatenated key list, invalid keys included (a
+ * tuple that names an invalid key gets its code).  The `..._batch_mixed` extra-key tail follows reg_n: after an append,
+ * index i >= reg_n names extra key i - reg_n with the new reg_n.
+ *  - b200_registry_append: validate n more keys; they become indices reg_n .. reg_n + n - 1.  Keys already in the
+ *    registry are neither copied from the host nor validated again.  n == 0 succeeds and changes nothing.
+ *  - b200_registry_load_state: replace the registry with the public keys of every validator of a single-GPU resident
+ *    state (b200_state_upload_deneb), read from its Validator records in HBM: no key crosses PCIe.
+ *  - b200_registry_sync_state: append the state's validators reg_n .. n_validators - 1, i.e. those that
+ *    b200_state_append_elements added since the registry last matched the state.  Keys 0 .. reg_n - 1 are taken to be
+ *    the state's first reg_n public keys (pubkeys are immutable, phase0/validator.rs:10-13) and are not compared again;
+ *    a sync with nothing new succeeds and changes nothing.
+ * The registry holds its own copy of the keys: freeing the state afterwards leaves it intact.  Each call sets
+ * b200_last_kernel_ms to the device time of its kernels.  B200_ERR_BAD_ARG, with the registry left as it was (size, keys,
+ * codes): a NULL pointer with n > 0; reg_n + n > 0x7fffffff (the bound of b200_registry_load); a state handle that is
+ * NULL, not uploaded or sharded; a sync against a state with fewer validators than the registry. */
+B200_API int32_t b200_registry_append(const uint8_t* pks_flat, size_t n);
+B200_API int32_t b200_registry_load_state(b200_state* handle);
+B200_API int32_t b200_registry_sync_state(b200_state* handle);
 B200_API int32_t b200_registry_key_codes(int32_t* out_codes, size_t n);
 B200_API int32_t b200_fast_aggregate_verify_batch_indexed(const uint32_t* indices, const uint32_t* offsets,
                                                           const uint8_t* msgs32, const uint8_t* sigs, size_t n_tuples,
