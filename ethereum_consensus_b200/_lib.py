@@ -64,6 +64,7 @@ _PROTOS = {
     # multi-GPU (comm.cu): the exchange step lives inside the library
     "b200_comm_unique_id": (C.c_int32, [C.c_void_p]),
     "b200_comm_init": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),
+    "b200_comm_init_loopback": (C.c_int32, [C.c_char_p, C.c_int32, C.c_int32, C.c_uint64, C.c_uint32]),
     "b200_comm_info": (C.c_int32, [C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200_comm_destroy": (None, []),
     "b200_collective_count": (C.c_uint64, []),

@@ -159,13 +159,13 @@ enum PairMode { MODE_FAST_AGGREGATE = 0, MODE_AGGREGATE = 1 };
 constexpr size_t kMaxBatchTuples = size_t(1) << 26;
 // keys a `..._batch_mixed` call may bring along (a block carries <= 16 deposits + 16 bls-to-execution changes)
 constexpr size_t kRegistryExtraKeys = size_t(1) << 16;
-constexpr size_t kRlcPart = sizeof(Fp12) + sizeof(G2Jac) + 16;   // one rank's exchanged RLC partial: Gt | G2 | bad flag
+constexpr size_t kRlcPart = sizeof(Fp12) + 16;   // one rank's exchanged RLC partial: Gt | bad flag (and 12 zero bytes)
 
 // whole-batch RLC request: when passed, the pairing phase answers ONE boolean for all tuples instead of T codes
 struct RlcReq {
     const uint8_t* seed32;  // scalars r_t = H(seed || t0 + t)
     uint64_t t0;            // global index of this call's first tuple (sharded batches)
-    bool exchange;          // all-gather the per-rank (Gt, G2) partials over the library's communicator
+    bool exchange;          // all-gather the per-rank Gt partials and bad flags over the library's communicator
     int32_t all_ok;         // out
 };
 
@@ -557,7 +557,7 @@ int32_t VerifyRun::rlc_tail() {
         // its own partial sum and only the Gt partial (576 B) and the bad flag travel; then the same fold on all ranks
         uint8_t* x = static_cast<uint8_t*>(s.rlc_xch.p);
         B200_CUDA_TRY(cudaMemcpyAsync(x, fi, sizeof(Fp12), cudaMemcpyDeviceToDevice, sa));
-        B200_CUDA_TRY(cudaMemcpyAsync(x + sizeof(Fp12) + sizeof(G2Jac), d_misc + 32, 16, cudaMemcpyDeviceToDevice, sa));
+        B200_CUDA_TRY(cudaMemcpyAsync(x + sizeof(Fp12), d_misc + 32, 16, cudaMemcpyDeviceToDevice, sa));
         int32_t rcx = comm_all_gather(e, x, x + kPart, kPart, sa);
         if (rcx) return rcx;
         for (uint32_t r = 0; r < rlc_world; r++)   // unpack into the fold's input array (world <= a few dozen)
@@ -579,7 +579,7 @@ int32_t VerifyRun::rlc_tail() {
     if (rlc->exchange && rlc_world > 1)
         for (uint32_t r = 0; r < rlc_world; r++) {
             int32_t flag;
-            memcpy(&flag, h_x + size_t(r) * kPart + sizeof(Fp12) + sizeof(G2Jac), 4);
+            memcpy(&flag, h_x + size_t(r) * kPart + sizeof(Fp12), 4);
             bad = bad || flag != 0;
         }
     rlc->all_ok = (!bad && h_out[8] == BLS_SUCCESS) ? 1 : 0;
@@ -1069,8 +1069,8 @@ int32_t b200_fast_aggregate_verify_batch_indexed_all(const uint32_t* indices, co
                               .n_msgs = uint32_t(n_tuples), .sigs = sigs, .T = uint32_t(n_tuples)}, seed32, 0, false, all_ok);
 }
 
-// every rank passes the same batch AND the same seed; each verifies its block, the (Gt, G2) partials are all-gathered and
-// every rank finishes the same single final exponentiation
+// every rank passes the same batch AND the same seed; each verifies its block, the Gt partials and bad flags are
+// all-gathered and every rank finishes the same single final exponentiation
 int32_t b200_fast_aggregate_verify_batch_all_sharded(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs32,
                                                      const uint8_t* sigs, size_t n_tuples, const uint8_t seed32[32], int32_t* all_ok) {
     Engine& e = engine();

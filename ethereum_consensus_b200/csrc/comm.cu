@@ -6,12 +6,15 @@
 // shares that copy instead of loading a second, and a single-GPU deployment never needs the library at all.
 // The reference has no counterpart (it is single-process, SURVEY.md §2a); the messages are tiny (160 B of subtree
 // roots, 4 B per verdict, 576 B of Gt) so the collectives are latency-bound over NVLink — one per call.
+// b200_comm_init_loopback puts a test transport behind the same comm_all_gather (comm_loopback.h): one file shared by
+// processes on one GPU, so the sharded paths run at world > 1 where two GPUs are not available.
 #include <dlfcn.h>
 #include <nccl.h>
 
 #include <cstring>
 
 #include "comm.h"
+#include "comm_loopback.h"
 
 namespace b200 {
 namespace {
@@ -22,12 +25,12 @@ struct NcclApi {
     ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
     ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
     ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
-    ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
     const char* (*GetErrorString)(ncclResult_t) = nullptr;
     ncclResult_t (*GetVersion)(int*) = nullptr;
 };
 NcclApi g_nccl;
 Comm g_comm;
+Loopback g_loop;   // active between b200_comm_init_loopback and b200_comm_destroy
 
 template <class F>
 bool bind(F& fn, const char* name) {
@@ -49,7 +52,7 @@ int32_t load_nccl(Engine& e) {
     }
     bool ok = bind(g_nccl.GetUniqueId, "ncclGetUniqueId") && bind(g_nccl.CommInitRank, "ncclCommInitRank") &&
               bind(g_nccl.CommDestroy, "ncclCommDestroy") && bind(g_nccl.AllGather, "ncclAllGather") &&
-              bind(g_nccl.AllReduce, "ncclAllReduce") && bind(g_nccl.GetErrorString, "ncclGetErrorString") &&
+              bind(g_nccl.GetErrorString, "ncclGetErrorString") &&
               bind(g_nccl.GetVersion, "ncclGetVersion");
     if (!ok) {
         e.last_error = "NCCL library lacks a required symbol";
@@ -65,6 +68,22 @@ int32_t nccl_fail(Engine& e, const char* what, ncclResult_t r) {
     return B200_ERR_COMM;
 }
 
+// The all-gather through the loopback file: the send bytes go to this rank's slot once the stream has produced them,
+// the ranks meet at the file's barrier, and the world slots are copied to `recv` on the stream.
+int32_t loopback_all_gather(Engine& e, const void* send, void* recv, size_t bytes_per_rank, cudaStream_t stream) {
+    uint8_t* mine = g_loop.send_slot(bytes_per_rank, e.last_error);
+    if (!mine) return B200_ERR_COMM;
+    if (bytes_per_rank) B200_CUDA_TRY(cudaMemcpyAsync(mine, send, bytes_per_rank, cudaMemcpyDeviceToHost, stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(stream));
+    const uint8_t* all = g_loop.arrive(e.last_error);
+    if (!all) return B200_ERR_COMM;
+    for (int r = 0; r < g_comm.world && bytes_per_rank; r++)
+        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(recv) + size_t(r) * bytes_per_rank, all + size_t(r) * g_loop.slot_bytes(),
+                                      bytes_per_rank, cudaMemcpyHostToDevice, stream));
+    e.collectives++;
+    return B200_SUCCESS;
+}
+
 }  // namespace
 
 Comm& comm() { return g_comm; }
@@ -77,21 +96,9 @@ int32_t comm_all_gather(Engine& e, const void* send, void* recv, size_t bytes_pe
             B200_CUDA_TRY(cudaMemcpyAsync(recv, send, bytes_per_rank, cudaMemcpyDeviceToDevice, stream));
         return B200_SUCCESS;
     }
+    if (g_loop.active()) return loopback_all_gather(e, send, recv, bytes_per_rank, stream);
     ncclResult_t r = g_nccl.AllGather(send, recv, bytes_per_rank, ncclUint8, static_cast<ncclComm_t>(c.nccl), stream);
     if (r != ncclSuccess) return nccl_fail(e, "ncclAllGather", r);
-    e.collectives++;
-    return B200_SUCCESS;
-}
-
-int32_t comm_all_reduce_min_i32(Engine& e, const void* send, void* recv, size_t count, cudaStream_t stream) {
-    Comm& c = g_comm;
-    if (!c.ready) { e.last_error = "b200_comm_init has not been called"; return B200_ERR_NOT_INITIALIZED; }
-    if (c.world == 1) {
-        if (send != recv && count) B200_CUDA_TRY(cudaMemcpyAsync(recv, send, 4 * count, cudaMemcpyDeviceToDevice, stream));
-        return B200_SUCCESS;
-    }
-    ncclResult_t r = g_nccl.AllReduce(send, recv, count, ncclInt32, ncclMin, static_cast<ncclComm_t>(c.nccl), stream);
-    if (r != ncclSuccess) return nccl_fail(e, "ncclAllReduce", r);
     e.collectives++;
     return B200_SUCCESS;
 }
@@ -135,6 +142,19 @@ int32_t b200_comm_init(const uint8_t id[B200_COMM_ID_BYTES], int32_t rank, int32
         c.nccl = nc;
         g_nccl.GetVersion(&c.nccl_version);
     }
+    c.rank = rank; c.world = world; c.ready = true;
+    return B200_SUCCESS;
+}
+
+int32_t b200_comm_init_loopback(const char* path, int32_t rank, int32_t world, uint64_t slot_bytes, uint32_t timeout_ms) {
+    Engine& e = engine();
+    std::unique_lock<std::mutex> lk(e.mu);
+    if (!e.ready) { e.last_error = "b200_init must precede b200_comm_init_loopback"; return B200_ERR_NOT_INITIALIZED; }
+    if (!path || world < 1 || rank < 0 || rank >= world || !slot_bytes) return B200_ERR_BAD_ARG;
+    Comm& c = g_comm;
+    if (c.ready) return (c.rank == rank && c.world == world) ? B200_SUCCESS : B200_ERR_BAD_ARG;
+    B200_CUDA_TRY(cudaSetDevice(e.device));
+    if (!g_loop.open(path, rank, world, slot_bytes, timeout_ms, e.last_error)) return B200_ERR_COMM;
     c.rank = rank; c.world = world; c.ready = true;
     return B200_SUCCESS;
 }
@@ -183,6 +203,7 @@ void b200_comm_destroy(void) {
     if (!c.ready) return;
     if (e.ready) { cudaSetDevice(e.device); cudaStreamSynchronize(e.stream); }
     if (c.nccl && g_nccl.CommDestroy) g_nccl.CommDestroy(static_cast<ncclComm_t>(c.nccl));
+    g_loop.close();
     c = Comm();
 }
 

@@ -14,6 +14,5 @@ Comm& comm();
 
 // every rank contributes `bytes_per_rank` bytes; recv holds world x bytes_per_rank, rank-major.  Issued on `stream`.
 int32_t comm_all_gather(Engine& e, const void* send, void* recv, size_t bytes_per_rank, cudaStream_t stream);
-int32_t comm_all_reduce_min_i32(Engine& e, const void* send, void* recv, size_t count, cudaStream_t stream);
 
 }  // namespace b200

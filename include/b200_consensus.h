@@ -174,8 +174,18 @@ B200_API void b200_comm_destroy(void);
 /* all-gather of `bytes_per_rank` host bytes per rank into recv[world * bytes_per_rank] (rank-major): for the host's own
  * small exchanges, e.g. verdict vectors when every rank verified a different batch (weak scaling). */
 B200_API int32_t b200_comm_all_gather_bytes(const uint8_t* send, size_t bytes_per_rank, uint8_t* recv);
-/* NCCL collectives issued by the library since start-up (bench.py reports it next to gpu_launches). */
+/* NCCL collectives issued by the library since start-up (bench.py reports it next to gpu_launches); loopback
+ * all-gathers count too. */
 B200_API uint64_t b200_collective_count(void);
+/* Test use only: a communicator of `world` processes that may share ONE GPU, for running the sharded entry points at
+ * world > 1 without NCCL.  Every all-gather goes through the file `path`, which all ranks map (MAP_SHARED) and which must
+ * be new for each communicator: a 64-byte header (magic, world, slot size, arrival counter), then two generations of
+ * world x `slot_bytes` slots.  Same preconditions as b200_comm_init (b200_init first; a second init with another rank or
+ * world is refused; b200_comm_destroy resets).  A rank that finds a header with another world or slot size gets
+ * B200_ERR_COMM.  An all-gather larger than `slot_bytes` per rank returns B200_ERR_COMM; one that waits longer than
+ * `timeout_ms` for the other ranks returns B200_ERR_COMM (b200_last_error names the generation and how many ranks
+ * arrived), and every later collective of the communicator then fails at once. */
+B200_API int32_t b200_comm_init_loopback(const char* path, int32_t rank, int32_t world, uint64_t slot_bytes, uint32_t timeout_ms);
 
 /* hash_tree_root(deneb::BeaconState) computed by all ranks of the communicator in ONE call (deneb/spec/mod.rs:3215,3288):
  * every rank passes the same serialization, uploads and hashes only its power-of-two-aligned slice of the five big
@@ -272,8 +282,8 @@ B200_API int32_t b200_fast_aggregate_verify_batch_mixed(const uint8_t* extra_pks
                                                         const uint32_t* offsets, const uint8_t* msgs32, const uint8_t* sigs,
                                                         size_t n_tuples, int32_t* out_codes);
 /* RLC whole-batch check over registry indices, and over all ranks of the communicator: every rank passes the same batch
- * and the same (non-NULL) seed, verifies its block, and ONE ncclAllGather moves the per-rank Gt partial (576 B) and G2
- * partial (288 B); every rank then finishes the same final exponentiation and returns the same boolean.  Rank k scales
+ * and the same (non-NULL) seed, verifies its block, and ONE ncclAllGather moves the per-rank Gt partial (576 B) and the
+ * rank's bad flag (16 B); every rank then finishes the same final exponentiation and returns the same boolean.  Rank k scales
  * its tuples with r_t of their global index t.  The sharded call requires the caller's seed, so the caller must draw it
  * unpredictably (for instance from the OS after the signatures are fixed) and share it among the ranks: a seed known to
  * whoever produced the signatures lets them build an all-invalid batch that is accepted. */

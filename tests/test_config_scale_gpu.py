@@ -13,7 +13,6 @@ import hashlib
 import json
 import os
 import subprocess
-import sys
 from pathlib import Path
 
 import numpy as np
@@ -166,15 +165,13 @@ def _gpu_count():
 
 
 @pytest.mark.skipif(_gpu_count() < 2, reason="needs >= 2 GPUs")
-def test_two_rank_sharded_calls_over_nccl(tmp_path):
+def test_two_rank_sharded_calls_over_nccl(tmp_path, oracle_bls_c, oracle_ssz_c):
     """Two processes, one GPU each, NO torch: the library's own communicator (id handed over through a file), then the
-    sharded state root and the sharded verify batch must agree with the single-GPU answers on both ranks."""
-    worker = ROOT / "tests" / "mp_sharded_worker.py"
-    procs = []
-    for r in range(2):
-        env = dict(os.environ, B200_TEST_RANK=str(r), B200_TEST_WORLD="2", B200_TEST_DIR=str(tmp_path), CUDA_VISIBLE_DEVICES=str(r))
-        procs.append(subprocess.Popen([sys.executable, str(worker)], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = [p.communicate(timeout=900)[0] for p in procs]
-    for r, (p, o) in enumerate(zip(procs, outs)):
-        assert p.returncode == 0, f"rank {r}:\n{o}"
-        assert "SHARDED_OK" in o, o
+    world-2 case list of tests/sharded_cases.py (states, strict verify, RLC, host all-gathers, refusals) through the
+    same worker the loopback test uses, with the same expected values on both ranks."""
+    from tests import sharded_cases as sh
+    from tests.test_sharded_loopback_gpu import check, run_ranks
+    data = sh.write_cases(tmp_path / "box", 2, oracle_bls_c, oracle_ssz_c)
+    ranks = run_ranks(tmp_path / "box", 2, transport="nccl", devices=[0, 1])
+    n, bad = check(ranks, data)
+    assert not bad, "\n".join(bad[:40])

@@ -193,22 +193,16 @@ def _gpu_count():
 
 
 @pytest.mark.skipif(_gpu_count() < 2, reason="needs >= 2 GPUs")
-def test_crafted_batch_on_two_ranks(oracle_bls_c, tmp_path):
-    """A family-A batch through the sharded call at world 2: each rank hashes its global t0 + t, so both accept it
-    under the crafting seed and both reject it under another seed."""
-    _, M, fam = soak(oracle_bls_c)
-    c = next(c for c in fam["A"] if c.name == "A (t, t+32) T 64")
-    other = next(s for s, w in c.runs if s is not None and not w)
-    (tmp_path / "case.pkl").write_bytes(pickle.dumps({"args": [np.ascontiguousarray(a) for a in M.pack(c.batch)], "seed": rc.SEED, "other": other}))
-    worker = ROOT / "tests" / "mp_rlc_sharded_worker.py"
-    procs = []
-    for r in range(2):
-        env = dict(os.environ, B200_TEST_RANK=str(r), B200_TEST_WORLD="2", B200_TEST_DIR=str(tmp_path), CUDA_VISIBLE_DEVICES=str(r))
-        procs.append(subprocess.Popen([sys.executable, str(worker)], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = [p.communicate(timeout=900)[0] for p in procs]
-    for r, (p, o) in enumerate(zip(procs, outs)):
-        assert p.returncode == 0, f"rank {r}:\n{o}"
-        assert "RLC_SHARDED_OK" in o, o
+def test_crafted_batch_on_two_ranks(oracle_bls_c, oracle_ssz_c, tmp_path):
+    """The RLC section of the world-2 case list (tests/sharded_cases.py) over NCCL, one GPU per rank: defects that cancel
+    only across the rank boundary under the crafting seed, so each rank must hash its global t0 + t; both ranks accept
+    them under that seed and reject them under the four others."""
+    from tests import sharded_cases as sh
+    from tests.test_sharded_loopback_gpu import check, run_ranks
+    data = sh.write_cases(tmp_path / "box", 2, oracle_bls_c, oracle_ssz_c)
+    ranks = run_ranks(tmp_path / "box", 2, transport="nccl", devices=[0, 1], sections=["rlc"])
+    n, bad = check(ranks, data, sections={"rlc"})
+    assert not bad, "\n".join(bad[:40])
 
 
 def _child(path):
