@@ -73,6 +73,9 @@ _PROTOS = {
     "b200_state_upload_deneb_sharded": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_int32, C.POINTER(C.c_void_p)]),
     "b200_fast_aggregate_verify_batch_sharded": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "b200_fast_aggregate_verify_batch_mixed": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200_aggregate_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    "b200_eth_aggregate_public_keys_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    "b200_registry_aggregate_public_keys": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     "b200_tune": (C.c_int32, [C.c_char_p, C.c_int64]),
     "b200_vm_load_programs": (C.c_int32, [C.c_void_p, C.c_size_t]),
 }

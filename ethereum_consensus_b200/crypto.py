@@ -192,6 +192,40 @@ def _batch_size(off, msgs32, sigs, keys=None, indices=None, seed=None) -> int:
     return t
 
 
+def _groups(offsets, items, item_bytes: int, what: str):
+    """uint32 offsets of T groups over `items` (flat `item_bytes`-byte items, or uint32 indices when item_bytes is 0)."""
+    off = np.ascontiguousarray(offsets, dtype=np.uint32)
+    t = len(off) - 1
+    if off.ndim != 1 or t < 0:
+        raise ValueError("offsets must hold T + 1 entries")
+    if int(off[0]) != 0:
+        raise ValueError("offsets must start at 0")
+    n = int(off[-1])
+    have = len(items) if item_bytes == 0 else _nbytes(items)
+    if have != (n if item_bytes == 0 else item_bytes * n):
+        raise ValueError(f"buffer sizes do not match the offsets: {n} {what} for {t} groups, got {have}")
+    return off, t
+
+
+def aggregate_batch(sigs_flat, offsets):
+    """`aggregate` over T groups: group t is signatures offsets[t] .. offsets[t+1]-1 of sigs_flat (96 bytes each).
+    -> (uint8[T, 96] compressed sums, int32[T] codes: 0, a decode code, 3 not in group, 16 empty); failed rows are zero."""
+    off, t = _groups(offsets, sigs_flat, 96, "signatures")
+    out, codes = np.zeros((max(t, 1), 96), dtype=np.uint8), np.zeros(max(t, 1), dtype=np.int32)
+    _lib.check(_lib.lib().b200_aggregate_batch(_lib.ptr(sigs_flat), _lib.ptr(off), t, _lib.ptr(out), _lib.ptr(codes)),
+               "aggregate_batch")
+    return out[:t], codes[:t]
+
+
+def eth_aggregate_public_keys_batch(pks_flat, offsets):
+    """`eth_aggregate_public_keys` over T groups of 48-byte keys -> (uint8[T, 48], int32[T])."""
+    off, t = _groups(offsets, pks_flat, 48, "keys")
+    out, codes = np.zeros((max(t, 1), 48), dtype=np.uint8), np.zeros(max(t, 1), dtype=np.int32)
+    _lib.check(_lib.lib().b200_eth_aggregate_public_keys_batch(_lib.ptr(pks_flat), _lib.ptr(off), t, _lib.ptr(out), _lib.ptr(codes)),
+               "eth_aggregate_public_keys_batch")
+    return out[:t], codes[:t]
+
+
 def fast_aggregate_verify_batch(pks_flat, pk_offsets, msgs32, sigs) -> np.ndarray:
     """T tuples at once -> int32 code per tuple (0 Ok, 5 InvalidSignature, 1/2/3/6 BLST decode errors).
     pks_flat: (sum K) x 48 bytes; pk_offsets: uint32[T+1]; msgs32: T x 32; sigs: T x 96 (host buffers)."""
@@ -260,6 +294,16 @@ class Registry:
         out = np.empty(max(self.n, 1), dtype=np.int32)
         _lib.check(_lib.lib().b200_registry_key_codes(_lib.ptr(out), self.n), "registry_key_codes")
         return out[:self.n]
+
+    def aggregate_public_keys(self, indices, offsets):
+        """`eth_aggregate_public_keys` over T groups of registry indices (group t: indices[offsets[t] .. offsets[t+1]-1])
+        -> (uint8[T, 48], int32[T]); each key keeps the code it was validated with."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint32)
+        off, t = _groups(offsets, idx, 0, "indices")
+        out, codes = np.zeros((max(t, 1), 48), dtype=np.uint8), np.zeros(max(t, 1), dtype=np.int32)
+        _lib.check(_lib.lib().b200_registry_aggregate_public_keys(_lib.ptr(idx), _lib.ptr(off), t, _lib.ptr(out), _lib.ptr(codes)),
+                   "registry_aggregate_public_keys")
+        return out[:t], codes[:t]
 
     def verify_batch(self, indices, offsets, msgs32, sigs, extra_keys=None) -> np.ndarray:
         """`extra_keys` (flat 48-byte keys): keys that arrive with the block (deposits, bls-to-execution changes); index

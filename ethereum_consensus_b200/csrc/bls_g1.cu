@@ -23,6 +23,7 @@
 #define B200_POW_TAB_SMEM 1
 #include <cuda_runtime.h>
 
+#include "../../include/b200_consensus.h"
 #include "bls_kernels.cuh"
 
 namespace b200 {
@@ -134,8 +135,18 @@ __global__ void __launch_bounds__(32 * kAggWarps) k_g1_aggregate(const G1Aff* __
     }
 }
 
-__global__ void k_g1_compress(const G1Aff* p, uint8_t* out48) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) g1_compress(out48, *p);
+// `eth_aggregate_public_keys` (crypto/bls.rs:135-148) after K2: one thread per group.  The first failing key's code, else
+// EMPTY_AGGREGATE for a group without keys, else the compressed sum; a failed or empty group's 48 bytes are zero.
+__global__ void k_g1_compress_groups(const G1Aff* __restrict__ agg, const int32_t* __restrict__ pk_code,
+                                     const uint32_t* __restrict__ flags, uint32_t n_groups, uint8_t* __restrict__ out48,
+                                     int32_t* __restrict__ out_code) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= n_groups) return;
+    uint8_t* o = out48 + size_t(g) * 48;
+    const int32_t rc = pk_code[g] != BLS_SUCCESS ? pk_code[g] : (flags[g] & TUPLE_FLAG_EMPTY) ? int32_t(B200_EMPTY_AGGREGATE) : BLS_SUCCESS;
+    out_code[g] = rc;
+    if (rc == BLS_SUCCESS) g1_compress(o, agg[g]);
+    else for (int k = 0; k < 48; k++) o[k] = 0;
 }
 __global__ void k_neg_g1(G1Aff* out, G1Pre* out_pre) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -367,8 +378,12 @@ void launch_g1_aggregate(const G1Aff* keys, const int32_t* key_codes, const uint
                      static_cast<cudaStream_t>(stream)>>>(
         keys, key_codes, index, off, n_tuples, agg, agg_pre, pk_code, flags, extra_flags, agg_jac);
 }
-void launch_g1_compress(const G1Aff* p, uint8_t* out48, void* stream) {
-    k_g1_compress<<<1, 32, with_pow_tab(k_g1_compress, 32), static_cast<cudaStream_t>(stream)>>>(p, out48);
+void launch_g1_compress_groups(const G1Aff* agg, const int32_t* pk_code, const uint32_t* flags, uint32_t n_groups, uint8_t* out48,
+                               int32_t* out_code, void* stream) {
+    if (!n_groups) return;
+    const unsigned t = n_groups <= 32 ? 32 : 128;
+    k_g1_compress_groups<<<(n_groups + t - 1) / t, t, with_pow_tab(k_g1_compress_groups, t), static_cast<cudaStream_t>(stream)>>>(
+        agg, pk_code, flags, n_groups, out48, out_code);
 }
 void launch_neg_g1(G1Aff* out, G1Pre* out_pre, void* stream) { k_neg_g1<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(out, out_pre); }
 void launch_fp_selftest(uint32_t n, uint32_t seed, uint32_t* out_mismatch, void* stream) {

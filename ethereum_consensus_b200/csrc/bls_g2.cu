@@ -14,6 +14,9 @@
 #define B200_TOWER_NOINLINE 1   // (a build with the curve routines inlined as well returned wrong verdicts on the GPU — not investigated, not offered)
 #include <cuda_runtime.h>
 
+#include <algorithm>
+
+#include "../../include/b200_consensus.h"
 #include "bls_kernels.cuh"
 #include "h2c.cuh"
 
@@ -67,44 +70,107 @@ __global__ void B200_G2_BOUNDS k_hash_to_g2_finish(const G2Jac* __restrict__ tmp
     out[i] = h;
 }
 
-// `aggregate` (crypto/bls.rs:79-93): every signature decoded already; group-check each (first failure in order
-// wins), sum, compress.  One warp: lanes stride, shared-memory tree.
-__global__ void __launch_bounds__(32) k_g2_sum_compress(const G2Aff* __restrict__ sigs, const int32_t* __restrict__ sig_code,
-                                                         uint32_t n, uint8_t* out96, int32_t* out_code) {
-    __shared__ G2Jac part[32];
-    const uint32_t lane = threadIdx.x;
-    uint32_t first_bad = 0xffffffffu;
-    for (uint32_t k = lane; k < n; k += 32)
-        if (sig_code[k] != SIG_OK) { first_bad = k; break; }
-    for (int s = 16; s > 0; s >>= 1) first_bad = min(first_bad, __shfl_xor_sync(0xffffffffu, first_bad, s));
-    // decode errors take precedence over group-check errors (all signatures are decoded before any is checked)
-    uint32_t first_dec = 0xffffffffu;
-    for (uint32_t k = lane; k < n; k += 32)
-        if (sig_code[k] > 0) { first_dec = k; break; }
-    for (int s = 16; s > 0; s >>= 1) first_dec = min(first_dec, __shfl_xor_sync(0xffffffffu, first_dec, s));
-    if (first_dec != 0xffffffffu) { if (lane == 0) *out_code = sig_code[first_dec]; return; }
-    if (first_bad != 0xffffffffu) { if (lane == 0) *out_code = BLS_POINT_NOT_IN_GROUP; return; }
+// `aggregate` (crypto/bls.rs:79-93) over T groups, every signature decoded already (k_g2_sig_decode).  Group g is split
+// into chunks of `chunk` signatures; one warp per chunk, so that a group of 32 768 signatures is summed by hundreds of
+// warps instead of one.  Chunks of a group are numbered chunk_off[g] .. chunk_off[g+1]-1, chunk_group[c] names the group.
+__device__ __forceinline__ void warp_min(uint32_t& v) {
+    for (int s = 16; s > 0; s >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, s));
+}
+__device__ __forceinline__ void shfl_xor_fp(Fp& d, const Fp& a, int s) {
+#pragma unroll
+    for (int k = 0; k < 12; k++) d.l[k] = __shfl_xor_sync(0xffffffffu, a.l[k], s);
+}
+// butterfly: every lane ends with the warp's sum (as a possibly different Jacobian representative of the same point)
+__device__ __forceinline__ void warp_sum(G2Jac& acc) {
+    for (int s = 16; s > 0; s >>= 1) {
+        G2Jac o;
+        shfl_xor_fp(o.x.c0, acc.x.c0, s); shfl_xor_fp(o.x.c1, acc.x.c1, s);
+        shfl_xor_fp(o.y.c0, acc.y.c0, s); shfl_xor_fp(o.y.c1, acc.y.c1, s);
+        shfl_xor_fp(o.z.c0, acc.z.c0, s); shfl_xor_fp(o.z.c1, acc.z.c1, s);
+        jac_add(acc, acc, o);
+    }
+}
+
+// The chunks' partial results are read back by another warp of the same launch: through L2 (ld.global.cg), never from a
+// possibly stale L1 line
+__device__ __forceinline__ void load_cg(G2Jac& q, const G2Jac* p) {
+    const uint4* s = reinterpret_cast<const uint4*>(p);
+    uint4* d = reinterpret_cast<uint4*>(&q);
+#pragma unroll
+    for (int k = 0; k < int(sizeof(G2Jac) / 16); k++) d[k] = __ldcg(s + k);
+}
+
+// One warp per chunk.  part_code[c] = the code of the chunk's first decode failure (> 0), else SIG_NOT_IN_GROUP if any of
+// its signatures failed the group check, else SIG_OK and part[c] = the Jacobian sum of its signatures.  The warp that
+// completes a group's last outstanding chunk (counter done[g], zero at launch) then finishes the group: decode errors take
+// precedence over group-check errors (every signature is decoded before any is checked, as blst's aggregate does), else
+// the chunk sums are added, normalised and compressed.  A failed or empty group's 96 bytes are zero.  Every group, empty
+// ones included, has at least one chunk.
+__global__ void B200_G2_BOUNDS k_g2_aggregate(const G2Aff* __restrict__ sigs, const int32_t* __restrict__ sig_code,
+                                              const uint32_t* __restrict__ off, const uint32_t* __restrict__ chunk_group,
+                                              const uint32_t* __restrict__ chunk_off, uint32_t n_chunks, uint32_t chunk,
+                                              G2Jac* part, int32_t* part_code, uint32_t* done, uint8_t* __restrict__ out96,
+                                              int32_t* __restrict__ out_code) {
+    const uint32_t c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (c >= n_chunks) return;  // whole warp exits together
+    const uint32_t g = chunk_group[c];
+    const uint32_t lo = off[g] + (c - chunk_off[g]) * chunk, hi = min(off[g + 1], lo + chunk);
+    uint32_t first_dec = 0xffffffffu, first_bad = 0xffffffffu;
+    for (uint32_t k = lo + lane; k < hi; k += 32) {
+        const int32_t rc = sig_code[k];
+        if (rc != SIG_OK && first_bad == 0xffffffffu) first_bad = k;
+        if (rc > 0) { first_dec = k; break; }
+    }
+    warp_min(first_dec);
+    warp_min(first_bad);
     G2Jac acc;
     jac_set_inf(acc);
-    for (uint32_t k = lane; k < n; k += 32) {
-        const G2Aff q = sigs[k];
-        if (!q.inf) jac_add_mixed(acc, acc, q.x, q.y);
-    }
-    part[lane] = acc;
-    __syncwarp();
-    for (int s = 16; s > 0; s >>= 1) {
-        if (lane < s) {
-            G2Jac a = part[lane], b = part[lane + s];
-            jac_add(a, a, b);
-            part[lane] = a;
+    if (first_bad == 0xffffffffu) {
+        for (uint32_t k = lo + lane; k < hi; k += 32) {
+            const G2Aff q = sigs[k];
+            if (!q.inf) jac_add_mixed(acc, acc, q.x, q.y);
         }
-        __syncwarp();
+        warp_sum(acc);
     }
+    uint32_t last = 0;
+    if (lane == 0) {
+        part[c] = acc;
+        part_code[c] = first_bad == 0xffffffffu ? SIG_OK : first_dec != 0xffffffffu ? sig_code[first_dec] : SIG_NOT_IN_GROUP;
+        __threadfence();   // this chunk's result is visible before the counter says so
+        last = atomicAdd(done + g, 1u) == chunk_off[g + 1] - chunk_off[g] - 1;
+    }
+    if (!__shfl_sync(0xffffffffu, last, 0)) return;
+    __threadfence();
+    // the group's finish
+    const uint32_t clo = chunk_off[g], chi = chunk_off[g + 1];
+    first_dec = 0xffffffffu;
+    bool bad = false;
+    for (uint32_t k = clo + lane; k < chi; k += 32) {
+        const int32_t rc = __ldcg(part_code + k);
+        bad = bad || rc != SIG_OK;
+        if (rc > 0) { first_dec = k; break; }
+    }
+    warp_min(first_dec);
+    bad = __any_sync(0xffffffffu, bad);
+    uint8_t* o = out96 + size_t(g) * 96;
+    if (off[g] == off[g + 1] || bad) {
+        if (lane == 0) out_code[g] = off[g] == off[g + 1] ? B200_EMPTY_AGGREGATE
+                                     : first_dec != 0xffffffffu ? __ldcg(part_code + first_dec) : int32_t(BLS_POINT_NOT_IN_GROUP);
+        o[3 * lane] = 0; o[3 * lane + 1] = 0; o[3 * lane + 2] = 0;
+        return;
+    }
+    jac_set_inf(acc);
+    for (uint32_t k = clo + lane; k < chi; k += 32) {
+        G2Jac q;
+        load_cg(q, part + k);
+        jac_add(acc, acc, q);
+    }
+    warp_sum(acc);
     if (lane == 0) {
         G2Aff a;
-        jac_to_aff(a, part[0]);
-        g2_compress(out96, a);
-        *out_code = BLS_SUCCESS;
+        jac_to_aff(a, acc);
+        g2_compress(o, a);
+        out_code[g] = BLS_SUCCESS;
     }
 }
 
@@ -204,8 +270,32 @@ void launch_hash_to_g2(const uint8_t* msgs, const uint32_t* moff, uint32_t n, G2
     k_hash_to_g2_map<<<(2 * n + threads - 1) / threads, threads, kPowTab, static_cast<cudaStream_t>(stream)>>>(msgs, moff, n, tmp);
     k_hash_to_g2_finish<<<(n + threads - 1) / threads, threads, kPowTab, static_cast<cudaStream_t>(stream)>>>(tmp, n, out);
 }
-void launch_g2_sum_compress(const G2Aff* sigs, const int32_t* sig_code, uint32_t n, uint8_t* out96, int32_t* out_code, void* stream) {
-    k_g2_sum_compress<<<1, 32, kPowTab, static_cast<cudaStream_t>(stream)>>>(sigs, sig_code, n, out96, out_code);
+// Warps of one launch of the aggregation kernels: 32-thread CTAs spread a few warps over every SM; from four per SM on,
+// 128-thread CTAs
+static uint32_t sm_count() {
+    static int n = 0;
+    if (!n) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1)
+            n = 132;
+    }
+    return uint32_t(n);
+}
+static int agg_cta(uint32_t warps) { return warps >= 4 * sm_count() ? 128 : 32; }
+
+// About eight warps per SM over the whole call, in whole warps' strides (the sum is ~1 % of the decode's work, so only its
+// latency matters); a group gets one chunk per `chunk` signatures
+uint32_t g2_aggregate_chunk(uint32_t n_sigs) {
+    const uint32_t warps = 8 * sm_count();
+    return 32u * std::max<uint32_t>(1u, (n_sigs + 32u * warps - 1) / (32u * warps));
+}
+void launch_g2_aggregate(const G2Aff* sigs, const int32_t* sig_code, const uint32_t* off, const uint32_t* chunk_group,
+                         const uint32_t* chunk_off, uint32_t n_chunks, uint32_t chunk, G2Jac* part, int32_t* part_code,
+                         uint32_t* done, uint8_t* out96, int32_t* out_code, void* stream) {
+    if (!n_chunks) return;
+    const int t = agg_cta(n_chunks);
+    k_g2_aggregate<<<(n_chunks + t / 32 - 1) / (t / 32), t, kPowTab, static_cast<cudaStream_t>(stream)>>>(
+        sigs, sig_code, off, chunk_group, chunk_off, n_chunks, chunk, part, part_code, done, out96, out_code);
 }
 void launch_fp2_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream) {
     if (!n) return;

@@ -66,9 +66,18 @@ void launch_vm_miller(const G1Pre* g1, const uint32_t* g1_idx, const G2Aff* g2, 
                       uint32_t n_pairs, Fp12* f, void* stream);
 void launch_vm_final(const Fp12* f, const uint32_t* pair_off, const int32_t* pk_code, const uint32_t* flags,
                      const int32_t* sig_code, uint32_t n_tuples, int32_t* out_codes, void* stream);
-// aggregation helpers for `aggregate` / `eth_aggregate_public_keys`
-void launch_g2_sum_compress(const G2Aff* sigs, const int32_t* sig_code, uint32_t n, uint8_t* out96, int32_t* out_code, void* stream);
-void launch_g1_compress(const G1Aff* p, uint8_t* out48, void* stream);
+// `aggregate` over T groups (group g: signatures off[g] .. off[g+1]-1, decoded by K3) in one launch: per chunk of
+// `chunk` signatures (g2_aggregate_chunk) its first failure and partial sum; the warp that completes a group's last chunk
+// writes the group's verdict and compressed sum (out96[96 g..], zero unless out_code[g] == 0).  Chunks of group g:
+// chunk_off[g] .. chunk_off[g+1]-1, at least one per group (empty groups too); chunk c belongs to chunk_group[c].
+// `part` / `part_code` hold n_chunks entries; `done` holds T counters, zero at launch.
+uint32_t g2_aggregate_chunk(uint32_t n_sigs);
+void launch_g2_aggregate(const G2Aff* sigs, const int32_t* sig_code, const uint32_t* off, const uint32_t* chunk_group,
+                         const uint32_t* chunk_off, uint32_t n_chunks, uint32_t chunk, G2Jac* part, int32_t* part_code,
+                         uint32_t* done, uint8_t* out96, int32_t* out_code, void* stream);
+// `eth_aggregate_public_keys` over T groups after K2 (affine sums, codes, flags): code and compressed sum per group
+void launch_g1_compress_groups(const G1Aff* agg, const int32_t* pk_code, const uint32_t* flags, uint32_t n_groups, uint8_t* out48,
+                               int32_t* out_code, void* stream);
 // writes -g1 (the negated generator) to *out (and its G1Pre form)
 void launch_neg_g1(G1Aff* out, G1Pre* out_pre, void* stream);
 // on-device self-test of Fp arithmetic (portable vs tuned paths), returns mismatches in *out

@@ -55,6 +55,8 @@ struct BlsState {
     DevBuf keys, key_aff, key_code, g1pts, g1pre, pk_code, flags, sigs, g2pts, sig_code, msgs, small, f, out, h2c_tmp, gath;
     // RLC whole-batch check (bls_rlc.cu): Jacobian aggregates, scaled points, reduction ping-pong, zeros, indices, exchange
     DevBuf rlc_jac, rlc_g1, rlc_q, rlc_fa, rlc_fb, rlc_qa, rlc_qb, rlc_zero, rlc_idx, rlc_misc, rlc_xch;
+    // batch aggregation: per-chunk partial sums and codes of the signature groups
+    DevBuf agg_part;
     PinnedBuf stage;
     G1Aff* d_negg1 = nullptr;
     G1Pre* d_negg1_pre = nullptr;
@@ -708,6 +710,112 @@ static int32_t check_indices(Engine& e, const BlsState& s, const uint32_t* index
     return B200_SUCCESS;
 }
 
+// ---- aggregation of T groups (aggregate / eth_aggregate_public_keys)
+
+// the batch aggregation entry points' checks; n_groups == 0 passes (and sets last_kernel_ms); *n: the item count
+static int32_t check_aggregate_args(Engine& e, const uint32_t* off, size_t n_groups, const uint8_t* out, const int32_t* codes,
+                                    uint32_t* n) {
+    e.last_kernel_ms = 0.f;
+    *n = 0;
+    if (n_groups == 0) return B200_SUCCESS;
+    if (!off || !out || !codes || n_groups > kMaxBatchTuples) return B200_ERR_BAD_ARG;
+    int32_t rc = check_offsets(off, n_groups, n);
+    if (rc) return rc;
+    if (*n > 0x3fffffffu) { e.last_error = "aggregate: more than 0x3fffffff items"; return B200_ERR_BAD_ARG; }
+    return B200_SUCCESS;
+}
+
+// device results of T groups (codes, then `bytes` per group) to the caller; last_kernel_ms from ev_k0 / ev_k1
+static int32_t aggregate_readback(Engine& e, BlsState& s, const void* d_codes, const void* d_bytes, uint32_t T, size_t bytes,
+                                  uint8_t* out, int32_t* out_codes) {
+    cudaStream_t sa = e.stream;
+    B200_CUDA_TRY(s.stage.reserve(size_t(T) * (4 + bytes)));
+    uint8_t* h = static_cast<uint8_t*>(s.stage.p);
+    B200_CUDA_TRY(cudaMemcpyAsync(h, d_codes, size_t(T) * 4, cudaMemcpyDeviceToHost, sa));
+    B200_CUDA_TRY(cudaMemcpyAsync(h + size_t(T) * 4, d_bytes, size_t(T) * bytes, cudaMemcpyDeviceToHost, sa));
+    B200_CUDA_TRY(cudaStreamSynchronize(sa));
+    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, s.ev_k0, s.ev_k1));
+    memcpy(out_codes, h, size_t(T) * 4);
+    memcpy(out, h + size_t(T) * 4, size_t(T) * bytes);
+    return B200_SUCCESS;
+}
+
+// n signatures (host), T groups by `off` (host): K3 over all n, then the chunked sum and the per-group finish
+static int32_t aggregate_sigs(Engine& e, BlsState& s, const uint8_t* sigs, uint32_t n, const uint32_t* off, uint32_t T,
+                              uint8_t* out96, int32_t* out_codes) {
+    const uint32_t chunk = g2_aggregate_chunk(n);
+    // small array: offsets (T + 1) | chunk_off (T + 1) | chunk_group (n_chunks)
+    std::vector<uint32_t> small(off, off + T + 1);
+    small.push_back(0);
+    auto chunks_of = [&](uint32_t g) { return std::max<uint32_t>(1u, (off[g + 1] - off[g] + chunk - 1) / chunk); };
+    for (uint32_t g = 0; g < T; g++) small.push_back(small.back() + chunks_of(g));
+    const uint32_t n_chunks = small.back();
+    for (uint32_t g = 0; g < T; g++) small.insert(small.end(), chunks_of(g), g);
+    B200_CUDA_TRY(s.sigs.reserve(size_t(n) * 96 + 64));
+    B200_CUDA_TRY(s.g2pts.reserve((size_t(n) + 1) * sizeof(G2Aff)));
+    B200_CUDA_TRY(s.sig_code.reserve((size_t(n) + 1) * 4));
+    B200_CUDA_TRY(s.small.reserve(small.size() * 4 + 64));
+    B200_CUDA_TRY(s.agg_part.reserve((size_t(n_chunks) + 1) * (sizeof(G2Jac) + 4) + size_t(T) * 4));
+    B200_CUDA_TRY(s.out.reserve(size_t(T) * (96 + 4) + 64));
+    cudaStream_t sa = e.stream;
+    uint32_t* d_small = static_cast<uint32_t*>(s.small.p);
+    B200_CUDA_TRY(cudaMemcpyAsync(d_small, small.data(), small.size() * 4, cudaMemcpyHostToDevice, sa));
+    if (n) B200_CUDA_TRY(cudaMemcpyAsync(s.sigs.p, sigs, size_t(n) * 96, cudaMemcpyHostToDevice, sa));
+    G2Jac* part = static_cast<G2Jac*>(s.agg_part.p);
+    int32_t* part_code = reinterpret_cast<int32_t*>(part + n_chunks);
+    uint32_t* done = reinterpret_cast<uint32_t*>(part_code + n_chunks);
+    B200_CUDA_TRY(cudaMemsetAsync(done, 0, size_t(T) * 4, sa));
+    int32_t* d_codes = static_cast<int32_t*>(s.out.p);
+    uint8_t* d_out96 = static_cast<uint8_t*>(s.out.p) + size_t(T) * 4;
+    B200_CUDA_TRY(cudaEventRecord(s.ev_k0, sa));
+    launch_g2_sig_decode(static_cast<const uint8_t*>(s.sigs.p), n, static_cast<G2Aff*>(s.g2pts.p), static_cast<int32_t*>(s.sig_code.p), sa);
+    launch_g2_aggregate(static_cast<const G2Aff*>(s.g2pts.p), static_cast<const int32_t*>(s.sig_code.p), d_small, d_small + 2 * T + 2,
+                        d_small + T + 1, n_chunks, chunk, part, part_code, done, d_out96, d_codes, sa);
+    e.launches += (n ? 1 : 0) + 1;
+    B200_CUDA_TRY(cudaEventRecord(s.ev_k1, sa));
+    B200_CUDA_TRY(cudaGetLastError());
+    return aggregate_readback(e, s, d_codes, d_out96, T, 96, out96, out_codes);
+}
+
+// n keys, T groups by `off` (host): strict (`keys`: K1 over all n, then K2 over the call's points) or from the registry
+// (`index`: K2 gathers the resident points and codes), then one compression thread per group
+static int32_t aggregate_keys(Engine& e, BlsState& s, bool registry, const uint8_t* keys, const uint32_t* index, uint32_t n,
+                              const uint32_t* off, uint32_t T, uint8_t* out48, int32_t* out_codes) {
+    const bool strict = !registry;
+    const size_t n_small = size_t(T) + 1 + (registry ? n : 0);
+    B200_CUDA_TRY(s.small.reserve(n_small * 4 + 64));
+    B200_CUDA_TRY(s.g1pts.reserve(size_t(T) * sizeof(G1Aff) + 64));
+    B200_CUDA_TRY(s.pk_code.reserve(size_t(T) * 4 + 64));
+    B200_CUDA_TRY(s.flags.reserve(size_t(T) * 4 + 64));
+    B200_CUDA_TRY(s.out.reserve(size_t(T) * (48 + 4) + 64));
+    if (strict) {
+        B200_CUDA_TRY(s.keys.reserve(size_t(n) * 48 + 64));
+        B200_CUDA_TRY(s.key_aff.reserve((size_t(n) + 1) * sizeof(G1Aff)));
+        B200_CUDA_TRY(s.key_code.reserve((size_t(n) + 1) * 4));
+    }
+    cudaStream_t sa = e.stream;
+    uint32_t* d_off = static_cast<uint32_t*>(s.small.p);
+    B200_CUDA_TRY(cudaMemcpyAsync(d_off, off, (size_t(T) + 1) * 4, cudaMemcpyHostToDevice, sa));
+    if (registry && n) B200_CUDA_TRY(cudaMemcpyAsync(d_off + T + 1, index, size_t(n) * 4, cudaMemcpyHostToDevice, sa));
+    if (strict && n) B200_CUDA_TRY(cudaMemcpyAsync(s.keys.p, keys, size_t(n) * 48, cudaMemcpyHostToDevice, sa));
+    int32_t* d_codes = static_cast<int32_t*>(s.out.p);
+    uint8_t* d_out48 = static_cast<uint8_t*>(s.out.p) + size_t(T) * 4;
+    B200_CUDA_TRY(cudaEventRecord(s.ev_k0, sa));
+    if (strict) {
+        launch_g1_validate(static_cast<const uint8_t*>(s.keys.p), n, static_cast<G1Aff*>(s.key_aff.p), static_cast<int32_t*>(s.key_code.p), sa);
+        e.launches += n ? 1 : 0;
+    }
+    launch_g1_aggregate(static_cast<const G1Aff*>(strict ? s.key_aff.p : s.reg_aff.p), static_cast<const int32_t*>(strict ? s.key_code.p : s.reg_code.p),
+                        registry ? d_off + T + 1 : nullptr, d_off, T, static_cast<G1Aff*>(s.g1pts.p), nullptr,
+                        static_cast<int32_t*>(s.pk_code.p), static_cast<uint32_t*>(s.flags.p), 0u, sa);
+    launch_g1_compress_groups(static_cast<const G1Aff*>(s.g1pts.p), static_cast<const int32_t*>(s.pk_code.p),
+                              static_cast<const uint32_t*>(s.flags.p), T, d_out48, d_codes, sa);
+    e.launches += 2;
+    B200_CUDA_TRY(cudaEventRecord(s.ev_k1, sa));
+    B200_CUDA_TRY(cudaGetLastError());
+    return aggregate_readback(e, s, d_codes, d_out48, T, 48, out48, out_codes);
+}
+
 static void rlc_seed(const uint8_t* seed32, uint8_t out[32]) {
     if (seed32) { memcpy(out, seed32, 32); return; }
     std::random_device rd;   // the scalars must be unpredictable to whoever produced the signatures
@@ -1268,78 +1376,88 @@ int32_t b200_aggregate_verify(const uint8_t* pks_flat, size_t n_pks, const uint8
     return rc ? rc : code;
 }
 
-// crypto/bls.rs:79-93
+// crypto/bls.rs:79-93: the batch path with one group
 int32_t b200_aggregate(const uint8_t* sigs_flat, size_t n, uint8_t out[96]) {
-    Engine& e = engine();
-    Guard g(e);
-    int32_t rc = check_ready(e);
-    if (rc) return rc;
-    if (n == 0) return B200_EMPTY_AGGREGATE;
+    if (n == 0) {
+        Engine& e = engine();
+        Guard g(e);
+        const int32_t rc = check_ready(e);
+        return rc ? rc : B200_EMPTY_AGGREGATE;
+    }
     if (!sigs_flat || !out || n > 0x3fffffffu) return B200_ERR_BAD_ARG;
-    BlsState* s;
-    rc = bls_state(e, &s);
+    const uint32_t off[2] = {0, uint32_t(n)};
+    uint8_t agg[96];
+    int32_t code = B200_ERR_CUDA;
+    const int32_t rc = b200_aggregate_batch(sigs_flat, off, 1, agg, &code);
     if (rc) return rc;
-    B200_CUDA_TRY(s->sigs.reserve(n * 96 + 64));
-    B200_CUDA_TRY(s->g2pts.reserve((n + 1) * sizeof(G2Aff)));
-    B200_CUDA_TRY(s->sig_code.reserve((n + 1) * 4));
-    B200_CUDA_TRY(s->out.reserve(256));
-    B200_CUDA_TRY(s->stage.reserve(256));
-    cudaStream_t sa = e.stream;
-    B200_CUDA_TRY(cudaMemcpyAsync(s->sigs.p, sigs_flat, n * 96, cudaMemcpyHostToDevice, sa));
-    launch_g2_sig_decode(static_cast<const uint8_t*>(s->sigs.p), uint32_t(n), static_cast<G2Aff*>(s->g2pts.p),
-                         static_cast<int32_t*>(s->sig_code.p), sa);
-    uint8_t* d_out = static_cast<uint8_t*>(s->out.p);
-    launch_g2_sum_compress(static_cast<const G2Aff*>(s->g2pts.p), static_cast<const int32_t*>(s->sig_code.p), uint32_t(n),
-                           d_out + 16, reinterpret_cast<int32_t*>(d_out), sa);
-    e.launches += 2;
-    B200_CUDA_TRY(cudaGetLastError());
-    B200_CUDA_TRY(cudaMemcpyAsync(s->stage.p, d_out, 16 + 96, cudaMemcpyDeviceToHost, sa));
-    B200_CUDA_TRY(cudaStreamSynchronize(sa));
-    const int32_t code = *static_cast<const int32_t*>(s->stage.p);
-    if (code == B200_SUCCESS) memcpy(out, static_cast<const uint8_t*>(s->stage.p) + 16, 96);
+    if (code == B200_SUCCESS) memcpy(out, agg, 96);
     return code;
 }
 
-// crypto/bls.rs:135-148
+// crypto/bls.rs:135-148: the batch path with one group
 int32_t b200_eth_aggregate_public_keys(const uint8_t* pks_flat, size_t n, uint8_t out[48]) {
+    if (n == 0) {
+        Engine& e = engine();
+        Guard g(e);
+        const int32_t rc = check_ready(e);
+        return rc ? rc : B200_EMPTY_AGGREGATE;
+    }
+    if (!pks_flat || !out || n > 0x3fffffffu) return B200_ERR_BAD_ARG;
+    const uint32_t off[2] = {0, uint32_t(n)};
+    uint8_t agg[48];
+    int32_t code = B200_ERR_CUDA;
+    const int32_t rc = b200_eth_aggregate_public_keys_batch(pks_flat, off, 1, agg, &code);
+    if (rc) return rc;
+    if (code == B200_SUCCESS) memcpy(out, agg, 48);
+    return code;
+}
+
+int32_t b200_aggregate_batch(const uint8_t* sigs_flat, const uint32_t* offsets, size_t n_groups, uint8_t* out96, int32_t* out_codes) {
     Engine& e = engine();
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (n == 0) return B200_EMPTY_AGGREGATE;
-    if (!pks_flat || !out || n > 0x3fffffffu) return B200_ERR_BAD_ARG;
+    uint32_t n;
+    if ((rc = check_aggregate_args(e, offsets, n_groups, out96, out_codes, &n))) return rc;
+    if (n_groups == 0) return B200_SUCCESS;
+    if (n && !sigs_flat) return B200_ERR_BAD_ARG;
     BlsState* s;
     rc = bls_state(e, &s);
     if (rc) return rc;
-    B200_CUDA_TRY(s->keys.reserve(n * 48 + 64));
-    B200_CUDA_TRY(s->key_aff.reserve((n + 1) * sizeof(G1Aff)));
-    B200_CUDA_TRY(s->key_code.reserve((n + 1) * 4));
-    B200_CUDA_TRY(s->g1pts.reserve(2 * sizeof(G1Aff)));
-    B200_CUDA_TRY(s->pk_code.reserve(16));
-    B200_CUDA_TRY(s->flags.reserve(16));
-    B200_CUDA_TRY(s->small.reserve(64));
-    B200_CUDA_TRY(s->out.reserve(256));
-    B200_CUDA_TRY(s->stage.reserve(256));
-    cudaStream_t sa = e.stream;
-    uint32_t* h = static_cast<uint32_t*>(s->stage.p);
-    h[0] = 0; h[1] = uint32_t(n);
-    B200_CUDA_TRY(cudaMemcpyAsync(s->small.p, h, 8, cudaMemcpyHostToDevice, sa));
-    B200_CUDA_TRY(cudaMemcpyAsync(s->keys.p, pks_flat, n * 48, cudaMemcpyHostToDevice, sa));
-    launch_g1_validate(static_cast<const uint8_t*>(s->keys.p), uint32_t(n), static_cast<G1Aff*>(s->key_aff.p),
-                       static_cast<int32_t*>(s->key_code.p), sa);
-    launch_g1_aggregate(static_cast<const G1Aff*>(s->key_aff.p), static_cast<const int32_t*>(s->key_code.p), nullptr,
-                        static_cast<const uint32_t*>(s->small.p), 1, static_cast<G1Aff*>(s->g1pts.p), nullptr,
-                        static_cast<int32_t*>(s->pk_code.p), static_cast<uint32_t*>(s->flags.p), 0u, sa);
-    uint8_t* d_out = static_cast<uint8_t*>(s->out.p);
-    launch_g1_compress(static_cast<const G1Aff*>(s->g1pts.p), d_out, sa);
-    e.launches += 3;
-    B200_CUDA_TRY(cudaGetLastError());
-    B200_CUDA_TRY(cudaMemcpyAsync(h + 4, s->pk_code.p, 4, cudaMemcpyDeviceToHost, sa));
-    B200_CUDA_TRY(cudaMemcpyAsync(h + 8, d_out, 48, cudaMemcpyDeviceToHost, sa));
-    B200_CUDA_TRY(cudaStreamSynchronize(sa));
-    const int32_t code = int32_t(h[4]);
-    if (code == B200_SUCCESS) memcpy(out, h + 8, 48);
-    return code;
+    return aggregate_sigs(e, *s, sigs_flat, n, offsets, uint32_t(n_groups), out96, out_codes);
+}
+
+int32_t b200_eth_aggregate_public_keys_batch(const uint8_t* pks_flat, const uint32_t* offsets, size_t n_groups, uint8_t* out48,
+                                             int32_t* out_codes) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    uint32_t n;
+    if ((rc = check_aggregate_args(e, offsets, n_groups, out48, out_codes, &n))) return rc;
+    if (n_groups == 0) return B200_SUCCESS;
+    if (n && !pks_flat) return B200_ERR_BAD_ARG;
+    BlsState* s;
+    rc = bls_state(e, &s);
+    if (rc) return rc;
+    return aggregate_keys(e, *s, false, pks_flat, nullptr, n, offsets, uint32_t(n_groups), out48, out_codes);
+}
+
+int32_t b200_registry_aggregate_public_keys(const uint32_t* indices, const uint32_t* offsets, size_t n_groups, uint8_t* out48,
+                                            int32_t* out_codes) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    uint32_t n;
+    if ((rc = check_aggregate_args(e, offsets, n_groups, out48, out_codes, &n))) return rc;
+    if (n_groups == 0) return B200_SUCCESS;
+    if (n && !indices) return B200_ERR_BAD_ARG;
+    BlsState* s;
+    rc = bls_state(e, &s);
+    if (rc) return rc;
+    if ((rc = check_indices(e, *s, indices, n, 0))) return rc;
+    return aggregate_keys(e, *s, true, nullptr, indices, n, offsets, uint32_t(n_groups), out48, out_codes);
 }
 
 }  // extern "C"

@@ -227,6 +227,25 @@ B200_API int32_t b200_aggregate_verify(const uint8_t* pks_flat, size_t n_pks, co
 B200_API int32_t b200_aggregate(const uint8_t* sigs_flat, size_t n, uint8_t out[96]);
 /* eth_aggregate_public_keys — crypto/bls.rs:135-148 */
 B200_API int32_t b200_eth_aggregate_public_keys(const uint8_t* pks_flat, size_t n, uint8_t out[48]);
+/* aggregate (crypto/bls.rs:79-93) over T groups: group t is signatures offsets[t] .. offsets[t+1]-1 of sigs_flat
+ * (96 bytes each).  out_codes[t] and out96[96t..] are exactly what b200_aggregate returns for that group's bytes:
+ * 0 and the compressed sum; 16 (EMPTY_AGGREGATE) for an empty group; otherwise the decode code of the first
+ * signature that does not decode, else 3 (POINT_NOT_IN_GROUP).  out96 of a failed group is zero-filled.
+ * b200_aggregate and b200_eth_aggregate_public_keys are the T = 1 case of these calls.
+ * Arguments as on the verify batches: T + 1 non-decreasing offsets, T <= 2^26, offsets[T] <= 0x3fffffff items, and a
+ * NULL pointer with a non-zero count -> B200_ERR_BAD_ARG; n_groups == 0 succeeds and changes nothing.  The return value
+ * is B200_SUCCESS or an engine error (>= 0x100); each call sets b200_last_kernel_ms to the device time of its kernels. */
+B200_API int32_t b200_aggregate_batch(const uint8_t* sigs_flat, const uint32_t* offsets, size_t n_groups,
+                                      uint8_t* out96, int32_t* out_codes);
+/* eth_aggregate_public_keys (crypto/bls.rs:135-148) over T groups of 48-byte keys; per group exactly
+ * b200_eth_aggregate_public_keys. */
+B200_API int32_t b200_eth_aggregate_public_keys_batch(const uint8_t* pks_flat, const uint32_t* offsets, size_t n_groups,
+                                                      uint8_t* out48, int32_t* out_codes);
+/* The same over keys named by registry (validator) index: no key crosses PCIe or is validated again.  Each key keeps
+ * the code it was given at load / append, so out_codes[t] equals b200_eth_aggregate_public_keys on the same key bytes,
+ * invalid keys included.  An index >= reg_n -> B200_ERR_BAD_ARG for the call. */
+B200_API int32_t b200_registry_aggregate_public_keys(const uint32_t* indices, const uint32_t* offsets, size_t n_groups,
+                                                     uint8_t* out48, int32_t* out_codes);
 
 /* The throughput path: T independent fast_aggregate_verify tuples in one call (the batch of attestation checks
  * `process_block` issues one by one at deneb/block_processing.rs:104-108).  Tuple t uses public keys
