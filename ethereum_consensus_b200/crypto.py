@@ -41,6 +41,9 @@ _lib.register_protos({
     "b200_registry_sync_state": (C.c_int32, [C.c_void_p]),
     "b200_registry_key_codes": (C.c_int32, [C.c_void_p, C.c_size_t]),
     "b200_fast_aggregate_verify_batch_indexed": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200_aggregate_verify_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "b200_aggregate_verify_batch_indexed": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                        C.c_void_p]),
     "b200_fast_aggregate_verify_batch_all": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int32)]),
     "b200_fast_aggregate_verify_batch_indexed_all": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int32)]),
     "b200_fast_aggregate_verify_batch_all_sharded": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int32)]),
@@ -256,6 +259,36 @@ def fast_aggregate_verify_batch_all(pks_flat, pk_offsets, msgs32, sigs, seed: by
     return bool(ok.value)
 
 
+def _messages(msgs, msg_group, t: int):
+    """Flat bytes and uint32[n + 1] byte offsets of the messages (a sequence of bytes), and their T + 1 group offsets."""
+    grp = np.ascontiguousarray(msg_group, dtype=np.uint32)
+    if grp.ndim != 1 or len(grp) != t + 1:
+        raise ValueError(f"msg_group must hold T + 1 = {t + 1} entries, got {len(grp)}")
+    if int(grp[0]) != 0 or int(grp[-1]) != len(msgs):
+        raise ValueError(f"msg_group must run from 0 to the {len(msgs)} messages")
+    lens = [len(m) for m in msgs]
+    moff = np.zeros(len(msgs) + 1, dtype=np.uint64)
+    np.cumsum(lens, out=moff[1:])
+    if int(moff[-1]) > 0xFFFFFFFF:
+        raise ValueError("messages exceed 4 GiB in total")
+    flat = np.frombuffer(b"".join(bytes(m) for m in msgs), dtype=np.uint8)
+    return flat, moff.astype(np.uint32), grp
+
+
+def aggregate_verify_batch(pks_flat, pk_offsets, msgs, msg_group, sigs) -> np.ndarray:
+    """`aggregate_verify` over T tuples at once -> int32 code per tuple, as `aggregate_verify` would decide it (0 Ok,
+    5 InvalidSignature, 1/2/3/6 BLST decode errors).  Tuple t: keys pk_offsets[t] .. pk_offsets[t+1]-1 of pks_flat (48 bytes
+    each), messages msg_group[t] .. msg_group[t+1]-1 of `msgs` (a sequence of bytes, any lengths), signature sigs[96 t ..]."""
+    off, t = _groups(pk_offsets, pks_flat, 48, "keys")
+    if _nbytes(sigs) != 96 * t:
+        raise ValueError(f"sigs must hold {t} x 96 bytes, got {_nbytes(sigs)}")
+    flat, moff, grp = _messages(msgs, msg_group, t)
+    out = np.empty(max(t, 1), dtype=np.int32)
+    _lib.check(_lib.lib().b200_aggregate_verify_batch(_lib.ptr(pks_flat), _lib.ptr(off), _lib.ptr(flat), _lib.ptr(moff), _lib.ptr(grp),
+                                                      _lib.ptr(sigs), t, _lib.ptr(out)), "aggregate_verify_batch")
+    return out[:t]
+
+
 class Registry:
     """Validated validator public keys resident in HBM (`state.validators[i].public_key` is immutable,
     phase0/validator.rs:10-13): `load` runs key_validate once per key, `verify_batch` names signers by index.
@@ -320,6 +353,19 @@ class Registry:
         else:
             _lib.check(_lib.lib().b200_fast_aggregate_verify_batch_indexed(_lib.ptr(idx), _lib.ptr(off), _lib.ptr(msgs32),
                                                                            _lib.ptr(sigs), t, _lib.ptr(out)), "verify_batch_indexed")
+        return out[:t]
+
+    def aggregate_verify_batch(self, indices, offsets, msgs, msg_group, sigs) -> np.ndarray:
+        """`aggregate_verify_batch` with tuple t's keys named by registry indices indices[offsets[t] .. offsets[t+1]-1]."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint32)
+        off, t = _groups(offsets, idx, 0, "indices")
+        if _nbytes(sigs) != 96 * t:
+            raise ValueError(f"sigs must hold {t} x 96 bytes, got {_nbytes(sigs)}")
+        flat, moff, grp = _messages(msgs, msg_group, t)
+        out = np.empty(max(t, 1), dtype=np.int32)
+        _lib.check(_lib.lib().b200_aggregate_verify_batch_indexed(_lib.ptr(idx), _lib.ptr(off), _lib.ptr(flat), _lib.ptr(moff),
+                                                                  _lib.ptr(grp), _lib.ptr(sigs), t, _lib.ptr(out)),
+                   "aggregate_verify_batch_indexed")
         return out[:t]
 
     def verify_batch_all(self, indices, offsets, msgs32, sigs, seed: bytes = None) -> bool:
@@ -393,13 +439,14 @@ PAIRING_EVAL_OPS = {"fp6_mul": 0, "fp6_inv": 1, "fp12_mul": 2, "fp12_sqr": 3, "f
                     "fp12_frobenius1": 6, "fp12_frobenius2": 7, "fp12_cyclotomic_sqr": 8, "fp12_pow_z": 9,
                     "miller_double_step": 10, "miller_add_step": 11, "miller_loop": 12, "final_exp": 13,
                     "vm_miller8": 32, "vm_miller16": 33, "vm_final8": 34, "vm_final16": 35,
-                    "fold_fp12": 48, "fold_g2": 49}
+                    "fold_fp12": 48, "fold_g2": 49, "fold_segments": 50}
 
 
 def pairing_eval(op: str, a, b=None) -> np.ndarray:
     """Self-test: one device pairing operation on raw limbs.  a, b: uint32[n, 145] (twelve 12-word Fp slots in Fp12
     memory order, then the infinity flag of a point); returns uint32[n, 145]: the result's slots, then the flag word (the
-    final exponentiation's verdict, or the infinity flag of the G2 fold's sum).  The folds return their one result in row 0."""
+    final exponentiation's verdict, or the infinity flag of the G2 fold's sum).  The folds return their one result in row 0;
+    fold_segments takes the segment count T and T + 1 offsets as the first words of b and returns rows 2t, 2t + 1."""
     a = np.ascontiguousarray(a, dtype=np.uint32)
     b = np.zeros_like(a) if b is None else np.ascontiguousarray(b, dtype=np.uint32)
     if a.ndim != 2 or a.shape[1] != 145 or b.shape != a.shape:

@@ -70,7 +70,8 @@ __global__ void __launch_bounds__(32 * kAggWarps) k_g1_aggregate(const G1Aff* __
                                                                   G1Aff* __restrict__ agg, G1Pre* __restrict__ agg_pre,
                                                                   int32_t* __restrict__ pk_code,
                                                                   uint32_t* __restrict__ flags, uint32_t extra_flags,
-                                                                  G1Jac* __restrict__ agg_jac) {
+                                                                  G1Jac* __restrict__ agg_jac,
+                                                                  const uint32_t* __restrict__ tuple_flags) {
     __shared__ G1Jac part[kAggWarps][32];
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t t = blockIdx.x * kAggWarps + warp;
@@ -90,6 +91,7 @@ __global__ void __launch_bounds__(32 * kAggWarps) k_g1_aggregate(const G1Aff* __
         }
         return;
     }
+    if (tuple_flags) extra_flags |= tuple_flags[t];
     if (agg == nullptr && agg_pre == nullptr) {  // code scan only
         if (lane == 0) { pk_code[t] = BLS_SUCCESS; flags[t] = (hi == lo ? TUPLE_FLAG_EMPTY : 0u) | extra_flags; }
         return;
@@ -147,6 +149,20 @@ __global__ void k_g1_compress_groups(const G1Aff* __restrict__ agg, const int32_
     out_code[g] = rc;
     if (rc == BLS_SUCCESS) g1_compress(o, agg[g]);
     else for (int k = 0; k < 48; k++) o[k] = 0;
+}
+// aggregate_verify batches: one thread per key of the call, its pair's G1 operand (launch_g1_pair_operands).  Keys that
+// failed validation are converted as well; their tuples are dead and no pairing kernel reads them.
+__global__ void k_g1_pair_operands(const G1Aff* __restrict__ keys, const uint32_t* __restrict__ index, uint32_t n,
+                                   G1Pre* __restrict__ pre, G1Aff* __restrict__ aff) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const G1Aff a = keys[index ? index[i] : i];
+    if (pre) {
+        G1Pre p;
+        p.xz = a.x; p.y = a.y; p.z3 = fp_one(); p.inf = a.inf;
+        pre[i] = p;
+    }
+    if (aff) aff[i] = a;
 }
 __global__ void k_neg_g1(G1Aff* out, G1Pre* out_pre) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -372,11 +388,15 @@ void launch_gather_validator_keys(const uint8_t* records, uint32_t n, uint8_t* k
 }
 void launch_g1_aggregate(const G1Aff* keys, const int32_t* key_codes, const uint32_t* index, const uint32_t* off,
                          uint32_t n_tuples, G1Aff* agg, G1Pre* agg_pre, int32_t* pk_code, uint32_t* flags,
-                         uint32_t extra_flags, void* stream, G1Jac* agg_jac) {
+                         uint32_t extra_flags, void* stream, G1Jac* agg_jac, const uint32_t* tuple_flags) {
     if (!n_tuples) return;
     k_g1_aggregate<<<(n_tuples + kAggWarps - 1) / kAggWarps, 32 * kAggWarps, with_pow_tab(k_g1_aggregate, 32 * kAggWarps),
                      static_cast<cudaStream_t>(stream)>>>(
-        keys, key_codes, index, off, n_tuples, agg, agg_pre, pk_code, flags, extra_flags, agg_jac);
+        keys, key_codes, index, off, n_tuples, agg, agg_pre, pk_code, flags, extra_flags, agg_jac, tuple_flags);
+}
+void launch_g1_pair_operands(const G1Aff* keys, const uint32_t* index, uint32_t n, G1Pre* pre, G1Aff* aff, void* stream) {
+    if (!n) return;
+    k_g1_pair_operands<<<(n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(keys, index, n, pre, aff);
 }
 void launch_g1_compress_groups(const G1Aff* agg, const int32_t* pk_code, const uint32_t* flags, uint32_t n_groups, uint8_t* out48,
                                int32_t* out_code, void* stream) {

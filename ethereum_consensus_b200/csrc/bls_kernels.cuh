@@ -35,15 +35,27 @@ void launch_gather_validator_keys(const uint8_t* records, uint32_t n, uint8_t* k
 //     first failing key (in order) decides pk_code[t]
 //     agg == nullptr: only the code scan (aggregate_verify keeps keys separate); extra_flags is OR-ed into flags
 //     agg_pre != nullptr: write the un-normalised sum for the VM Miller kernel instead of the affine point
+//     tuple_flags != nullptr: per-tuple flags OR-ed into flags[t] as well (aggregate_verify batches: a tuple whose key and
+//     message counts differ is flagged EMPTY)
 void launch_g1_aggregate(const G1Aff* keys, const int32_t* key_codes, const uint32_t* index, const uint32_t* off,
                          uint32_t n_tuples, G1Aff* agg, G1Pre* agg_pre, int32_t* pk_code, uint32_t* flags,
-                         uint32_t extra_flags, void* stream, G1Jac* agg_jac = nullptr);
+                         uint32_t extra_flags, void* stream, G1Jac* agg_jac = nullptr, const uint32_t* tuple_flags = nullptr);
+// aggregate_verify batches: the G1 operand of key i's pair, keys[i] (or keys[index[i]] when index is non-null), as the VM
+// Miller kernel's G1Pre (x, y, 1) into pre[i] and / or as the affine point into aff[i] (either may be null)
+void launch_g1_pair_operands(const G1Aff* keys, const uint32_t* index, uint32_t n, G1Pre* pre, G1Aff* aff, void* stream);
 // RLC whole-batch check (bls_rlc.cu): scale per tuple, fold 32 -> 1 per launch, sum -> affine
 void launch_rlc_scale(const G1Jac* agg, const G2Aff* sig, const int32_t* pk_code, const uint32_t* flags, const int32_t* sig_code,
                       const uint32_t* seed_words, uint64_t t0, uint32_t n, G1Pre* out_g1, G2Jac* out_g2, int32_t* bad, void* stream);
 uint32_t launch_rlc_reduce(const Fp12* f_in, const G2Jac* q_in, uint32_t n, Fp12* f_out, G2Jac* q_out, void* stream);
 void launch_rlc_finish(const G2Jac* q, G2Aff* out, void* stream);
 void launch_fp12_one(Fp12* out, void* stream);
+// Segmented Gt product, one level (bls_rlc.cu): segment t holds values in[seg_in[t] .. seg_in[t+1]) of the n_in inputs and
+// seg_of[i] names value i's segment.  Each 32-value chunk of the input goes to one warp; the part ("piece") of a segment
+// inside chunk c, its k-th, leaves as one product: to out[seg_out[t] + k], or with seg_out == nullptr (a level after which
+// every segment has at most two pieces) to out[2t + k], with Fp12 one at out[2t + 1] for a segment of one piece -- the
+// layout launch_vm_final reads with pair_off[t] = 2t.  With pk_code non-null the segments of failed tuples are skipped.
+void launch_fold_segments(const Fp12* in, uint32_t n_in, const uint32_t* seg_of, const uint32_t* seg_in, const uint32_t* seg_out,
+                          const int32_t* pk_code, const uint32_t* flags, const int32_t* sig_code, Fp12* out, void* stream);
 // K3: decompress + subgroup-check every 96-byte signature
 //     `threads`: CTA size (32 = spread for latency, 512 = pack onto few SMs while the per-key kernel runs)
 void launch_g2_sig_decode(const uint8_t* sigs, uint32_t n, G2Aff* out, int32_t* sig_code, void* stream);
@@ -131,7 +143,11 @@ enum : int32_t {
     PAIRING_EVAL_VM_FINAL8 = 34, PAIRING_EVAL_VM_FINAL16 = 35,       // a: f0, b: f1 -> the six program outputs, flag = verdict
     PAIRING_EVAL_VM_END = 36,                                        // bls_vm.cu, teams of 8 / 16 lanes under vm_cta
     PAIRING_EVAL_FOLD_FP12 = 48, PAIRING_EVAL_FOLD_G2 = 49,          // n inputs of a (Fp12 / G2 Jacobian) -> record 0: the
-    PAIRING_EVAL_FOLD_END = 50                                       // product / the affine sum (flag: infinity); bls_rlc.cu
+                                                                     // product / the affine sum (flag: infinity); bls_rlc.cu
+    PAIRING_EVAL_FOLD_SEGMENTS = 50,                                 // a: n Fp12 values; b: words b[0] = T, b[1 .. T+1] = segment
+                                                                     // offsets (from 0, non-decreasing, <= n; 2T <= n) -> records
+                                                                     // 2t, 2t + 1: the two values segment t folds to (zero when empty)
+    PAIRING_EVAL_FOLD_END = 51
 };
 constexpr uint32_t kPairingEvalWords = 145;
 void launch_pairing_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);

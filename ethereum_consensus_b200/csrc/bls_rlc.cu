@@ -122,6 +122,42 @@ __global__ void __launch_bounds__(32) k_rlc_reduce(const Fp12* __restrict__ f_in
         if (lane == 0) q_out[blockIdx.x] = q;
     }
 }
+// Segmented Gt product for aggregate_verify batches (launch_fold_segments): k_rlc_reduce's warp and shuffles, with the
+// tree replaced by a segmented suffix scan, so that one warp serves every segment its 32 values touch.  Step d = 1, 2, ..,
+// 16: lane l multiplies in lane l + d's partial while l + d is still in l's segment; afterwards the first lane of each piece
+// holds the piece's product.  Five dependent products per level, whatever the segments' lengths; a segment of n values
+// needs about log32(n) levels.
+__global__ void __launch_bounds__(64) k_fold_segments(const Fp12* __restrict__ in, uint32_t n_in, const uint32_t* __restrict__ seg_of,
+                                                       const uint32_t* __restrict__ seg_in, const uint32_t* __restrict__ seg_out,
+                                                       const int32_t* __restrict__ pk_code, const uint32_t* __restrict__ flags,
+                                                       const int32_t* __restrict__ sig_code, Fp12* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31u, chunk = i >> 5;
+    bool live = i < n_in;
+    uint32_t t = 0, last = 0;   // the segment, and the lane of its last value in this chunk
+    if (live) {
+        t = seg_of[i];
+        last = min(seg_in[t + 1], (chunk + 1) * 32u) - 1 - chunk * 32u;
+        if (pk_code && (pk_code[t] != BLS_SUCCESS || flags[t] != 0 || sig_code[t] != SIG_OK)) live = false;   // failed tuple
+    }
+    Fp12 f = fp12_one();
+    if (live) f = in[i];
+#pragma unroll 1
+    for (uint32_t d = 1; d < 32; d <<= 1) {   // every lane shuffles: the whole warp takes part in each step
+        Fp12 fo;
+        shfl_down_words(fo, f, int(d));
+        if (live && lane + d <= last) fp12_mul(f, f, fo);
+    }
+    if (!live) return;
+    const uint32_t first = seg_in[t];
+    if (i != first && lane != 0) return;   // not the head of a piece
+    const uint32_t k = chunk - first / 32u;
+    if (seg_out) {
+        out[seg_out[t] + k] = f;
+    } else {
+        out[2 * size_t(t) + k] = f;
+        if ((seg_in[t + 1] - 1) / 32u == first / 32u) out[2 * size_t(t) + 1] = fp12_one();   // one piece: pad with one
+    }
+}
 __global__ void k_fp12_one(Fp12* out) {
     if (threadIdx.x == 0 && blockIdx.x == 0) *out = fp12_one();
 }
@@ -148,6 +184,12 @@ uint32_t launch_rlc_reduce(const Fp12* f_in, const G2Jac* q_in, uint32_t n, Fp12
     const uint32_t blocks = (n + 31) / 32;
     if (blocks) k_rlc_reduce<<<blocks, 32, 0, static_cast<cudaStream_t>(stream)>>>(f_in, q_in, n, f_out, q_out);
     return blocks;
+}
+void launch_fold_segments(const Fp12* in, uint32_t n_in, const uint32_t* seg_of, const uint32_t* seg_in, const uint32_t* seg_out,
+                          const int32_t* pk_code, const uint32_t* flags, const int32_t* sig_code, Fp12* out, void* stream) {
+    if (!n_in) return;
+    k_fold_segments<<<(n_in + 63) / 64, 64, 0, static_cast<cudaStream_t>(stream)>>>(in, n_in, seg_of, seg_in, seg_out, pk_code, flags,
+                                                                                     sig_code, out);
 }
 void launch_fp12_one(Fp12* out, void* stream) { k_fp12_one<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(out); }
 void launch_rlc_finish(const G2Jac* q, G2Aff* out, void* stream) { k_rlc_finish<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(q, out); }

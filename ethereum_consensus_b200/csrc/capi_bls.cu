@@ -57,6 +57,8 @@ struct BlsState {
     DevBuf rlc_jac, rlc_g1, rlc_q, rlc_fa, rlc_fb, rlc_qa, rlc_qb, rlc_zero, rlc_idx, rlc_misc, rlc_xch;
     // batch aggregation: per-chunk partial sums and codes of the signature groups
     DevBuf agg_part;
+    // aggregate_verify batches: the segmented Gt product's ping-pong levels
+    DevBuf fold_a, fold_b;
     PinnedBuf stage;
     G1Aff* d_negg1 = nullptr;
     G1Pre* d_negg1_pre = nullptr;
@@ -156,7 +158,7 @@ static int32_t bls_state(Engine& e, BlsState** out) {
     return B200_SUCCESS;
 }
 
-enum PairMode { MODE_FAST_AGGREGATE = 0, MODE_AGGREGATE = 1 };
+enum PairMode { MODE_FAST_AGGREGATE = 0, MODE_AGGREGATE = 1, MODE_AGGREGATE_BATCH = 2 };
 // message offsets travel as uint32 (32 bytes per tuple on the batch paths): 32 * T must not wrap
 constexpr size_t kMaxBatchTuples = size_t(1) << 26;
 // keys a `..._batch_mixed` call may bring along (a block carries <= 16 deposits + 16 bls-to-execution changes)
@@ -173,6 +175,7 @@ struct RlcReq {
 
 // One call's work: T tuples.  MODE_FAST_AGGREGATE: tuple t sums keys [key_off[t], key_off[t+1]) and checks
 // e(sum, H(msg_t)) e(-g1, sig_t) == 1.  MODE_AGGREGATE: one tuple, pairs (key_i, H(msg_i)) + (-g1, sig).
+// MODE_AGGREGATE_BATCH: T such tuples, tuple t pairing keys [key_off[t], ..) with messages [msg_group[t], ..).
 struct Batch {
     PairMode mode = MODE_FAST_AGGREGATE;
     // host key bytes (strict); with `index` as well: n_keys EXTRA keys (deposits, bls-to-execution changes) validated by this
@@ -185,11 +188,70 @@ struct Batch {
     const uint8_t* msgs = nullptr;     // host bytes + offsets (n_msgs + 1)
     const uint32_t* msg_off = nullptr;
     uint32_t n_msgs = 0;
+    const uint32_t* msg_group = nullptr;   // MODE_AGGREGATE_BATCH: T + 1 offsets into the messages
     const uint8_t* sigs = nullptr;
     uint32_t T = 0;
     bool force_fail_shape = false;     // MODE_AGGREGATE: no pairs, the tuple is flagged EMPTY
     RlcReq* rlc = nullptr;
 };
+
+// aggregate_verify batches: tuple t has a pairing to check iff it has keys and as many messages as keys; the others are
+// flagged EMPTY (VERIFY_FAIL after the key and signature decoding checks, as crypto/bls.rs:102-104)
+static bool av_shape_ok(const Batch& b, uint32_t t) {
+    const uint32_t nk = b.key_off[t + 1] - b.key_off[t];
+    return nk != 0 && nk == b.msg_group[t + 1] - b.msg_group[t];
+}
+static uint32_t av_pairs(const Batch& b) {   // n + 1 pairs per tuple with a pairing
+    uint32_t n = 0;
+    for (uint32_t t = 0; t < b.T; t++)
+        if (av_shape_ok(b, t)) n += b.key_off[t + 1] - b.key_off[t] + 1;
+    return n;
+}
+
+// One level of the segmented Gt product (launch_fold_segments); o_*: word offsets of its arrays in the staged small array,
+// o_out == kFinalLevel for the level that writes two values per segment
+struct FoldLevel {
+    size_t o_map, o_in, o_out;
+    uint32_t n_in, n_out;
+};
+constexpr size_t kFinalLevel = ~size_t(0);
+
+// Plans the segmented product of T segments whose T + 1 offsets are words[o_off ..]: each level's value -> segment map
+// (level 0's at o_map0 unless that is kFinalLevel) and output offsets are appended to `words`.  Levels follow until every
+// segment is in at most two pieces; with skip_pairs no level at all when every segment already holds two values or none.
+static std::vector<FoldLevel> plan_fold(std::vector<uint32_t>& words, size_t o_off, uint32_t T, size_t o_map0, bool skip_pairs) {
+    std::vector<FoldLevel> lv;
+    auto len = [&](size_t o, uint32_t t) { return words[o + t + 1] - words[o + t]; };
+    if (skip_pairs) {
+        bool pairs = true;
+        for (uint32_t t = 0; t < T && pairs; t++) pairs = len(o_off, t) == 0 || len(o_off, t) == 2;
+        if (pairs) return lv;
+    }
+    auto pieces = [&](size_t o, uint32_t t) { return len(o, t) ? (words[o + t + 1] - 1) / 32 - words[o + t] / 32 + 1 : 0u; };
+    size_t o_in = o_off, o_map = o_map0;
+    for (;;) {
+        const uint32_t n_in = words[o_in + T];
+        if (o_map == kFinalLevel) {
+            o_map = words.size();
+            words.resize(o_map + n_in);
+            for (uint32_t t = 0; t < T; t++)
+                for (uint32_t i = words[o_in + t]; i < words[o_in + t + 1]; i++) words[o_map + i] = t;
+        }
+        uint32_t most = 0;
+        for (uint32_t t = 0; t < T; t++) most = std::max(most, pieces(o_in, t));
+        if (most <= 2) {
+            lv.push_back({o_map, o_in, kFinalLevel, n_in, 2 * T});
+            return lv;
+        }
+        const size_t o_out = words.size();
+        words.resize(o_out + T + 1);
+        words[o_out] = 0;
+        for (uint32_t t = 0; t < T; t++) words[o_out + t + 1] = words[o_out + t] + pieces(o_in, t);
+        lv.push_back({o_map, o_in, o_out, n_in, words[o_out + T]});
+        o_in = o_out;
+        o_map = kFinalLevel;
+    }
+}
 
 // One run_verify call in phases.  The members are the sizes every phase derives from the batch, set once here, and where
 // stage_small put the index arrays.
@@ -198,15 +260,17 @@ struct VerifyRun {
     BlsState& s;
     const Batch& b;
     const uint32_t T = b.T, n_keys = b.n_keys, n_msgs = b.n_msgs;
-    const bool fa = b.mode == MODE_FAST_AGGREGATE, registry = b.index != nullptr;
-    const uint32_t n_g1 = (fa ? T : n_keys) + 1;  // + (-g1)
-    const uint32_t n_pairs = fa ? 2 * T : (b.force_fail_shape ? 0 : n_msgs + 1);
+    const bool fa = b.mode == MODE_FAST_AGGREGATE, avb = b.mode == MODE_AGGREGATE_BATCH, registry = b.index != nullptr;
+    const uint32_t n_ops = registry ? b.n_index : n_keys;   // MODE_AGGREGATE_BATCH: one G1 operand per key of the call
+    const uint32_t n_g1 = (fa ? T : avb ? n_ops : n_keys) + 1;  // + (-g1)
+    const uint32_t n_pairs = fa ? 2 * T : avb ? av_pairs(b) : (b.force_fail_shape ? 0 : n_msgs + 1);
     const uint32_t n_g2 = n_msgs + T;
     const uint32_t msg_bytes = b.msg_off[n_msgs];
     const uint32_t rlc_world = b.rlc && b.rlc->exchange ? uint32_t(comm().world) : 1u;
     const cudaStream_t sa = e.stream;
     // set by stage_small: word offsets in s.small, the pair arrays on the device, the pinned area results come back to
-    size_t o_koff = 0, o_index = 0, o_moff = 0;
+    size_t o_koff = 0, o_index = 0, o_moff = 0, o_tflags = 0, o_two = 0;
+    std::vector<FoldLevel> fold;   // MODE_AGGREGATE_BATCH with the VM: the levels of the segmented Gt product
     const uint32_t *d_small = nullptr, *d_g1i = nullptr, *d_g2i = nullptr, *d_ptu = nullptr, *d_poff = nullptr;
     int32_t* h_out = nullptr;
     bool chunked = false;   // set by key_phase: the pairing chain is already queued on stream D
@@ -273,13 +337,14 @@ int32_t VerifyRun::reserve_buffers() {
     return B200_SUCCESS;
 }
 
-// small host-built arrays, one staged copy on stream A: [key_off | index | msg_off | g1_idx | g2_idx | pair_tuple | pair_off]
+// small host-built arrays, one staged copy on stream A: [key_off | index | msg_off | g1_idx | g2_idx | pair_tuple | pair_off],
+// then for MODE_AGGREGATE_BATCH [tuple flags | 0, 2, .., 2T | the fold levels' maps and offsets]
 int32_t VerifyRun::stage_small() {
-    const uint32_t n_koff = fa ? T + 1 : 2;
+    const uint32_t n_koff = (fa || avb) ? T + 1 : 2;
     std::vector<uint32_t> small;
     small.reserve(size_t(n_koff) + b.n_index + n_msgs + 1 + 3 * size_t(n_pairs) + T + 1 + 8);
     o_koff = small.size();
-    if (fa) small.insert(small.end(), b.key_off, b.key_off + T + 1);
+    if (fa || avb) small.insert(small.end(), b.key_off, b.key_off + T + 1);
     else { small.push_back(0); small.push_back(n_keys); }
     o_index = small.size();
     if (registry) small.insert(small.end(), b.index, b.index + b.n_index);
@@ -299,6 +364,27 @@ int32_t VerifyRun::stage_small() {
             poff[t] = 2 * t;
         }
         poff[T] = 2 * T;
+    } else if (avb) {   // tuple t: (key_i, H(msg_i)) for its n keys and messages, then (-g1, sig_t); none without a pairing
+        uint32_t p = 0;
+        for (uint32_t t = 0; t < T; t++) {
+            poff[t] = p;
+            if (!av_shape_ok(b, t)) continue;
+            for (uint32_t k = b.key_off[t], m = b.msg_group[t]; k < b.key_off[t + 1]; k++, m++, p++) { g1i[p] = k; g2i[p] = m; ptu[p] = t; }
+            g1i[p] = n_ops; g2i[p] = n_msgs + t; ptu[p] = t;
+            p++;
+        }
+        poff[T] = p;
+        o_tflags = small.size();
+        for (uint32_t t = 0; t < T; t++) small.push_back(av_shape_ok(b, t) ? 0u : uint32_t(TUPLE_FLAG_EMPTY));
+        o_two = small.size();
+        for (uint32_t t = 0; t <= T; t++) small.push_back(2 * t);
+        if (s.use_vm) {   // level 0 reads the Miller values, with pair_tuple as its map
+            fold = plan_fold(small, o_g1i + 3 * size_t(n_pairs), T, o_g1i + 2 * size_t(n_pairs), true);
+            uint32_t most = 0;
+            for (const FoldLevel& l : fold) most = std::max(most, l.n_out);
+            B200_CUDA_TRY(s.fold_a.reserve((size_t(most) + 1) * sizeof(Fp12)));
+            B200_CUDA_TRY(s.fold_b.reserve((size_t(most) + 1) * sizeof(Fp12)));
+        }
     } else {
         for (uint32_t i = 0; i + 1 < n_pairs; i++) { g1i[i] = i; g2i[i] = i; ptu[i] = 0; }
         if (n_pairs) { g1i[n_pairs - 1] = n_keys; g2i[n_pairs - 1] = n_msgs; ptu[n_pairs - 1] = 0; }
@@ -432,14 +518,23 @@ int32_t VerifyRun::keys_one_range(uint32_t k_split) {
     }
     B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
     if (s.trace) cudaEventRecord(s.ev_t[0], sa);
-    launch_g1_aggregate(key_aff, key_code, registry ? d_small + o_index : nullptr, d_small + o_koff, fa ? T : 1,
+    launch_g1_aggregate(key_aff, key_code, registry ? d_small + o_index : nullptr, d_small + o_koff, (fa || avb) ? T : 1,
                         (fa && !s.use_vm) ? d_g1 : nullptr, (fa && s.use_vm) ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
                         static_cast<int32_t*>(s.pk_code.p), static_cast<uint32_t*>(s.flags.p),
-                        b.force_fail_shape ? uint32_t(TUPLE_FLAG_EMPTY) : 0u, sa, b.rlc ? static_cast<G1Jac*>(s.rlc_jac.p) : nullptr);
+                        b.force_fail_shape ? uint32_t(TUPLE_FLAG_EMPTY) : 0u, sa, b.rlc ? static_cast<G1Jac*>(s.rlc_jac.p) : nullptr,
+                        avb ? d_small + o_tflags : nullptr);
     e.launches++;
     if (fa) {
         B200_CUDA_TRY(cudaMemcpyAsync(d_g1 + T, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
         B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
+    } else if (avb && (s.use_vm || registry)) {
+        // every key's pair operand (the VM's G1Pre, or the registry's points gathered for the one-thread kernels), -g1 behind them
+        const bool pre = s.use_vm;
+        launch_g1_pair_operands(key_aff, registry ? d_small + o_index : nullptr, n_ops, pre ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
+                                pre ? nullptr : d_g1, sa);
+        if (n_ops) e.launches++;
+        if (pre) B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + n_ops, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
+        else B200_CUDA_TRY(cudaMemcpyAsync(d_g1 + n_ops, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
     } else {   // the pairs read the key array itself (pairing_tail)
         B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Aff*>(s.key_aff.p) + n_keys, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
     }
@@ -476,10 +571,24 @@ void VerifyRun::pairing_tail() {
         launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
         if (s.trace) cudaEventRecord(s.ev_t[3], sa);
         launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
+    } else if (avb && s.use_vm) {
+        // n_t + 1 Miller values per tuple, folded level by level to the two per tuple the final exponentiation reads
+        launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
+        if (s.trace) cudaEventRecord(s.ev_t[3], sa);
+        const Fp12* fin = static_cast<const Fp12*>(s.f.p);
+        Fp12* const buf[2] = {static_cast<Fp12*>(s.fold_a.p), static_cast<Fp12*>(s.fold_b.p)};
+        for (size_t k = 0; k < fold.size(); k++) {
+            const FoldLevel& l = fold[k];
+            launch_fold_segments(fin, l.n_in, d_small + l.o_map, d_small + l.o_in, l.o_out == kFinalLevel ? nullptr : d_small + l.o_out,
+                                 d_pk, d_fl, d_sc, buf[k & 1], sa);
+            if (l.n_in) e.launches++;
+            fin = buf[k & 1];
+        }
+        launch_vm_final(fin, fold.empty() ? d_poff : d_small + o_two, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
     } else {
         // aggregate_verify pairs the keys themselves: len(msgs) != len(pks) or no keys was flagged EMPTY by K2 -> VERIFY_FAIL
         // after the decoding checks
-        const G1Aff* pair_g1 = static_cast<const G1Aff*>(fa ? s.g1pts.p : s.key_aff.p);
+        const G1Aff* pair_g1 = static_cast<const G1Aff*>((fa || (avb && registry)) ? s.g1pts.p : s.key_aff.p);
         launch_miller(pair_g1, d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
         launch_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
     }
@@ -816,6 +925,29 @@ static int32_t aggregate_keys(Engine& e, BlsState& s, bool registry, const uint8
     return aggregate_readback(e, s, d_codes, d_out48, T, 48, out48, out_codes);
 }
 
+// ---- aggregate_verify over T tuples
+
+// T + 1 offsets from 0, non-decreasing; *count: the last one
+static int32_t check_offsets0(const uint32_t* off, size_t n, uint32_t* count) {
+    if (off[0] != 0) return B200_ERR_BAD_ARG;
+    return check_offsets(off, n, count);
+}
+
+// the checks of both aggregate_verify batch entry points (n_tuples > 0): key (or index) offsets, message groups, message
+// byte offsets; *n_keys: keys (indices) of the call, *n_msgs: its messages
+static int32_t check_aggregate_verify_args(Engine& e, const uint32_t* key_off, const uint8_t* msgs, const uint32_t* msg_offsets,
+                                           const uint32_t* msg_group, const uint8_t* sigs, size_t n_tuples, const int32_t* out_codes,
+                                           uint32_t* n_keys, uint32_t* n_msgs) {
+    if (!key_off || !msg_offsets || !msg_group || !sigs || !out_codes || n_tuples > kMaxBatchTuples) return B200_ERR_BAD_ARG;
+    int32_t rc;
+    uint32_t n_bytes;
+    if ((rc = check_offsets0(key_off, n_tuples, n_keys)) || (rc = check_offsets0(msg_group, n_tuples, n_msgs))) return rc;
+    if (*n_keys > 0x3fffffffu || *n_msgs > 0x3fffffffu) { e.last_error = "aggregate_verify_batch: more than 0x3fffffff keys or messages"; return B200_ERR_BAD_ARG; }
+    if ((rc = check_offsets0(msg_offsets, *n_msgs, &n_bytes))) return rc;   // n_msgs + 1 byte offsets
+    if (n_bytes && !msgs) return B200_ERR_BAD_ARG;
+    return B200_SUCCESS;
+}
+
 static void rlc_seed(const uint8_t* seed32, uint8_t out[32]) {
     if (seed32) { memcpy(out, seed32, 32); return; }
     std::random_device rd;   // the scalars must be unpredictable to whoever produced the signatures
@@ -960,6 +1092,10 @@ int32_t b200_pairing_eval(int32_t op, uint32_t n, const uint32_t* a, const uint3
     if (!(vm || fold || (op >= 0 && op < PAIRING_EVAL_END)) || n > (1u << 24)) return B200_ERR_BAD_ARG;
     if (n == 0) return B200_SUCCESS;
     if (!a || !b || !out) return B200_ERR_BAD_ARG;
+    if (op == PAIRING_EVAL_FOLD_SEGMENTS) {   // T segments over at most n values, two result records each
+        uint32_t last;
+        if (b[0] == 0 || 2 * size_t(b[0]) > n || check_offsets0(b + 1, b[0], &last) || last > n) return B200_ERR_BAD_ARG;
+    }
     BlsState* s;
     if ((rc = bls_state(e, &s))) return rc;   // the VM's programs and constants
     constexpr size_t W = kPairingEvalWords;
@@ -1049,6 +1185,31 @@ int32_t b200_pairing_eval(int32_t op, uint32_t n, const uint32_t* a, const uint3
         if (ce == cudaSuccess) ce = cudaMemcpyAsync(&v, r, sizeof(Fp12), cudaMemcpyDeviceToHost, st);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
         put(0, &v, sizeof(Fp12), 0);
+    } else if (op == PAIRING_EVAL_FOLD_SEGMENTS) {   // the aggregate_verify batches' levels, from the values of a
+        const uint32_t T = b[0];
+        std::vector<uint32_t> words(b + 1, b + 2 + T);
+        const std::vector<FoldLevel> lv = plan_fold(words, 0, T, kFinalLevel, false);
+        std::vector<Fp12> f(n);
+        for (uint32_t i = 0; i < n; i++) f[i] = fp12_of(a + i * W);
+        Fp12* df = reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12)));
+        Fp12* buf[2] = {reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12))), reinterpret_cast<Fp12*>(carve(n * sizeof(Fp12)))};
+        uint32_t* dw = reinterpret_cast<uint32_t*>(carve(words.size() * 4));
+        cudaMemcpyAsync(df, f.data(), n * sizeof(Fp12), cudaMemcpyHostToDevice, st);
+        cudaMemcpyAsync(dw, words.data(), words.size() * 4, cudaMemcpyHostToDevice, st);
+        const Fp12* in = df;
+        for (size_t k = 0; k < lv.size(); k++) {
+            const FoldLevel& l = lv[k];
+            if (l.o_out == kFinalLevel) cudaMemsetAsync(buf[k & 1], 0, 2 * size_t(T) * sizeof(Fp12), st);   // empty segments: zero
+            launch_fold_segments(in, l.n_in, dw + l.o_map, dw + l.o_in, l.o_out == kFinalLevel ? nullptr : dw + l.o_out, nullptr, nullptr,
+                                 nullptr, buf[k & 1], st);
+            if (l.n_in) e.launches++;
+            in = buf[k & 1];
+        }
+        std::vector<Fp12> fo(2 * size_t(T));
+        ce = cudaGetLastError();
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(fo.data(), in, 2 * size_t(T) * sizeof(Fp12), cudaMemcpyDeviceToHost, st);
+        if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+        for (uint32_t i = 0; i < 2 * T; i++) put(i, &fo[i], sizeof(Fp12), 0);
     } else {   // the sum of the n Jacobian points of a, through rlc_tail's fold and k_rlc_finish
         std::vector<G2Jac> q(n);
         for (uint32_t i = 0; i < n; i++) memcpy(&q[i], a + i * W, sizeof(G2Jac));
@@ -1374,6 +1535,47 @@ int32_t b200_aggregate_verify(const uint8_t* pks_flat, size_t n_pks, const uint8
     rc = run_verify(e, *s, {.mode = MODE_AGGREGATE, .keys = pks_flat, .n_keys = uint32_t(n_pks), .msgs = flat.data(), .msg_off = moff.data(),
                             .n_msgs = uint32_t(moff.size() - 1), .sigs = sig, .T = 1, .force_fail_shape = shape_fail}, &code);
     return rc ? rc : code;
+}
+
+// crypto/bls.rs:95-112 over T tuples: the same codes as T calls of b200_aggregate_verify, on the lane-parallel pairing
+int32_t b200_aggregate_verify_batch(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs, const uint32_t* msg_offsets,
+                                    const uint32_t* msg_group, const uint8_t* sigs, size_t n_tuples, int32_t* out_codes) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (n_tuples == 0) return B200_SUCCESS;
+    uint32_t nk, nm;
+    if ((rc = check_aggregate_verify_args(e, pk_offsets, msgs, msg_offsets, msg_group, sigs, n_tuples, out_codes, &nk, &nm))) return rc;
+    if (nk && !pks_flat) return B200_ERR_BAD_ARG;
+    BlsState* s;
+    rc = bls_state(e, &s);
+    if (rc) return rc;
+    return run_verify(e, *s, {.mode = MODE_AGGREGATE_BATCH, .keys = pks_flat, .n_keys = nk, .key_off = pk_offsets, .msgs = msgs,
+                              .msg_off = msg_offsets, .n_msgs = nm, .msg_group = msg_group, .sigs = sigs, .T = uint32_t(n_tuples)},
+                      out_codes);
+}
+
+int32_t b200_aggregate_verify_batch_indexed(const uint32_t* indices, const uint32_t* offsets, const uint8_t* msgs,
+                                            const uint32_t* msg_offsets, const uint32_t* msg_group, const uint8_t* sigs,
+                                            size_t n_tuples, int32_t* out_codes) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (n_tuples == 0) return B200_SUCCESS;
+    uint32_t ni, nm;
+    if ((rc = check_aggregate_verify_args(e, offsets, msgs, msg_offsets, msg_group, sigs, n_tuples, out_codes, &ni, &nm))) return rc;
+    if (ni && !indices) return B200_ERR_BAD_ARG;
+    BlsState* s;
+    rc = bls_state(e, &s);
+    if (rc) return rc;
+    if (!s->reg_aff.p) { e.last_error = "no registry loaded"; return B200_ERR_BAD_ARG; }
+    if ((rc = check_indices(e, *s, indices, ni, 0))) return rc;
+    static const uint32_t dummy = 0;
+    return run_verify(e, *s, {.mode = MODE_AGGREGATE_BATCH, .index = indices ? indices : &dummy, .n_index = ni, .key_off = offsets,
+                              .msgs = msgs, .msg_off = msg_offsets, .n_msgs = nm, .msg_group = msg_group, .sigs = sigs,
+                              .T = uint32_t(n_tuples)}, out_codes);
 }
 
 // crypto/bls.rs:79-93: the batch path with one group

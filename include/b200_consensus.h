@@ -223,6 +223,26 @@ B200_API int32_t b200_eth_fast_aggregate_verify(const uint8_t* const* pks, size_
 /* aggregate_verify — crypto/bls.rs:95-112; n_pks x 48 contiguous bytes, n_msgs (pointer,length) messages */
 B200_API int32_t b200_aggregate_verify(const uint8_t* pks_flat, size_t n_pks, const uint8_t* const* msgs,
                                        const size_t* msg_lens, size_t n_msgs, const uint8_t sig[96]);
+/* aggregate_verify (crypto/bls.rs:95-112) over T tuples in one call.  Tuple t: keys [pk_offsets[t], pk_offsets[t+1]) of
+ * pks_flat (48 B each), messages [msg_group[t], msg_group[t+1]) where message j is bytes [msg_offsets[j], msg_offsets[j+1])
+ * of msgs, signature sigs[96 t ..].  out_codes[t] = what b200_aggregate_verify returns for that tuple alone: the first
+ * invalid key's code, else the signature's decode code, else 5 (VERIFY_FAIL) for a tuple without keys or with as many
+ * keys as messages not holding, for a signature outside G2 or a pairing product other than one; else 0.  Duplicate keys and
+ * messages, empty messages and tuples without keys or messages are allowed.  All pairs of all tuples run on the
+ * lane-parallel pairing kernels together, and each tuple's n + 1 Miller values are multiplied by a segmented warp-shuffle
+ * product before its final exponentiation.
+ * B200_ERR_BAD_ARG, nothing changed: a NULL pointer with a non-zero count; an offset array (T + 1 key offsets, T + 1
+ * message groups, n_msgs + 1 byte offsets) that does not start at 0 or decreases; more than 0x3fffffff keys or messages;
+ * T > 2^26.  n_tuples == 0 succeeds and changes nothing.  Each call sets b200_last_kernel_ms. */
+B200_API int32_t b200_aggregate_verify_batch(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs,
+                                             const uint32_t* msg_offsets, const uint32_t* msg_group, const uint8_t* sigs,
+                                             size_t n_tuples, int32_t* out_codes);
+/* The same with keys named by validator index into the resident registry (b200_registry_load / _append / _load_state):
+ * each key keeps the code it was validated with, so the codes equal the strict call's on the same key bytes.  Also
+ * B200_ERR_BAD_ARG: no registry loaded, or an index >= the registry's size. */
+B200_API int32_t b200_aggregate_verify_batch_indexed(const uint32_t* indices, const uint32_t* offsets, const uint8_t* msgs,
+                                                     const uint32_t* msg_offsets, const uint32_t* msg_group,
+                                                     const uint8_t* sigs, size_t n_tuples, int32_t* out_codes);
 /* aggregate — crypto/bls.rs:79-93; n == 0 -> B200_EMPTY_AGGREGATE; out = compressed sum */
 B200_API int32_t b200_aggregate(const uint8_t* sigs_flat, size_t n, uint8_t out[96]);
 /* eth_aggregate_public_keys — crypto/bls.rs:135-148 */
@@ -347,7 +367,8 @@ B200_API int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const u
 B200_API int32_t b200_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
 /* On-device self-test of the pairing, for comparison with a big-integer oracle: `op` (bls_kernels.cuh, PAIRING_EVAL_*) runs
  * in the unit whose production kernel runs it: Fp6 / Fp12 operations, Miller steps and loop, the final exponentiation
- * (one thread per record), the lane-parallel Miller and final programs at teams of 8 or 16 lanes, and the RLC folds.
+ * (one thread per record), the lane-parallel Miller and final programs at teams of 8 or 16 lanes, the RLC folds, and the
+ * segmented product of the aggregate_verify batches (a: the values; b: the word T, then T + 1 segment offsets).
  * a, b, out: n x 145 words: twelve 12-word Fp slots in Fp12 memory order of raw little-endian 32-bit Montgomery limbs,
  * then a flag word (in: the infinity flag of a point; out: the final exponentiation's verdict, or the infinity flag of the
  * G2 fold's affine sum).  n = 0 .. 2^24.  Test use only. */
