@@ -61,6 +61,11 @@ _PROTOS = {
     "b200_compute_shuffled_indices": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_void_p]),
     "b200_get_active_validator_indices": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p, C.POINTER(C.c_size_t)]),
     "b200_state_shuffled_active_indices": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_size_t)]),
+    "b200_state_get_seed": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "b200_state_proposer_indices": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p]),
+    "b200_state_next_sync_committee": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
+    "b200_state_sync_committee_updates": (C.c_int32, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "b200_state_sync_committee_indices": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p]),
     # multi-GPU (comm.cu): the exchange step lives inside the library
     "b200_comm_unique_id": (C.c_int32, [C.c_void_p]),
     "b200_comm_init": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),

@@ -371,10 +371,12 @@ void launch_g1_validate(const uint8_t* keys, uint32_t n, G1Aff* out, int32_t* co
 }
 // The registry's key staging from a resident state: the 48-byte public key at the head of each 121-byte Validator record,
 // packed back to back so that K1 reads every key as three 16-byte words.  Records sit at odd byte offsets: byte loads.
-static __global__ void k_gather_validator_keys(const uint8_t* __restrict__ records, uint32_t n, uint4* __restrict__ keys) {
+// `index` (device, optional): key i is that of record index[i] (a sync committee's members) instead of record i.
+static __global__ void k_gather_validator_keys(const uint8_t* __restrict__ records, const uint64_t* __restrict__ index, uint32_t n,
+                                               uint4* __restrict__ keys) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint8_t* r = records + size_t(i) * 121;
+    const uint8_t* r = records + (index ? index[i] : uint64_t(i)) * 121;
     uint32_t w[12];
 #pragma unroll
     for (int k = 0; k < 12; k++)
@@ -382,9 +384,9 @@ static __global__ void k_gather_validator_keys(const uint8_t* __restrict__ recor
 #pragma unroll
     for (int k = 0; k < 3; k++) keys[size_t(i) * 3 + k] = make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]);
 }
-void launch_gather_validator_keys(const uint8_t* records, uint32_t n, uint8_t* keys, void* stream) {
+void launch_gather_validator_keys(const uint8_t* records, uint32_t n, uint8_t* keys, void* stream, const uint64_t* index) {
     if (!n) return;
-    k_gather_validator_keys<<<(n + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(records, n, reinterpret_cast<uint4*>(keys));
+    k_gather_validator_keys<<<(n + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream)>>>(records, index, n, reinterpret_cast<uint4*>(keys));
 }
 void launch_g1_aggregate(const G1Aff* keys, const int32_t* key_codes, const uint32_t* index, const uint32_t* off,
                          uint32_t n_tuples, G1Aff* agg, G1Pre* agg_pre, int32_t* pk_code, uint32_t* flags,

@@ -28,9 +28,9 @@ void set_vm_team16_max(uint32_t n);
 void set_vm_cta(int threads);
 // cta = 0: by batch size (384-thread CTAs above the small-batch bound, 128 below); 128 / 384 force one (default variant only)
 void launch_g1_validate(const uint8_t* keys, uint32_t n, G1Aff* out, int32_t* codes, void* stream, int cta = 0);
-// K1's input from n 121-byte Validator records in device memory (public key first): keys[48 i ..] = records[121 i ..][0, 48);
-// `keys` 16-byte aligned
-void launch_gather_validator_keys(const uint8_t* records, uint32_t n, uint8_t* keys, void* stream);
+// K1's input from n 121-byte Validator records in device memory (public key first): keys[48 i ..] = records[121 j ..][0, 48)
+// with j = i, or j = index[i] when `index` (device) is given; `keys` 16-byte aligned
+void launch_gather_validator_keys(const uint8_t* records, uint32_t n, uint8_t* keys, void* stream, const uint64_t* index = nullptr);
 // K2: per tuple t, sum the validated keys [off[t], off[t+1]) (or gather through `index` when non-null);
 //     first failing key (in order) decides pk_code[t]
 //     agg == nullptr: only the code scan (aggregate_verify keeps keys separate); extra_flags is OR-ed into flags

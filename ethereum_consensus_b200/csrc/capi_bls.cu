@@ -887,9 +887,11 @@ static int32_t aggregate_sigs(Engine& e, BlsState& s, const uint8_t* sigs, uint3
 }
 
 // n keys, T groups by `off` (host): strict (`keys`: K1 over all n, then K2 over the call's points) or from the registry
-// (`index`: K2 gathers the resident points and codes), then one compression thread per group
+// (`index`: K2 gathers the resident points and codes), then one compression thread per group.  Strict keys come from the
+// host, or (`records`) from the Validator records rec_index[0 .. n) in HBM, packed into K1's staging buffer on the device.
 static int32_t aggregate_keys(Engine& e, BlsState& s, bool registry, const uint8_t* keys, const uint32_t* index, uint32_t n,
-                              const uint32_t* off, uint32_t T, uint8_t* out48, int32_t* out_codes) {
+                              const uint32_t* off, uint32_t T, uint8_t* out48, int32_t* out_codes,
+                              const uint8_t* records = nullptr, const uint64_t* rec_index = nullptr) {
     const bool strict = !registry;
     const size_t n_small = size_t(T) + 1 + (registry ? n : 0);
     B200_CUDA_TRY(s.small.reserve(n_small * 4 + 64));
@@ -906,10 +908,14 @@ static int32_t aggregate_keys(Engine& e, BlsState& s, bool registry, const uint8
     uint32_t* d_off = static_cast<uint32_t*>(s.small.p);
     B200_CUDA_TRY(cudaMemcpyAsync(d_off, off, (size_t(T) + 1) * 4, cudaMemcpyHostToDevice, sa));
     if (registry && n) B200_CUDA_TRY(cudaMemcpyAsync(d_off + T + 1, index, size_t(n) * 4, cudaMemcpyHostToDevice, sa));
-    if (strict && n) B200_CUDA_TRY(cudaMemcpyAsync(s.keys.p, keys, size_t(n) * 48, cudaMemcpyHostToDevice, sa));
+    if (strict && n && !records) B200_CUDA_TRY(cudaMemcpyAsync(s.keys.p, keys, size_t(n) * 48, cudaMemcpyHostToDevice, sa));
     int32_t* d_codes = static_cast<int32_t*>(s.out.p);
     uint8_t* d_out48 = static_cast<uint8_t*>(s.out.p) + size_t(T) * 4;
     B200_CUDA_TRY(cudaEventRecord(s.ev_k0, sa));
+    if (records) {
+        launch_gather_validator_keys(records, n, static_cast<uint8_t*>(s.keys.p), sa, rec_index);
+        e.launches += n ? 1 : 0;
+    }
     if (strict) {
         launch_g1_validate(static_cast<const uint8_t*>(s.keys.p), n, static_cast<G1Aff*>(s.key_aff.p), static_cast<int32_t*>(s.key_code.p), sa);
         e.launches += n ? 1 : 0;
@@ -923,6 +929,22 @@ static int32_t aggregate_keys(Engine& e, BlsState& s, bool registry, const uint8
     B200_CUDA_TRY(cudaEventRecord(s.ev_k1, sa));
     B200_CUDA_TRY(cudaGetLastError());
     return aggregate_readback(e, s, d_codes, d_out48, T, 48, out48, out_codes);
+}
+
+// get_next_sync_committee's public keys and aggregate_pubkey (deneb/spec/mod.rs:2014-2060): the keys of Validator records
+// index[0 .. n) (device) gathered in HBM, then eth_aggregate_public_keys' strict path over them.  keys48 (host) receives the
+// n gathered keys, out48 the aggregate and *code its code.  The caller holds the engine lock.
+int32_t aggregate_record_keys(const uint8_t* records, const uint64_t* index, uint32_t n, uint8_t* keys48, uint8_t out48[48],
+                              int32_t* code) {
+    Engine& e = engine();
+    BlsState* s;
+    int32_t rc = bls_state(e, &s);
+    if (rc) return rc;
+    const uint32_t off[2] = {0, n};
+    rc = aggregate_keys(e, *s, false, nullptr, nullptr, n, off, 1, out48, code, records, index);
+    if (rc) return rc;
+    B200_CUDA_TRY(cudaMemcpy(keys48, s->keys.p, size_t(n) * 48, cudaMemcpyDeviceToHost));
+    return B200_SUCCESS;
 }
 
 // ---- aggregate_verify over T tuples

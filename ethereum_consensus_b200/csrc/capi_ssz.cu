@@ -8,6 +8,7 @@
 #include "comm.h"
 #include "engine.h"
 #include "sha256.cuh"
+#include "sha256_hd.cuh"
 #include "shuffle.h"
 #include "ssz_plan.h"
 
@@ -510,11 +511,18 @@ int32_t b200_state_update_elements(b200_state* h, int32_t field, const uint64_t*
     return B200_SUCCESS;
 }
 
+static int32_t update_bytes(Engine& e, b200_state* h, uint64_t ssz_offset, const uint8_t* data, size_t n);
+
 int32_t b200_state_update_bytes(b200_state* h, uint64_t ssz_offset, const uint8_t* data, size_t n) {
     Engine& e = engine();
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
+    return update_bytes(e, h, ssz_offset, data, n);
+}
+
+// b200_state_update_bytes with the engine lock held (the sync-committee rotation writes through it too)
+static int32_t update_bytes(Engine& e, b200_state* h, uint64_t ssz_offset, const uint8_t* data, size_t n) {
     if (!h || !h->uploaded || h->sharded || (n && !data) || ssz_offset > h->len || n > h->len - ssz_offset) return B200_ERR_BAD_ARG;
     if (!n) return B200_SUCCESS;
     const uint64_t lo = ssz_offset, hi = ssz_offset + n;
@@ -752,6 +760,193 @@ int32_t b200_state_shuffled_active_indices(b200_state* h, uint64_t epoch, const 
     B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
     B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, e.ev0, e.ev1));
     *out_n = size_t(cnt);
+    return B200_SUCCESS;
+}
+
+// ---- duties on a resident state: proposer lookahead and sync committees (deneb/spec/mod.rs) ----
+namespace {
+struct DutyPreset {
+    uint64_t slots_per_epoch, epochs_per_historical_vector, epochs_per_sync_committee_period;
+    uint32_t shuffle_round_count, sync_committee_size;
+};
+// phase0/presets/{mainnet,minimal}.rs, altair/presets/{mainnet,minimal}.rs
+DutyPreset duty_preset(int preset) {
+    if (preset == B200_PRESET_MINIMAL) return {8, 64, 8, 10, 32};
+    return {32, 65536, 256, 90, 512};
+}
+constexpr uint8_t kDomainBeaconProposer[4] = {0, 0, 0, 0}, kDomainSyncCommittee[4] = {7, 0, 0, 0};   // domains.rs:19-30
+constexpr size_t kSlotOffset = 40;   // genesis_time (8), genesis_validators_root (32), then slot
+
+uint64_t shadow_slot(const b200_state* h) {
+    const uint8_t* p = h->shadow + kSlotOffset;
+    uint64_t v = 0;
+    for (int k = 7; k >= 0; k--) v = (v << 8) | p[k];
+    return v;
+}
+void sha256_host(const uint8_t* data, size_t len, uint8_t out[32]) {
+    Sha256Ctx c;
+    sha_init(c);
+    sha_update(c, data, len);
+    sha_final(c, out);
+}
+// get_seed (deneb/spec/mod.rs:2713-2748): SHA-256(domain || le64(epoch) || randao_mixes[(epoch + EPHV - 2) mod EPHV]),
+// the mix index in wrapping u64 (EPHV divides 2^64, so the wrap does not change it); the mixes are read from the shadow
+void state_seed(const b200_state* h, uint64_t epoch, const uint8_t domain[4], uint8_t out[32]) {
+    const DutyPreset P = duty_preset(h->preset);
+    const uint64_t mix = (epoch + P.epochs_per_historical_vector - 2) % P.epochs_per_historical_vector;
+    uint8_t in[44];
+    memcpy(in, domain, 4);
+    for (int k = 0; k < 8; k++) in[4 + k] = uint8_t(epoch >> (8 * k));
+    memcpy(in + 12, h->shadow + h->so.randao_mixes + 32 * mix, 32);
+    sha256_host(in, sizeof(in), out);
+}
+bool duty_handle_ok(const b200_state* h) { return h && h->uploaded && !h->sharded; }
+
+// get_active_validator_indices(state, epoch) into the shuffle scratch: *d_act (device) holds *n_active indices, *d_out
+// (device) has room for max(N, min_out) more; *recs: the Validator records in HBM.  No active validator (the reference's
+// CollectionCannotBeEmpty, or its `i % 0` panic for the sync committee) -> B200_ERR_BAD_ARG.
+int32_t duty_active(Engine& e, b200_state* h, uint64_t epoch, uint64_t min_out, const uint8_t** recs, uint64_t** d_act,
+                    uint64_t** d_out, uint64_t* n_active) {
+    const uint64_t n = big_count(h, 0);
+    uint64_t field_off = 0; size_t nbytes = 0;
+    if (n == 0 || !h->plan.chain_field(0, &field_off, &nbytes)) { e.last_error = "duties: no active validator"; return B200_ERR_BAD_ARG; }
+    *recs = static_cast<const uint8_t*>(h->fields.p) + field_off;
+    int32_t rc = shuffle_scratch(e, std::max(n, min_out), d_act, d_out);
+    if (rc) return rc;
+    rc = active_indices_on_device(e, *recs, n, epoch, *d_act, n_active);
+    if (rc) return rc;
+    if (*n_active == 0) { e.last_error = "duties: no active validator"; return B200_ERR_BAD_ARG; }
+    return B200_SUCCESS;
+}
+
+// get_next_sync_committee (deneb/spec/mod.rs:1973-2060) with the engine lock held: indices (host, SIZE) and the SyncCommittee
+// bytes (host, SIZE x 48 keys then the 48-byte aggregate; zero on a non-zero *code)
+int32_t next_sync_committee(Engine& e, b200_state* h, uint64_t* out_indices, uint8_t* out_committee, int32_t* out_code) {
+    const DutyPreset P = duty_preset(h->preset);
+    const uint64_t epoch = shadow_slot(h) / P.slots_per_epoch + 1;
+    uint8_t seed[32];
+    state_seed(h, epoch, kDomainSyncCommittee, seed);
+    const uint8_t* recs;
+    uint64_t *d_act, *d_idx, cnt = 0;
+    B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
+    int32_t rc = duty_active(e, h, epoch, P.sync_committee_size, &recs, &d_act, &d_idx, &cnt);
+    if (rc) return rc;
+    rc = sample_committee_on_device(e, seed, P.sync_committee_size, P.shuffle_round_count, d_act, cnt, recs, d_idx);
+    if (rc) return rc;
+    const size_t size = P.sync_committee_size;
+    rc = aggregate_record_keys(recs, d_idx, uint32_t(size), out_committee, out_committee + size * 48, out_code);
+    if (rc) return rc;
+    B200_CUDA_TRY(cudaEventRecord(e.ev1, e.stream));
+    B200_CUDA_TRY(cudaMemcpyAsync(out_indices, d_idx, size * 8, cudaMemcpyDeviceToHost, e.stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, e.ev0, e.ev1));
+    if (*out_code) memset(out_committee, 0, size * 48 + 48);
+    return B200_SUCCESS;
+}
+}  // namespace
+
+int32_t b200_state_get_seed(b200_state* h, uint64_t epoch, const uint8_t domain_type[4], uint8_t out[32]) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || !domain_type || !out) return B200_ERR_BAD_ARG;
+    state_seed(h, epoch, domain_type, out);
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_proposer_indices(b200_state* h, uint64_t epoch, uint64_t* out) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || !out) return B200_ERR_BAD_ARG;
+    const DutyPreset P = duty_preset(h->preset);
+    if (epoch > ~uint64_t(0) / P.slots_per_epoch) { e.last_error = "proposer_indices: epoch * SLOTS_PER_EPOCH overflows u64"; return B200_ERR_BAD_ARG; }
+    // get_beacon_proposer_index (deneb/spec/mod.rs:2822-2856) for every slot of the epoch: seed SHA-256(get_seed(epoch,
+    // BeaconProposer) || le64(slot)), the active set and the balances being those of the epoch
+    uint8_t epoch_seed[32], in[40];
+    state_seed(h, epoch, kDomainBeaconProposer, epoch_seed);
+    memcpy(in, epoch_seed, 32);
+    std::vector<uint8_t> slot_seeds(P.slots_per_epoch * 32);
+    for (uint64_t j = 0; j < P.slots_per_epoch; j++) {
+        const uint64_t slot = epoch * P.slots_per_epoch + j;
+        for (int k = 0; k < 8; k++) in[32 + k] = uint8_t(slot >> (8 * k));
+        sha256_host(in, sizeof(in), slot_seeds.data() + 32 * j);
+    }
+    const uint8_t* recs;
+    uint64_t *d_act, *d_out, cnt = 0;
+    B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
+    rc = duty_active(e, h, epoch, 0, &recs, &d_act, &d_out, &cnt);
+    if (rc) return rc;
+    std::vector<uint64_t> res(P.slots_per_epoch);
+    rc = sample_proposers_on_device(e, slot_seeds.data(), uint32_t(P.slots_per_epoch), P.shuffle_round_count, d_act, cnt, recs, res.data());
+    if (rc) return rc;
+    B200_CUDA_TRY(cudaEventRecord(e.ev1, e.stream));
+    B200_CUDA_TRY(cudaEventSynchronize(e.ev1));
+    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, e.ev0, e.ev1));
+    memcpy(out, res.data(), res.size() * 8);
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_next_sync_committee(b200_state* h, uint64_t* out_indices, uint8_t* out_committee, int32_t* out_code) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || !out_indices || !out_committee || !out_code) return B200_ERR_BAD_ARG;
+    return next_sync_committee(e, h, out_indices, out_committee, out_code);
+}
+
+int32_t b200_state_sync_committee_updates(b200_state* h, int32_t* rotated, int32_t* out_code) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || !rotated || !out_code) return B200_ERR_BAD_ARG;
+    const DutyPreset P = duty_preset(h->preset);
+    const uint64_t next_epoch = shadow_slot(h) / P.slots_per_epoch + 1;
+    if (next_epoch % P.epochs_per_sync_committee_period != 0) {
+        *rotated = 0; *out_code = B200_SUCCESS;
+        return B200_SUCCESS;
+    }
+    // current_sync_committee <- next_sync_committee <- get_next_sync_committee: the two fields are adjacent, one patch
+    const size_t committee = (size_t(P.sync_committee_size) + 1) * 48;
+    std::vector<uint8_t> both(2 * committee);
+    std::vector<uint64_t> idx(P.sync_committee_size);
+    memcpy(both.data(), h->shadow + h->so.next_sync_committee, committee);
+    int32_t code = B200_SUCCESS;
+    rc = next_sync_committee(e, h, idx.data(), both.data() + committee, &code);
+    if (rc) return rc;
+    *out_code = code;
+    *rotated = 0;
+    if (code) return B200_SUCCESS;   // the reference's `?` before mem::replace: the state stays as it was
+    rc = update_bytes(e, h, h->so.current_sync_committee, both.data(), both.size());
+    if (rc) return rc;
+    *rotated = 1;
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_sync_committee_indices(b200_state* h, int32_t which, uint64_t* out) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || !out || (which != 0 && which != 1)) return B200_ERR_BAD_ARG;
+    const DutyPreset P = duty_preset(h->preset);
+    const uint8_t* keys = h->shadow + (which ? h->so.next_sync_committee : h->so.current_sync_committee);
+    const uint64_t n = big_count(h, 0);
+    uint64_t field_off = 0; size_t nbytes = 0;
+    const uint8_t* recs = nullptr;
+    if (n && h->plan.chain_field(0, &field_off, &nbytes)) recs = static_cast<const uint8_t*>(h->fields.p) + field_off;
+    B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
+    std::vector<uint64_t> res(P.sync_committee_size);
+    rc = match_committee_keys_on_device(e, recs, recs ? n : 0, keys, P.sync_committee_size, res.data());
+    if (rc) return rc;
+    B200_CUDA_TRY(cudaEventRecord(e.ev1, e.stream));
+    B200_CUDA_TRY(cudaEventSynchronize(e.ev1));
+    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, e.ev0, e.ev1));
+    memcpy(out, res.data(), res.size() * 8);
     return B200_SUCCESS;
 }
 

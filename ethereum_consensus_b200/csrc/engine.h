@@ -72,6 +72,12 @@ Engine& engine();
 // engine lock.
 int32_t state_validator_records(const b200_state* h, const uint8_t** records, uint64_t* n);
 
+// eth_aggregate_public_keys (strict) of the public keys of Validator records index[0 .. n) (device) in HBM, the keys packed
+// and validated on the device: *code and out48 as b200_eth_aggregate_public_keys_batch gives them for one group; keys48
+// (host, n x 48) receives the keys.  The caller holds the engine lock (capi_bls.cu).
+int32_t aggregate_record_keys(const uint8_t* records, const uint64_t* index, uint32_t n, uint8_t* keys48, uint8_t out48[48],
+                              int32_t* code);
+
 // Every entry point holds the engine lock for the whole call.
 struct Guard {
     std::unique_lock<std::mutex> lk;

@@ -125,6 +125,7 @@ class DeviceBeaconState:
         rank constructs it and calls hash_tree_root together; root only)."""
         nbytes = ssz.nbytes if hasattr(ssz, "nbytes") else len(ssz)
         self._h = C.c_void_p()
+        self.preset = preset
         self.n_validators = _count_validators(ssz, preset)
         fn = _lib.lib().b200_state_upload_deneb_sharded if sharded else _lib.lib().b200_state_upload_deneb
         _rc(fn(_lib.ptr(ssz), nbytes, _lib.PRESET[preset], C.byref(self._h)), "state_upload")

@@ -160,6 +160,41 @@ B200_API int32_t b200_get_active_validator_indices(const uint8_t* validators_ssz
 B200_API int32_t b200_state_shuffled_active_indices(b200_state* handle, uint64_t epoch, const uint8_t seed[32], uint32_t rounds,
                                                     uint64_t* out, size_t* out_n);
 
+/* Duties on a device-resident state (single-GPU handles; a NULL, not uploaded or sharded handle gets B200_ERR_BAD_ARG and
+ * is left as it was): who proposes each slot and who sits on the sync committee, computed where the Validator records
+ * are.  Preset constants follow the handle's preset: SLOTS_PER_EPOCH 32 / 8, SHUFFLE_ROUND_COUNT 90 / 10,
+ * EPOCHS_PER_HISTORICAL_VECTOR 65536 / 64, SYNC_COMMITTEE_SIZE 512 / 32, EPOCHS_PER_SYNC_COMMITTEE_PERIOD 256 / 8
+ * (mainnet / minimal); MAX_EFFECTIVE_BALANCE is 32 ETH in both.
+ *  - b200_state_get_seed: get_seed (deneb/spec/mod.rs:2713-2748), SHA-256(domain_type || le64(epoch) ||
+ *    randao_mixes[(epoch + EPHV - 2) mod EPHV]).  domain_type: the 4 bytes of DomainType::as_bytes (domains.rs:19-30), e.g.
+ *    {1,0,0,0} BeaconAttester for b200_state_shuffled_active_indices' seed.
+ *  - b200_state_proposer_indices: out[j] (SLOTS_PER_EPOCH entries) = get_beacon_proposer_index (:2822-2856) on this state
+ *    with slot = epoch * SLOTS_PER_EPOCH + j: one call gives the epoch's whole proposer table (the active set and the
+ *    effective balances do not change inside an epoch).  No active validator at `epoch`, or an epoch * SLOTS_PER_EPOCH
+ *    that overflows u64 -> B200_ERR_BAD_ARG.
+ *  - b200_state_next_sync_committee: get_next_sync_committee (:1973-2060) at epoch slot / SLOTS_PER_EPOCH + 1.
+ *    out_indices (SIZE) are the members in selection order, repeats kept; out_committee (SIZE x 48 + 48 bytes) is the
+ *    SSZ SyncCommittee: their public keys, gathered from the records in HBM, then eth_aggregate_public_keys of them
+ *    (strict: every key validated as b200_eth_aggregate_public_keys does).  *out_code is that aggregation's code; on a
+ *    non-zero code out_committee is zero-filled and out_indices still returned.  No active validator -> B200_ERR_BAD_ARG.
+ *  - b200_state_sync_committee_updates: process_sync_committee_updates (:1263-1297).  When (slot / SLOTS_PER_EPOCH + 1) is
+ *    a multiple of EPOCHS_PER_SYNC_COMMITTEE_PERIOD, current_sync_committee <- next_sync_committee <- the result of
+ *    b200_state_next_sync_committee, written as b200_state_update_bytes writes (both roots follow) and *rotated = 1;
+ *    otherwise nothing changes and *rotated = 0.  A non-zero aggregation code is returned in *out_code with *rotated = 0
+ *    and the state unchanged.
+ *  - b200_state_sync_committee_indices: the committee-key -> validator-index map of process_sync_aggregate (:463-473) for
+ *    which = 0 (current_sync_committee) or 1 (next): out[j] (SIZE entries) is the LARGEST i with
+ *    validators[i].pubkey == pubkeys[j] (the reference's HashMap keeps the last insert), UINT64_MAX when no validator
+ *    holds the key (the reference panics).
+ * The sampling loops, unbounded in the reference (each candidate is accepted with probability >= 1/256), stop after
+ * 2^26 candidates with B200_ERR_LIMIT.  effective_balance * 255 is computed in wrapping u64, as a release build of the
+ * reference does.  b200_last_kernel_ms: the device time of the call. */
+B200_API int32_t b200_state_get_seed(b200_state* handle, uint64_t epoch, const uint8_t domain_type[4], uint8_t out[32]);
+B200_API int32_t b200_state_proposer_indices(b200_state* handle, uint64_t epoch, uint64_t* out);
+B200_API int32_t b200_state_next_sync_committee(b200_state* handle, uint64_t* out_indices, uint8_t* out_committee, int32_t* out_code);
+B200_API int32_t b200_state_sync_committee_updates(b200_state* handle, int32_t* rotated, int32_t* out_code);
+B200_API int32_t b200_state_sync_committee_indices(b200_state* handle, int32_t which, uint64_t* out);
+
 /* ---- multi-GPU: one process per GPU, the exchange step lives INSIDE the library (SURVEY.md §8b `b200_init(n_gpus)`,
  * §8e).  The reference is single-process (no counterpart, SURVEY.md §2a); a Rust host with one process per GPU calls:
  *   rank 0:   b200_comm_unique_id(id)  -> ships the 128 bytes to the other ranks by any means it likes (pipe, file, TCP)
