@@ -66,6 +66,9 @@ _PROTOS = {
     "b200_state_next_sync_committee": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
     "b200_state_sync_committee_updates": (C.c_int32, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200_state_sync_committee_indices": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "b200_state_process_epoch": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_int32)]),
+    "b200_state_serialized_len": (C.c_int32, [C.c_void_p, C.POINTER(C.c_uint64)]),
+    "b200_state_read_bytes": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t]),
     # multi-GPU (comm.cu): the exchange step lives inside the library
     "b200_comm_unique_id": (C.c_int32, [C.c_void_p]),
     "b200_comm_init": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32]),

@@ -7,6 +7,7 @@
 
 #include "comm.h"
 #include "engine.h"
+#include "epoch.h"
 #include "sha256.cuh"
 #include "sha256_hd.cuh"
 #include "shuffle.h"
@@ -768,11 +769,46 @@ namespace {
 struct DutyPreset {
     uint64_t slots_per_epoch, epochs_per_historical_vector, epochs_per_sync_committee_period;
     uint32_t shuffle_round_count, sync_committee_size;
+    // process_epoch
+    uint64_t slots_per_historical_root, epochs_per_slashings_vector, epochs_per_eth1_voting_period;
+    uint64_t min_per_epoch_churn_limit, max_per_epoch_activation_churn_limit, churn_limit_quotient;
+    uint64_t effective_balance_increment, max_effective_balance, ejection_balance;
+    uint64_t hysteresis_quotient, hysteresis_downward_multiplier, hysteresis_upward_multiplier;
+    uint64_t inactivity_score_bias, inactivity_score_recovery_rate, inactivity_penalty_quotient_bellatrix;
+    uint64_t proportional_slashing_multiplier_bellatrix, base_reward_factor, min_epochs_to_inactivity_penalty;
+    uint64_t max_seed_lookahead, min_validator_withdrawability_delay;
 };
-// phase0/presets/{mainnet,minimal}.rs, altair/presets/{mainnet,minimal}.rs
+// phase0/presets/{mainnet,minimal}.rs, altair/presets/{mainnet,minimal}.rs, bellatrix/presets/{mainnet,minimal}.rs,
+// configs/{mainnet,minimal}.rs
 DutyPreset duty_preset(int preset) {
-    if (preset == B200_PRESET_MINIMAL) return {8, 64, 8, 10, 32};
-    return {32, 65536, 256, 90, 512};
+    const bool minimal = preset == B200_PRESET_MINIMAL;
+    DutyPreset P;
+    P.slots_per_epoch = minimal ? 8 : 32;
+    P.epochs_per_historical_vector = minimal ? 64 : 65536;
+    P.epochs_per_sync_committee_period = minimal ? 8 : 256;
+    P.shuffle_round_count = minimal ? 10 : 90;
+    P.sync_committee_size = minimal ? 32 : 512;
+    P.slots_per_historical_root = minimal ? 64 : 8192;
+    P.epochs_per_slashings_vector = minimal ? 64 : 8192;
+    P.epochs_per_eth1_voting_period = minimal ? 4 : 64;
+    P.min_per_epoch_churn_limit = minimal ? 2 : 4;
+    P.max_per_epoch_activation_churn_limit = minimal ? 4 : 8;
+    P.churn_limit_quotient = minimal ? 32 : 65536;
+    P.effective_balance_increment = 1000000000ull;
+    P.max_effective_balance = 32000000000ull;
+    P.ejection_balance = 16000000000ull;
+    P.hysteresis_quotient = 4;
+    P.hysteresis_downward_multiplier = 1;
+    P.hysteresis_upward_multiplier = 5;
+    P.inactivity_score_bias = 4;
+    P.inactivity_score_recovery_rate = 16;
+    P.inactivity_penalty_quotient_bellatrix = uint64_t(1) << 24;
+    P.proportional_slashing_multiplier_bellatrix = 3;
+    P.base_reward_factor = 64;
+    P.min_epochs_to_inactivity_penalty = 4;
+    P.max_seed_lookahead = 4;
+    P.min_validator_withdrawability_delay = 256;
+    return P;
 }
 constexpr uint8_t kDomainBeaconProposer[4] = {0, 0, 0, 0}, kDomainSyncCommittee[4] = {7, 0, 0, 0};   // domains.rs:19-30
 constexpr size_t kSlotOffset = 40;   // genesis_time (8), genesis_validators_root (32), then slot
@@ -843,6 +879,30 @@ int32_t next_sync_committee(Engine& e, b200_state* h, uint64_t* out_indices, uin
     if (*out_code) memset(out_committee, 0, size * 48 + 48);
     return B200_SUCCESS;
 }
+// process_sync_committee_updates with the engine lock held (b200_state_sync_committee_updates, b200_state_process_epoch)
+int32_t sync_committee_updates(Engine& e, b200_state* h, int32_t* rotated, int32_t* out_code) {
+    const DutyPreset P = duty_preset(h->preset);
+    const uint64_t next_epoch = shadow_slot(h) / P.slots_per_epoch + 1;
+    if (next_epoch % P.epochs_per_sync_committee_period != 0) {
+        *rotated = 0; *out_code = B200_SUCCESS;
+        return B200_SUCCESS;
+    }
+    // current_sync_committee <- next_sync_committee <- get_next_sync_committee: the two fields are adjacent, one patch
+    const size_t committee = (size_t(P.sync_committee_size) + 1) * 48;
+    std::vector<uint8_t> both(2 * committee);
+    std::vector<uint64_t> idx(P.sync_committee_size);
+    memcpy(both.data(), h->shadow + h->so.next_sync_committee, committee);
+    int32_t code = B200_SUCCESS;
+    int32_t rc = next_sync_committee(e, h, idx.data(), both.data() + committee, &code);
+    if (rc) return rc;
+    *out_code = code;
+    *rotated = 0;
+    if (code) return B200_SUCCESS;   // the reference's `?` before mem::replace: the state stays as it was
+    rc = update_bytes(e, h, h->so.current_sync_committee, both.data(), both.size());
+    if (rc) return rc;
+    *rotated = 1;
+    return B200_SUCCESS;
+}
 }  // namespace
 
 int32_t b200_state_get_seed(b200_state* h, uint64_t epoch, const uint8_t domain_type[4], uint8_t out[32]) {
@@ -904,27 +964,7 @@ int32_t b200_state_sync_committee_updates(b200_state* h, int32_t* rotated, int32
     int32_t rc = check_ready(e);
     if (rc) return rc;
     if (!duty_handle_ok(h) || !rotated || !out_code) return B200_ERR_BAD_ARG;
-    const DutyPreset P = duty_preset(h->preset);
-    const uint64_t next_epoch = shadow_slot(h) / P.slots_per_epoch + 1;
-    if (next_epoch % P.epochs_per_sync_committee_period != 0) {
-        *rotated = 0; *out_code = B200_SUCCESS;
-        return B200_SUCCESS;
-    }
-    // current_sync_committee <- next_sync_committee <- get_next_sync_committee: the two fields are adjacent, one patch
-    const size_t committee = (size_t(P.sync_committee_size) + 1) * 48;
-    std::vector<uint8_t> both(2 * committee);
-    std::vector<uint64_t> idx(P.sync_committee_size);
-    memcpy(both.data(), h->shadow + h->so.next_sync_committee, committee);
-    int32_t code = B200_SUCCESS;
-    rc = next_sync_committee(e, h, idx.data(), both.data() + committee, &code);
-    if (rc) return rc;
-    *out_code = code;
-    *rotated = 0;
-    if (code) return B200_SUCCESS;   // the reference's `?` before mem::replace: the state stays as it was
-    rc = update_bytes(e, h, h->so.current_sync_committee, both.data(), both.size());
-    if (rc) return rc;
-    *rotated = 1;
-    return B200_SUCCESS;
+    return sync_committee_updates(e, h, rotated, out_code);
 }
 
 int32_t b200_state_sync_committee_indices(b200_state* h, int32_t which, uint64_t* out) {
@@ -947,6 +987,249 @@ int32_t b200_state_sync_committee_indices(b200_state* h, int32_t which, uint64_t
     B200_CUDA_TRY(cudaEventSynchronize(e.ev1));
     B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, e.ev0, e.ev1));
     memcpy(out, res.data(), res.size() * 8);
+    return B200_SUCCESS;
+}
+
+// ---- process_epoch on a resident state (deneb/spec/mod.rs:965-1003) ----
+namespace {
+uint64_t le64(const uint8_t* p) {
+    uint64_t v = 0;
+    for (int k = 7; k >= 0; k--) v = (v << 8) | p[k];
+    return v;
+}
+// floor(sqrt(x)) exactly (u64::integer_sqrt): Newton's iteration on integers from above
+uint64_t integer_sqrt(uint64_t x) {
+    if (x < 2) return x;
+    unsigned __int128 r = x, y = (r + 1) / 2;
+    while (y < r) { r = y; y = (r + x / r) / 2; }
+    return uint64_t(r);
+}
+// get_block_root (:2552, :2582) from the shadow's block_roots; false where the reference returns SlotOutOfRange
+bool block_root(const b200_state* h, const DutyPreset& P, uint64_t slot, uint64_t epoch, const uint8_t** root) {
+    const uint64_t at = epoch * P.slots_per_epoch;
+    if (at >= slot || slot > at + P.slots_per_historical_root) return false;
+    *root = h->shadow + h->so.block_roots + 32 * (at % P.slots_per_historical_root);
+    return true;
+}
+constexpr uint32_t kPerValidatorSteps = B200_EPOCH_INACTIVITY_UPDATES | B200_EPOCH_REWARDS_AND_PENALTIES |
+                                        B200_EPOCH_REGISTRY_UPDATES | B200_EPOCH_SLASHINGS | B200_EPOCH_EFFECTIVE_BALANCE_UPDATES;
+}  // namespace
+
+int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_code) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || !out_code || (steps & ~uint32_t(B200_EPOCH_ALL))) return B200_ERR_BAD_ARG;
+    *out_code = B200_SUCCESS;
+    const DutyPreset P = duty_preset(h->preset);
+    const uint64_t n = big_count(h, 0);
+    for (int f = 1; f < 5; f++)
+        if (big_count(h, f) != n) { e.last_error = "process_epoch: the five big lists differ in length"; return B200_ERR_BAD_ARG; }
+    uint8_t* dev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // validators, balances, participation x 2, scores
+    for (int f = 0; f < 5 && n; f++) {
+        uint64_t off = 0; size_t nbytes = 0;
+        if (!h->plan.chain_field(f, &off, &nbytes)) return B200_ERR_BAD_ARG;
+        dev[f] = static_cast<uint8_t*>(h->fields.p) + off;
+    }
+    const uint64_t slot = shadow_slot(h), cur = slot / P.slots_per_epoch, prev = cur ? cur - 1 : 0, next = cur + 1;
+    const uint64_t inc = P.effective_balance_increment;
+    B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
+    EpochTotals T;
+    rc = epoch_totals_on_device(e, dev[0], dev[2], dev[3], n, cur, prev, P.ejection_balance, &T);
+    if (rc) return rc;
+
+    // ---- the host step: every refusal is decided here, before anything is written ----
+    const bool run_jf = (steps & B200_EPOCH_JUSTIFICATION_AND_FINALIZATION) && cur > 1;
+    const bool run_inactivity = (steps & B200_EPOCH_INACTIVITY_UPDATES) && cur > 0;
+    const bool run_rewards = (steps & B200_EPOCH_REWARDS_AND_PENALTIES) && cur > 0;
+    const bool run_sync = (steps & B200_EPOCH_SYNC_COMMITTEE_UPDATES) && next % P.epochs_per_sync_committee_period == 0;
+    const bool run_summary = (steps & B200_EPOCH_HISTORICAL_SUMMARIES_UPDATE) &&
+                             next % (P.slots_per_historical_root / P.slots_per_epoch) == 0;
+    // get_total_balance: checked sum, then at least one increment
+    const bool total_read = run_jf || run_rewards || (steps & B200_EPOCH_SLASHINGS);
+    if ((total_read && T.hi[0]) || (run_jf && (T.hi[2] || T.hi[4])) || (run_rewards && (T.hi[1] || T.hi[2] || T.hi[3]))) {
+        e.last_error = "process_epoch: get_total_balance overflows u64";
+        return B200_ERR_LIMIT;
+    }
+    auto total = [&](int k) { return std::max(T.lo[k], inc); };
+    uint8_t jf[121];   // justification_bits, previous_justified, current_justified, finalized (adjacent)
+    memcpy(jf, h->shadow + h->so.justification_bits, sizeof(jf));
+    if (run_jf) {   // weigh_justification_and_finalization (:1469-1520)
+        const uint64_t old_pj = le64(jf + 1), old_cj = le64(jf + 41);
+        uint8_t cp_pj[40], cp_cj[40];
+        memcpy(cp_pj, jf + 1, 40); memcpy(cp_cj, jf + 41, 40);
+        memcpy(jf + 1, cp_cj, 40);
+        uint8_t bits = uint8_t(((jf[0] << 1) & 0x0e) | (jf[0] & 0xf0));
+        const uint64_t active = total(0);
+        const uint64_t targets[2] = {total(2), total(4)}, epochs[2] = {prev, cur};
+        for (int k = 0; k < 2; k++) {
+            if (targets[k] * 3 < active * 2) continue;
+            const uint8_t* root;
+            if (!block_root(h, P, slot, epochs[k], &root)) { e.last_error = "process_epoch: get_block_root out of range"; return B200_ERR_BAD_ARG; }
+            for (int b = 0; b < 8; b++) jf[41 + b] = uint8_t(epochs[k] >> (8 * b));
+            memcpy(jf + 49, root, 32);
+            bits |= uint8_t(k == 0 ? 2 : 1);
+        }
+        jf[0] = bits;
+        if ((bits & 0x0e) == 0x0e && old_pj + 3 == cur) memcpy(jf + 81, cp_pj, 40);
+        if ((bits & 0x06) == 0x06 && old_pj + 2 == cur) memcpy(jf + 81, cp_pj, 40);
+        if ((bits & 0x07) == 0x07 && old_cj + 2 == cur) memcpy(jf + 81, cp_cj, 40);
+        if ((bits & 0x03) == 0x03 && old_cj + 1 == cur) memcpy(jf + 81, cp_cj, 40);
+    }
+    EpochParams p{};
+    p.steps = steps & kPerValidatorSteps;
+    if (!run_inactivity) p.steps &= ~uint32_t(B200_EPOCH_INACTIVITY_UPDATES);
+    if (!run_rewards) p.steps &= ~uint32_t(B200_EPOCH_REWARDS_AND_PENALTIES);
+    p.cur = cur; p.prev = prev;
+    p.finalized_epoch = le64(jf + 81);
+    p.leak = prev - p.finalized_epoch > P.min_epochs_to_inactivity_penalty;   // get_finality_delay wraps
+    p.total_active = total(0);
+    p.base_per_inc = inc * P.base_reward_factor / integer_sqrt(p.total_active);
+    p.active_inc = p.total_active / inc;
+    for (int f = 0; f < 3; f++) p.part_inc[f] = total(1 + f) / inc;
+    // the exit queue (initiate_validator_exit, :3062-3111) in closed form, and the activation churn
+    p.churn = std::max(P.min_per_epoch_churn_limit, T.n_active_cur / P.churn_limit_quotient);
+    p.activation_epoch = cur + 1 + P.max_seed_lookahead;
+    const uint64_t max_exit = T.max_exit_plus1 - 1;
+    p.exit0 = T.max_exit_plus1 ? std::max(max_exit, p.activation_epoch) : p.activation_epoch;
+    p.c0 = T.max_exit_plus1 && max_exit == p.exit0 ? T.n_at_max_exit : 0;
+    if ((steps & B200_EPOCH_REGISTRY_UPDATES) && T.n_eject) {
+        const uint64_t k = T.n_eject - 1;
+        const unsigned __int128 last = p.c0 < p.churn ? (unsigned __int128)p.exit0 + (p.c0 + k) / p.churn
+                                                      : (unsigned __int128)p.exit0 + 1 + k / p.churn;
+        if (last + P.min_validator_withdrawability_delay > ~uint64_t(0)) {
+            e.last_error = "process_epoch: an ejected validator's withdrawable_epoch overflows u64";
+            return B200_ERR_LIMIT;
+        }
+    }
+    p.activation_limit = (steps & B200_EPOCH_REGISTRY_UPDATES) ? uint32_t(std::min(P.max_per_epoch_activation_churn_limit, p.churn)) : 0;
+    p.slash_epoch = cur + P.epochs_per_slashings_vector / 2;
+    uint64_t slashings_sum = 0;   // `.sum::<Gwei>()` wraps in a release build
+    for (uint64_t k = 0; k < P.epochs_per_slashings_vector; k++) slashings_sum += le64(h->shadow + h->so.slashings + 8 * k);
+    p.adjusted_slashing = std::min(slashings_sum * P.proportional_slashing_multiplier_bellatrix, p.total_active);
+    p.increment = inc;
+    p.max_effective = P.max_effective_balance;
+    p.ejection_balance = P.ejection_balance;
+    p.hysteresis_down = inc / P.hysteresis_quotient * P.hysteresis_downward_multiplier;
+    p.hysteresis_up = inc / P.hysteresis_quotient * P.hysteresis_upward_multiplier;
+    p.score_bias = P.inactivity_score_bias;
+    p.score_recovery = P.inactivity_score_recovery_rate;
+    p.inactivity_denominator = P.inactivity_score_bias * P.inactivity_penalty_quotient_bellatrix;
+    p.withdraw_delay = P.min_validator_withdrawability_delay;
+    if (run_sync && T.n_active_next == 0) { e.last_error = "process_epoch: no active validator for the next sync committee"; return B200_ERR_BAD_ARG; }
+    const uint64_t n_summaries = (h->so.var[9] - h->so.var[8]) / 64;
+    if (run_summary && n_summaries + 1 > historical_roots_limit(h->preset)) {
+        e.last_error = "process_epoch: historical_summaries is full";
+        return B200_ERR_LIMIT;
+    }
+
+    // ---- the per-validator steps and the participation rotation on the device ----
+    if (p.steps && n) {
+        const uint32_t* changed = nullptr;
+        uint64_t n_changed = 0;
+        rc = epoch_apply_on_device(e, dev[0], reinterpret_cast<uint64_t*>(dev[1]), reinterpret_cast<uint64_t*>(dev[4]), dev[2], n,
+                                   p, &changed, &n_changed);
+        if (rc) return rc;
+        // changed records: re-hash their paths, or the whole list once they are more than a sixteenth of it
+        if (n_changed > std::max<uint64_t>(4096, n / 16)) {
+            h->rehash[0] = 1;
+        } else if (n_changed) {
+            std::vector<uint32_t> idx(n_changed);
+            B200_CUDA_TRY(cudaMemcpyAsync(idx.data(), changed, n_changed * 4, cudaMemcpyDeviceToHost, e.stream));
+            B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+            h->dirty[0].insert(h->dirty[0].end(), idx.begin(), idx.end());
+        }
+        if (p.steps & (B200_EPOCH_REWARDS_AND_PENALTIES | B200_EPOCH_SLASHINGS | B200_EPOCH_EFFECTIVE_BALANCE_UPDATES))
+            h->rehash[1] = 1;
+        if (p.steps & B200_EPOCH_INACTIVITY_UPDATES) h->rehash[4] = 1;
+    }
+    if ((steps & B200_EPOCH_PARTICIPATION_FLAG_UPDATES) && n) {   // process_participation_flag_updates (:1231-1262)
+        B200_CUDA_TRY(cudaMemcpyAsync(dev[2], dev[3], n, cudaMemcpyDeviceToDevice, e.stream));
+        B200_CUDA_TRY(cudaMemsetAsync(dev[3], 0, n, e.stream));
+        h->rehash[2] = h->rehash[3] = 1;
+    }
+    B200_CUDA_TRY(cudaEventRecord(e.ev1, e.stream));
+    B200_CUDA_TRY(cudaEventSynchronize(e.ev1));
+    float ms = 0;
+    B200_CUDA_TRY(cudaEventElapsedTime(&ms, e.ev0, e.ev1));
+
+    // ---- the small fields, through the paths b200_state_update_bytes and the reshaping calls take ----
+    if (run_jf) {
+        rc = update_bytes(e, h, h->so.justification_bits, jf, sizeof(jf));
+        if (rc) return rc;
+    }
+    if ((steps & B200_EPOCH_ETH1_DATA_RESET) && next % P.epochs_per_eth1_voting_period == 0) {   // :1298-1328
+        rc = set_small(e, h, 1, nullptr, 0);
+        if (rc) return rc;
+    }
+    if (steps & B200_EPOCH_SLASHINGS_RESET) {   // :1371-1400
+        const uint8_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        rc = update_bytes(e, h, h->so.slashings + 8 * (next % P.epochs_per_slashings_vector), zero, 8);
+        if (rc) return rc;
+    }
+    if (steps & B200_EPOCH_RANDAO_MIXES_RESET) {   // :1401-1430
+        uint8_t mix[32];
+        memcpy(mix, h->shadow + h->so.randao_mixes + 32 * (cur % P.epochs_per_historical_vector), 32);
+        rc = update_bytes(e, h, h->so.randao_mixes + 32 * (next % P.epochs_per_historical_vector), mix, 32);
+        if (rc) return rc;
+    }
+    if (run_summary) {   // :929-964: hash_tree_root of block_roots and state_roots, pushed as one HistoricalSummary
+        SszPlan sp;
+        const uint64_t sphr = P.slots_per_historical_root;
+        std::vector<uint32_t> outs{sp.wide_chunks(sp.stage_field(h->shadow + h->so.block_roots, 32 * sphr), sphr, depth_for(sphr)),
+                                   sp.wide_chunks(sp.stage_field(h->shadow + h->so.state_roots, 32 * sphr), sphr, depth_for(sphr))};
+        const size_t old_bytes = n_summaries * 64;
+        std::vector<uint8_t> buf(old_bytes + 64);
+        memcpy(buf.data(), h->shadow + h->so.var[8], old_bytes);
+        rc = run_oneshot(e, sp, outs, buf.data() + old_bytes);
+        if (rc) return rc;
+        rc = set_small(e, h, 8, buf.data(), buf.size());
+        if (rc) return rc;
+    }
+    if (run_sync) {   // last: a failed aggregation leaves every earlier sub-step applied
+        int32_t rotated = 0;
+        rc = sync_committee_updates(e, h, &rotated, out_code);
+        if (rc) return rc;
+        ms += e.last_kernel_ms;
+    }
+    e.last_kernel_ms = ms;
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_serialized_len(b200_state* h, uint64_t* out_len) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || !out_len) return B200_ERR_BAD_ARG;
+    *out_len = h->len;
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_read_bytes(b200_state* h, uint64_t ssz_offset, uint8_t* out, size_t n) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!duty_handle_ok(h) || (n && !out) || ssz_offset > h->len || n > h->len - ssz_offset) return B200_ERR_BAD_ARG;
+    const uint64_t lo = ssz_offset, hi = ssz_offset + n;
+    auto from_shadow = [&](uint64_t a, uint64_t b) {
+        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
+        if (x < y) memcpy(out + (x - lo), h->shadow + x, y - x);
+    };
+    from_shadow(0, h->so.var[2]);
+    from_shadow(h->so.var[7], h->len);
+    for (int f = 0; f < 5; f++) {   // the big lists from HBM
+        const uint64_t a = h->so.var[kBigVar[f]], b = h->so.var[kBigVar[f] + 1];
+        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
+        if (x >= y) continue;
+        uint64_t field_off = 0; size_t nbytes = 0;
+        if (!h->plan.chain_field(f, &field_off, &nbytes)) return B200_ERR_BAD_ARG;
+        B200_CUDA_TRY(cudaMemcpyAsync(out + (x - lo), static_cast<const uint8_t*>(h->fields.p) + field_off + (x - a), y - x,
+                                      cudaMemcpyDeviceToHost, e.stream));
+    }
+    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
     return B200_SUCCESS;
 }
 

@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "engine.h"
+#include "records.cuh"
 #include "sha256.cuh"
 #include "shuffle.h"
 
@@ -104,22 +105,13 @@ __global__ void __launch_bounds__(kThreads) k_shuffle_map(const uint64_t* __rest
     out[i] = indices ? indices[idx] : uint64_t(idx);
 }
 
-__device__ __forceinline__ uint64_t load_le64_unaligned(const uint8_t* p) {
-    uint64_t v = 0;
-#pragma unroll
-    for (int k = 7; k >= 0; k--) v = (v << 8) | p[k];
-    return v;
-}
-// is_active_validator(v, epoch): activation_epoch <= epoch < exit_epoch; record layout phase0/validator.rs:10-26:
-// pubkey 0..48, withdrawal_credentials 48..80, effective_balance 80..88, slashed 88, activation_eligibility_epoch 89..97,
-// activation_epoch 97..105, exit_epoch 105..113, withdrawable_epoch 113..121
+// is_active_validator(v, epoch) over the records (records.cuh)
 __global__ void __launch_bounds__(kThreads) k_active_count(const uint8_t* __restrict__ recs, uint64_t n, uint64_t epoch,
                                                              uint32_t* __restrict__ block_counts) {
     const uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     bool act = false;
     if (i < n) {
-        const uint8_t* r = recs + i * 121;
-        act = load_le64_unaligned(r + 97) <= epoch && epoch < load_le64_unaligned(r + 105);
+        act = record_active(recs + i * 121, epoch);
     }
     const int c = __syncthreads_count(act ? 1 : 0);
     if (threadIdx.x == 0) block_counts[blockIdx.x] = uint32_t(c);
@@ -149,8 +141,7 @@ __global__ void __launch_bounds__(kThreads) k_active_scatter(const uint8_t* __re
     const uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     bool act = false;
     if (i < n) {
-        const uint8_t* r = recs + i * 121;
-        act = load_le64_unaligned(r + 97) <= epoch && epoch < load_le64_unaligned(r + 105);
+        act = record_active(recs + i * 121, epoch);
     }
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t m = __ballot_sync(0xffffffffu, act);
@@ -218,7 +209,7 @@ __device__ __forceinline__ uint32_t sample_window(const uint32_t sw[8], const ui
             return digest_word(h, (pos & 255u) >> 5);
         });
     const uint64_t c = active[idx];
-    const uint64_t eff = load_le64_unaligned(recs + c * 121 + 80);
+    const uint64_t eff = load_le64_unaligned(recs + c * 121 + kRecEffectiveBalance);
     uint32_t h[8];
     sha256_seed_le64(sw, window, h);
     const uint64_t byte = (digest_word(h, lane >> 2) >> (24u - 8u * (lane & 3u))) & 0xffu;

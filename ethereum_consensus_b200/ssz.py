@@ -189,6 +189,25 @@ class DeviceBeaconState:
         self.append_elements("current_epoch_participation", np.zeros(n, np.uint8))
         self.append_elements("inactivity_scores", np.zeros(n, "<u8"))
 
+    # ---- read-back: the serialization as the resident state holds it (big lists from HBM, the rest from the host copy) ----
+    def serialized_len(self) -> int:
+        n = C.c_uint64(0)
+        _lib.check(_lib.lib().b200_state_serialized_len(self._h, C.byref(n)), "state_serialized_len")
+        return n.value
+
+    def read_bytes(self, offset: int, n: int) -> bytes:
+        """Bytes [offset, offset + n) of the serialization, in the coordinates `update_bytes` takes."""
+        out = np.zeros(n, dtype=np.uint8)
+        _lib.check(_lib.lib().b200_state_read_bytes(self._h, offset, _lib.ptr(out), n), "state_read_bytes")
+        return out.tobytes()
+
+    def serialize(self) -> np.ndarray:
+        """The whole SSZ serialization as a uint8 array."""
+        n = self.serialized_len()
+        out = np.zeros(n, dtype=np.uint8)
+        _lib.check(_lib.lib().b200_state_read_bytes(self._h, 0, _lib.ptr(out), n), "state_read_bytes")
+        return out
+
     def hash_tree_root_incremental(self) -> bytes:
         out = _out32()
         _rc(_lib.lib().b200_state_root_incremental(self._h, out), "state_root_incremental")

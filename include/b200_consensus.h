@@ -195,6 +195,62 @@ B200_API int32_t b200_state_next_sync_committee(b200_state* handle, uint64_t* ou
 B200_API int32_t b200_state_sync_committee_updates(b200_state* handle, int32_t* rotated, int32_t* out_code);
 B200_API int32_t b200_state_sync_committee_indices(b200_state* handle, int32_t which, uint64_t* out);
 
+/* Epoch processing on a device-resident state (single-GPU handles, as the duties above).  Sub-steps of deneb
+ * process_epoch (deneb/spec/mod.rs:991-1002), in the reference's order: */
+#define B200_EPOCH_JUSTIFICATION_AND_FINALIZATION  (1u << 0)
+#define B200_EPOCH_INACTIVITY_UPDATES              (1u << 1)
+#define B200_EPOCH_REWARDS_AND_PENALTIES           (1u << 2)
+#define B200_EPOCH_REGISTRY_UPDATES                (1u << 3)
+#define B200_EPOCH_SLASHINGS                       (1u << 4)
+#define B200_EPOCH_ETH1_DATA_RESET                 (1u << 5)
+#define B200_EPOCH_EFFECTIVE_BALANCE_UPDATES       (1u << 6)
+#define B200_EPOCH_SLASHINGS_RESET                 (1u << 7)
+#define B200_EPOCH_RANDAO_MIXES_RESET              (1u << 8)
+#define B200_EPOCH_HISTORICAL_SUMMARIES_UPDATE     (1u << 9)
+#define B200_EPOCH_PARTICIPATION_FLAG_UPDATES      (1u << 10)
+#define B200_EPOCH_SYNC_COMMITTEE_UPDATES          (1u << 11)
+#define B200_EPOCH_ALL                             0xfffu
+/*  - b200_state_process_epoch applies the selected sub-steps, each with exactly the effect of the reference function of
+ *    that name; one bit is one handler of spec-tests/runners/epoch_processing.rs, B200_EPOCH_ALL is process_epoch.  The
+ *    mask only skips work.  Afterwards b200_state_root_incremental and b200_state_root both give the post-epoch root.
+ *    A NULL, not uploaded or sharded handle, a NULL out_code, a mask bit above bit 11, or a state whose five big lists
+ *    differ in length -> B200_ERR_BAD_ARG.  b200_last_kernel_ms: the device time of the call.
+ *    Where the reference returns Err, the call refuses before writing anything (the state stays byte for byte as it was):
+ *      - get_block_root out of range (:2582), asked only when a 2/3 target test passes -> B200_ERR_BAD_ARG;
+ *      - get_total_balance's checked_add overflowing u64 (:2857-2868), for any sum a selected sub-step reads -> B200_ERR_LIMIT;
+ *      - the checked_add of an ejected validator's withdrawable_epoch (:3106-3109) -> B200_ERR_LIMIT;
+ *      - no validator active at the next epoch when the sync committees are due to rotate -> B200_ERR_BAD_ARG (the active
+ *        set at the next epoch does not depend on this epoch's registry changes);
+ *      - historical_summaries already at HISTORICAL_ROOTS_LIMIT when a summary is due -> B200_ERR_LIMIT.
+ *    One failure comes after the writes: the sync-committee aggregation, which runs last.  Its code is returned in
+ *    *out_code with B200_SUCCESS; every earlier sub-step stays applied and the committees stay as they were (what the
+ *    reference's `&mut state` holds at its `?`).
+ *    All other arithmetic wraps in u64, as a release build of the reference does: increase_balance,
+ *    effective_balance * inactivity_score, the reward numerators, base_reward * weight, the slashings sum and its
+ *    multiple, current_epoch + 1, balance + threshold, get_finality_delay.  decrease_balance saturates at zero.
+ *    integer_sqrt of the total active balance is the exact floor.  Inside a validator: the inactivity score updates before
+ *    the inactivity penalty reads it; the (reward, penalty) pairs apply in turn, flags 0, 1, 2, then inactivity, each
+ *    penalty saturating; ejection and the slashing test read withdrawable_epoch after the registry step; effective
+ *    balances read balances after the slashing penalty; the leak test and activation eligibility read
+ *    finalized_checkpoint after justification whenever that step runs.
+ *    The exit queue in closed form: ejections are assigned in index order; with E0 = max(the largest exit_epoch !=
+ *    FAR_FUTURE_EPOCH, compute_activation_exit_epoch(current)), c0 = the validators whose exit_epoch is E0 and
+ *    L = max(MIN_PER_EPOCH_CHURN_LIMIT, active / CHURN_LIMIT_QUOTIENT), the k-th ejection exits at E0 + (c0 + k) / L when
+ *    c0 < L and E0 + 1 + k / L otherwise, as initiate_validator_exit (:3062-3111) called once per ejection gives.  The
+ *    activation queue takes the first min(MAX_PER_EPOCH_ACTIVATION_CHURN_LIMIT, L) validators by
+ *    (activation_eligibility_epoch, index), the eligibility epochs as the first loop left them.
+ *    Preset constants: those of the duties, and SLOTS_PER_HISTORICAL_ROOT 8192 / 64, EPOCHS_PER_SLASHINGS_VECTOR
+ *    8192 / 64, EPOCHS_PER_ETH1_VOTING_PERIOD 64 / 4, MIN_PER_EPOCH_CHURN_LIMIT 4 / 2,
+ *    MAX_PER_EPOCH_ACTIVATION_CHURN_LIMIT 8 / 4, CHURN_LIMIT_QUOTIENT 65536 / 32 (mainnet / minimal); the rest are
+ *    equal in both (EJECTION_BALANCE 16 ETH, INACTIVITY_PENALTY_QUOTIENT_BELLATRIX 2^24,
+ *    PROPORTIONAL_SLASHING_MULTIPLIER_BELLATRIX 3, ...).
+ *  - b200_state_serialized_len / b200_state_read_bytes read the serialization back in the coordinates
+ *    b200_state_update_bytes takes, after any updates, reshapes or epochs: bytes inside the five big lists come from
+ *    HBM, the rest from the host copy.  A range past the end -> B200_ERR_BAD_ARG. */
+B200_API int32_t b200_state_process_epoch(b200_state* handle, uint32_t steps, int32_t* out_code);
+B200_API int32_t b200_state_serialized_len(b200_state* handle, uint64_t* out_len);
+B200_API int32_t b200_state_read_bytes(b200_state* handle, uint64_t ssz_offset, uint8_t* out, size_t n);
+
 /* ---- multi-GPU: one process per GPU, the exchange step lives INSIDE the library (SURVEY.md §8b `b200_init(n_gpus)`,
  * §8e).  The reference is single-process (no counterpart, SURVEY.md §2a); a Rust host with one process per GPU calls:
  *   rank 0:   b200_comm_unique_id(id)  -> ships the 128 bytes to the other ranks by any means it likes (pipe, file, TCP)
