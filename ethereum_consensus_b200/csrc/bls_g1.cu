@@ -61,6 +61,58 @@ __global__ void __maxnreg__(128) k_g1_validate_r128(const uint8_t* __restrict__ 
                                                     int32_t* __restrict__ codes) {
     g1_validate_body(keys, n, out, codes);
 }
+// The default launch of 384-thread CTAs (variant 7): the same 168-register budget split by role, so that both multiply
+// pipes of an SM work on the same keys.  Warps 0-7 run the subgroup checks of the CTA's 256 keys on the integer pipe
+// (g1_in_subgroup_iso, which needs x only); warps 8-11 run their square roots on the FP64 pipe (g1_y_from_x_fpd), two
+// keys per thread, one after the other.  One barrier, then each integer thread merges its key's code in the
+// reference's order and writes the point.  (Separate kernels on two streams would not share an SM: either one fills its
+// register file.)
+constexpr int kSplitIntThreads = 256, kSplitThreads = 384;
+__global__ void __maxnreg__(168) k_g1_validate_split(const uint8_t* __restrict__ keys, uint32_t n, G1Aff* __restrict__ out,
+                                                     int32_t* __restrict__ codes) {
+    __shared__ Fp s_y[kSplitIntThreads];
+    __shared__ uint8_t s_on_curve[kSplitIntThreads];
+    const uint32_t base = blockIdx.x * kSplitIntThreads;
+    __align__(16) uint8_t b[48];  // written through uint4*
+    Fp x;
+    uint32_t inf = 0;
+    bool largest = false, in_group = true;
+    int32_t rc = BLS_SUCCESS;
+    if (threadIdx.x < kSplitIntThreads) {
+        const uint32_t i = base + threadIdx.x;
+        if (i < n) {
+            const uint4* src = reinterpret_cast<const uint4*>(keys + size_t(i) * 48);
+            uint4* dst = reinterpret_cast<uint4*>(b);
+            dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
+            rc = g1_parse(x, inf, largest, b);
+            if (rc == BLS_SUCCESS && !inf) in_group = g1_in_subgroup_iso(x);
+        }
+    } else {
+#pragma unroll 1
+        for (uint32_t j = threadIdx.x - kSplitIntThreads; j < kSplitIntThreads; j += kSplitThreads - kSplitIntThreads) {
+            const uint32_t i = base + j;
+            if (i >= n) break;
+            const uint4* src = reinterpret_cast<const uint4*>(keys + size_t(i) * 48);
+            uint4* dst = reinterpret_cast<uint4*>(b);
+            dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
+            Fp y = fp_zero();
+            bool on_curve = true;
+            if (g1_parse(x, inf, largest, b) == BLS_SUCCESS && !inf) on_curve = g1_y_from_x_fpd(y, x, largest);
+            s_y[j] = y;
+            s_on_curve[j] = on_curve;
+        }
+    }
+    __syncthreads();
+    const uint32_t i = base + threadIdx.x;
+    if (threadIdx.x >= kSplitIntThreads || i >= n) return;
+    rc = g1_key_validate_code(rc, inf, s_on_curve[threadIdx.x] != 0, in_group);
+    codes[i] = rc;
+    if (rc == BLS_SUCCESS) {
+        G1Aff p;
+        p.x = x; p.y = s_y[threadIdx.x]; p.inf = 0;
+        out[i] = p;
+    }
+}
 constexpr int kAggWarps = 4;
 
 __global__ void __launch_bounds__(32 * kAggWarps) k_g1_aggregate(const G1Aff* __restrict__ keys,
@@ -338,13 +390,13 @@ static size_t k1_smem(K kernel, unsigned threads) {
     return with_pow_tab(kernel, threads);   // fp_sqrt -> fp_pow
 #else
     (void)threads;
-    static const void* done[3];
+    static const void* done[4];
     static int n_done = 0;
     const void* key = reinterpret_cast<const void*>(kernel);
     for (int i = 0; i < n_done; i++)
         if (done[i] == key) return 0;
     cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 0);
-    if (n_done < 3) done[n_done++] = key;
+    if (n_done < 4) done[n_done++] = key;
     return 0;
 #endif
 }
@@ -360,12 +412,14 @@ void launch_g1_validate(const uint8_t* keys, uint32_t n, G1Aff* out, int32_t* co
     case 6: k_g1_validate_r128<<<(n + 511) / 512, 512, k1_smem(k_g1_validate_r128, 512), st>>>(keys, n, out, codes); break;
     case 0: k_g1_validate_main<<<(n + 255) / 256, 256, k1_smem(k_g1_validate_main, 256), st>>>(keys, n, out, codes); break;
     default:
-        // 12 warps per SM either way; below ~3 full waves of 384-thread CTAs the same kernel goes out as three 128-thread
-        // CTAs per SM, so that the last, partial wave spreads over all SMs instead of leaving most of them idle
+        // 12 warps per SM either way; below ~3 full waves of 384-thread CTAs the keys go out as three 128-thread CTAs per
+        // SM of the unsplit kernel, so that the last, partial wave spreads over all SMs instead of leaving most of them
+        // idle; larger launches run the role-split kernel
         if (cta == 128 || (cta != 384 && n <= g_g1_small_n))
             k_g1_validate_r168<<<(n + 127) / 128, 128, k1_smem(k_g1_validate_r168, 128), st>>>(keys, n, out, codes);
         else
-            k_g1_validate_r168<<<(n + 383) / 384, 384, k1_smem(k_g1_validate_r168, 384), st>>>(keys, n, out, codes);
+            k_g1_validate_split<<<(n + kSplitIntThreads - 1) / kSplitIntThreads, kSplitThreads,
+                                  k1_smem(k_g1_validate_split, kSplitThreads), st>>>(keys, n, out, codes);
         break;
     }
 }

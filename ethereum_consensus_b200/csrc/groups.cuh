@@ -5,7 +5,7 @@
 //   POINT_NOT_ON_CURVE(2), POINT_NOT_IN_GROUP(3), PK_IS_INFINITY(6)
 #pragma once
 #include "curve.cuh"
-#include "fpl.cuh"
+#include "fpd.cuh"
 
 namespace b200 {
 
@@ -106,6 +106,51 @@ B200_HD bool g1_in_subgroup_lazy(const G1Aff& p) {
     f_mul(bx, px, fpl_from_fp(beta));
     f_neg(ny, py);
     return jac_eq_aff(t2, bx, ny);
+}
+
+// ---- the per-key kernel's split: the square root on the FP64 pipe (fpd.cuh), the subgroup check on x alone --------
+// the encoding checks of g1_uncompress_lazy: BLS_BAD_ENCODING, or success with inf = 1, or x and the sign flag
+B200_HD int32_t g1_parse(Fp& x, uint32_t& inf, bool& largest, const uint8_t b[48]) {
+    const uint8_t f = b[0];
+    inf = 0;
+    largest = (f & 0x20) != 0;
+    if (!(f & 0x80)) return BLS_BAD_ENCODING;
+    if (f & 0x40) {
+        if ((f & 0x3f) == 0 && bytes_all_zero(b + 1, 47)) { inf = 1; return BLS_SUCCESS; }
+        return BLS_BAD_ENCODING;
+    }
+    return fp_from_be48_masked(x, b, true) ? BLS_SUCCESS : BLS_BAD_ENCODING;
+}
+// g1_in_subgroup_lazy for a point with abscissa x, without its y: on E_u: Y^2 = X^3 + 4u^3 with u = x^3 + 4, which
+// iota(x, y) = (u x, y^4) = (u x, u^2) maps E onto (lambda = y: X = lambda^2 x, Y = lambda^3 y).  The a = 0 formulas
+// never read b, phi(X, Y) = (beta X, Y) commutes with iota, and iota is a group isomorphism, so
+// phi(P') == -[z^2]P' exactly when phi(P) == -[z^2]P, with the same exceptional branches taken in the ladders.  u != 0
+// for every x in Fp (#E(Fp) is odd, so E has no point with y = 0).  For an x that is not on E the answer is
+// meaningless, and the square root's BLS_POINT_NOT_ON_CURVE takes precedence.
+B200_HD bool g1_in_subgroup_iso(const Fp& x) {
+    const FpL xl = fpl_from_fp(x);
+    FpL u, px, py;
+    f_sqr(u, xl);
+    f_mul(u, u, xl);
+    f_add(u, u, curve_b<FpL>());
+    f_mul(px, xl, u);
+    f_sqr(py, u);
+    Jac<FpL> t, t2;
+    jac_mul_u64(t, px, py, B200_Z_ABS);
+    jac_mul_u64_jac_cached(t2, t, B200_Z_ABS);
+    const Fp beta = B200_FP_BETA;
+    FpL bx, ny;
+    f_mul(bx, px, fpl_from_fp(beta));
+    f_neg(ny, py);
+    return jac_eq_aff(t2, bx, ny);
+}
+// g1_key_validate's code from the two halves, in the reference's order: BAD_ENCODING, NOT_ON_CURVE, PK_IS_INFINITY,
+// POINT_NOT_IN_GROUP (parse_rc and inf from g1_parse, on_curve from g1_y_from_x_fpd, in_group from g1_in_subgroup_iso)
+B200_HD int32_t g1_key_validate_code(int32_t parse_rc, uint32_t inf, bool on_curve, bool in_group) {
+    if (parse_rc) return parse_rc;
+    if (inf) return BLS_PK_IS_INFINITY;
+    if (!on_curve) return BLS_POINT_NOT_ON_CURVE;
+    return in_group ? BLS_SUCCESS : BLS_POINT_NOT_IN_GROUP;
 }
 
 // blst `PublicKey::key_validate`.  -DB200_G1_CANONICAL_FP selects the fully reduced arithmetic (round 1's path).

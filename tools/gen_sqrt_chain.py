@@ -1,22 +1,30 @@
-"""Generates ethereum_consensus_b200/csrc/fpl_sqrt_chain.cuh: y = c^((p+1)/4) on the lazily reduced field (fpl.cuh) as a
-fixed addition chain, every temporary a named register variable.
+"""Generates ethereum_consensus_b200/csrc/fpl_sqrt_chain.cuh and fpd_sqrt_chain.cuh: y = c^((p+1)/4) on the lazily
+reduced field (fpl.cuh) and on the FP64 field (fpd.cuh) as a fixed addition chain, every temporary a named register
+variable.
 
 The chain is a sliding-window decomposition of the exponent over a small dictionary of odd powers, chosen with a
 shortest-cover dynamic programme.  Besides the small odd powers the dictionary holds c^255: the exponent has runs of 33,
 19 and 17 one-bits, which 8-bit windows cover with a quarter of the products of 4-bit windows.  The chain is checked with
 Python big integers (evaluate()) before the header is written.  Run from the repo root:  python tools/gen_sqrt_chain.py
-(`--check` compares with the committed header instead of writing it).
+(`--check` compares with the committed headers instead of writing them).
+
+An FpD element is 16 registers, so the FP64 chain keeps at most FPD_DICT_CAP odd powers: best_dictionary() picks the
+cap-sized dictionary of the cheapest chain, a product weighted FPD_MUL_WEIGHT squarings (the FP64-pipe instructions of
+fpd_mul_core over fpd_sqr_core in the sm_90a build).
 """
 import sys
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 HEADER = ROOT / "ethereum_consensus_b200" / "csrc" / "fpl_sqrt_chain.cuh"
+FPD_HEADER = ROOT / "ethereum_consensus_b200" / "csrc" / "fpd_sqrt_chain.cuh"
 
 P = 0x1a0111ea397fe69a4b1ba7b6434bacd764774b84f38512bf6730d2a0f6b0f6241eabfffeb153ffffb9feffffffffaaab
 EXP = (P + 1) // 4
 # odd powers of c kept for the windows, each built from earlier ones (build_dictionary)
 DICT = (1, 3, 5, 7, 9, 11, 13, 15, 21, 255)
+FPD_DICT_CAP = 5
+FPD_MUL_WEIGHT = 1.25
 
 
 def build_dictionary(dictionary):
@@ -100,7 +108,28 @@ def cost(prog):
     return s, sum(1 for op in prog if op[0] == "mul")
 
 
-def render(prog):
+def best_dictionary(cap, mul_weight, e=EXP):
+    """The dictionary of at most `cap` odd powers (c^1 among them) whose chain costs least, squarings + mul_weight x
+    products; ties go to the first in lexicographic order."""
+    from itertools import combinations
+    best = None
+    candidates = [v for v in range(3, 256, 2)
+                  if v < 32 or v in (63, 127, 255)]
+    for n in range(cap):
+        for rest in combinations(candidates, n):
+            d = (1,) + rest
+            try:
+                prog = chain(e, d)
+            except AssertionError:
+                continue
+            s, m = cost(prog)
+            c = s + mul_weight * m
+            if best is None or c < best[0]:
+                best = (c, d)
+    return best[1]
+
+
+def render(prog, dictionary=DICT):
     s, m = cost(prog)
     names = sorted({op[1] for op in prog if op[1] not in ("x1", "acc")}, key=lambda v: int(v[1:]))
     body = []
@@ -115,7 +144,7 @@ def render(prog):
             body.append(f"    f_mul({op[1]}, {op[2]}, {op[3]});")
     return (
         "// GENERATED by tools/gen_sqrt_chain.py — do not edit.  Included from fpl.cuh.\n"
-        f"// r = a^((p+1)/4) by a fixed addition chain: {s} squarings + {m} products, windows over c^{{{', '.join(map(str, DICT))}}}.\n"
+        f"// r = a^((p+1)/4) by a fixed addition chain: {s} squarings + {m} products, windows over c^{{{', '.join(map(str, dictionary))}}}.\n"
         "#pragma once\n\n"
         "namespace b200 {\n\n"
         "B200_BIG void fpl_sqrt_chain(FpL& r, const FpL& x1) {\n"
@@ -126,15 +155,27 @@ def render(prog):
         "}  // namespace b200\n")
 
 
+def render_fpd(prog, dictionary):
+    """The same program on FpD (fpd.cuh): products and squaring runs are calls there."""
+    text = render(prog, dictionary)
+    for a, b in (("Included from fpl.cuh", "Included from fpd.cuh"), ("fpl_sqrt_chain(FpL& r, const FpL& x1)",
+                 "fpd_sqrt_chain(FpD& r, const FpD& x1)"), ("    FpL ", "    FpD "), ("f_sqr(", "fpd_sqr("),
+                 ("f_mul(", "fpd_mul("), ("fpl_sqr_n(", "fpd_sqr_n(")):
+        text = text.replace(a, b)
+    return text
+
+
 def main(argv):
-    prog = chain()
-    assert evaluate(prog) == EXP, "the chain does not evaluate to (p+1)/4"
-    text = render(prog)
-    if "--check" in argv:
-        assert HEADER.read_text() == text, f"{HEADER.name} differs from what tools/gen_sqrt_chain.py generates"
-        return
-    HEADER.write_text(text)
-    print(f"wrote {HEADER.name}: {cost(prog)[0]} squarings + {cost(prog)[1]} products")
+    fpd_dict = best_dictionary(FPD_DICT_CAP, FPD_MUL_WEIGHT)
+    for path, dictionary, rend in ((HEADER, DICT, render), (FPD_HEADER, fpd_dict, render_fpd)):
+        prog = chain(EXP, dictionary)
+        assert evaluate(prog) == EXP, "the chain does not evaluate to (p+1)/4"
+        text = rend(prog, dictionary)
+        if "--check" in argv:
+            assert path.read_text() == text, f"{path.name} differs from what tools/gen_sqrt_chain.py generates"
+            continue
+        path.write_text(text)
+        print(f"wrote {path.name}: {cost(prog)[0]} squarings + {cost(prog)[1]} products over c^{dictionary}")
 
 
 if __name__ == "__main__":
