@@ -399,12 +399,15 @@ FP_EVAL_OPS = {"fp_mul": 0, "fp_sqr": 1, "fpl_mul": 2, "fpl_sqr": 3, "fp_add": 4
                "fpl_sub": 8, "fpl_neg": 9, "fp_add_raw": 10, "fp_sub_raw": 11, "fp_inv_kaliski": 12, "fp_inv_fermat": 13,
                "fp_sqrt": 14, "fpl_pow_sqrt": 15, "fp_is_lex_largest": 16, "fpl_sqrt_chain": 18,
                "fpl_mul_sub_mul": 19, "fpl_mul_sub_8sqr": 20,
-               "fp2_mul": 32, "fp2_sqr": 33, "fp2_inv": 34, "fp2_sqrt": 35, "fp2_sgn0": 36}
+               "fp2_mul": 32, "fp2_sqr": 33, "fp2_inv": 34, "fp2_sqrt": 35, "fp2_sgn0": 36,
+               "fpd_mul": 40, "fpd_sqr": 41, "fpd_add": 42, "fpd_from_fp": 43, "fpd_to_fpl": 44, "fpd_sqrt_chain": 45,
+               "fpd_y_from_x": 46}
 
 
 def fp_eval(op: str, a, b=None) -> np.ndarray:
-    """Self-test: one device field operation on raw limbs.  a, b: uint32[n, 24] (Fp in columns 0..11, Fp2 c0 | c1);
-    returns uint32[n, 25]: the result's limbs, then the flag word (carry, borrow, is-square, lex-largest or sgn0)."""
+    """Self-test: one device field operation on raw limbs.  a, b: uint32[n, 24] (Fp in columns 0..11, Fp2 c0 | c1, FpD
+    as 8 binary64 limbs in columns 0..15, i.e. a.view(np.float64)[:, :8]); returns uint32[n, 25]: the result's limbs,
+    then the flag word (carry, borrow, is-square, on-curve, lex-largest or sgn0)."""
     a = np.ascontiguousarray(a, dtype=np.uint32)
     b = np.zeros_like(a) if b is None else np.ascontiguousarray(b, dtype=np.uint32)
     if a.ndim != 2 or a.shape[1] != 24 or b.shape != a.shape:
@@ -415,7 +418,7 @@ def fp_eval(op: str, a, b=None) -> np.ndarray:
 
 
 # operations of curve_eval (bls_kernels.cuh CURVE_G1L_* / CURVE_G2_*)
-CURVE_EVAL_OPS = {"g1l_add_mixed": 0, "g1l_add": 1, "g1l_in_subgroup": 2, "g1l_double": 4,
+CURVE_EVAL_OPS = {"g1l_add_mixed": 0, "g1l_add": 1, "g1l_in_subgroup": 2, "g1l_double": 4, "g1_in_subgroup_iso": 6,
                   "g2_add": 32, "g2_add_mixed": 33, "g2_double": 34, "g2_in_subgroup": 35, "g2_psi": 36,
                   "g2_clear_cofactor": 37, "g2_sswu_iso": 38, "g2_h2c_finish": 39}
 

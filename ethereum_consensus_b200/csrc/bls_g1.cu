@@ -300,6 +300,15 @@ __global__ void k_fp_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a
     const FpL xl = fpl_from_fp(x), yl = fpl_from_fp(y), x1l = fpl_from_fp(x1), y1l = fpl_from_fp(y1);
     FpL rl;
     uint32_t flag = 0;
+    // FpD operands and result: words 0..15 as 8 binary64 limbs, bit for bit
+    auto fpd_load = [](const uint32_t* w) {
+        FpD d;
+        for (int k = 0; k < 8; k++) d.l[k] = __hiloint2double(int(w[2 * k + 1]), int(w[2 * k]));
+        return d;
+    };
+    const FpD xd = fpd_load(a + size_t(i) * kFpEvalIn), yd = fpd_load(b + size_t(i) * kFpEvalIn);
+    FpD rd;
+    bool fpd_out = false;
     switch (op) {
     case FP_EVAL_MUL: fp_mul(r, x, y); break;
     case FP_EVAL_SQR: fp_sqr(r, x); break;
@@ -321,10 +330,22 @@ __global__ void k_fp_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a
     case FPL_EVAL_MUL_SUB_MUL: f_mul_sub_mul(rl, xl, x1l, yl, y1l); r = rl.v; break;
     case FPL_EVAL_MUL_SUB_8SQR: f_mul_sub_8sqr(rl, xl, x1l, yl); r = rl.v; break;
     case FP_EVAL_IS_LEX_LARGEST: flag = fp_is_lex_largest(x) ? 1u : 0u; break;
+    case FPD_EVAL_MUL: fpd_mul(rd, xd, yd); fpd_out = true; break;
+    case FPD_EVAL_SQR: fpd_sqr(rd, xd); fpd_out = true; break;
+    case FPD_EVAL_ADD: fpd_add(rd, xd, yd); fpd_out = true; break;
+    case FPD_EVAL_FROM_FP: rd = fpd_from_fp(x); fpd_out = true; break;
+    case FPD_EVAL_TO_FPL: r = fpd_to_fpl(xd).v; break;
+    case FPD_EVAL_SQRT_CHAIN: fpd_sqrt_chain(rd, fpd_from_fp(x)); r = fpd_to_fpl(rd).v; break;
+    case FPD_EVAL_Y_FROM_X: flag = g1_y_from_x_fpd(r, x, y.l[0] != 0) ? 1u : 0u; break;
     default: break;
     }
     uint32_t* o = out + size_t(i) * kFpEvalOut;
     for (int k = 0; k < 12; k++) { o[k] = r.l[k]; o[12 + k] = 0; }
+    if (fpd_out)
+        for (int k = 0; k < 8; k++) {
+            o[2 * k] = uint32_t(__double2loint(rd.l[k]));
+            o[2 * k + 1] = uint32_t(__double2hiint(rd.l[k]));
+        }
     o[24] = flag;
 }
 
@@ -354,6 +375,7 @@ __global__ void k_curve_eval(int32_t op, uint32_t n, const uint32_t* __restrict_
         flag = g1_in_subgroup_lazy(s) ? 1u : 0u;
         break;
     }
+    case CURVE_G1_IN_SUBGROUP_ISO: flag = g1_in_subgroup_iso(p.x.v) ? 1u : 0u; break;
     default: break;
     }
     uint32_t* o = out + size_t(i) * kCurveEvalWords;

@@ -108,7 +108,16 @@ enum : int32_t {
     FPL_EVAL_MUL_SUB_MUL = 19, FPL_EVAL_MUL_SUB_8SQR = 20,            // bls_g1.cu: (a0 a1 - b0 b1)/R, (a0 a1 - 8 b0^2)/R
     FPL_EVAL_END = 21,                                               //   (a0 / a1: words 0..11 / 12..23 of operand a)
     FP2_EVAL_MUL = 32, FP2_EVAL_SQR = 33, FP2_EVAL_INV = 34, FP2_EVAL_SQRT = 35, FP2_EVAL_SGN0 = 36,
-    FP2_EVAL_END = 37                                                // bls_g2.cu: the signature / hash kernels' build
+    FP2_EVAL_END = 37,                                               // bls_g2.cu: the signature / hash kernels' build
+    // bls_g1.cu: the FP64 field of the split per-key kernel (fpd.cuh).  An FpD operand or result is words 0..15 of its
+    // slot, 8 little-endian binary64 limbs (limb k an integer multiple of 2^(48k)), taken and returned as raw bits
+    FPD_EVAL_MUL = 40, FPD_EVAL_SQR = 41, FPD_EVAL_ADD = 42,          // FpD -> FpD
+    FPD_EVAL_FROM_FP = 43,                                           // Fp limbs (below 2^384 - 2^383) -> FpD
+    FPD_EVAL_TO_FPL = 44,                                            // FpD (|a| < 2p) -> Fp limbs in [0, 2p)
+    FPD_EVAL_SQRT_CHAIN = 45,                                        // Fp -> fpd_to_fpl(fpd_sqrt_chain(fpd_from_fp(a)))
+    FPD_EVAL_Y_FROM_X = 46,                                          // a: canonical Montgomery x, b word 0: sign flag ->
+                                                                     //   g1_y_from_x_fpd's y, flag = on the curve
+    FPD_EVAL_END = 47
 };
 constexpr uint32_t kFpEvalIn = 24, kFpEvalOut = 25;
 void launch_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out, void* stream);
@@ -120,6 +129,8 @@ enum : int32_t {
     CURVE_G1L_ADD_MIXED = 0, CURVE_G1L_ADD = 1, CURVE_G1L_IN_SUBGROUP = 2,
     CURVE_G1_N_OPS = 3,                                              // bls_g1.cu on FpL: the per-key kernel's formulas
     CURVE_G1L_DOUBLE = 4,                                            // bls_g1.cu as well; 3 stays unassigned
+    CURVE_G1_IN_SUBGROUP_ISO = 6,                                    // bls_g1.cu: g1_in_subgroup_iso(X), the split kernel's
+                                                                     //   check from x alone; 5 stays unassigned
     CURVE_G2_ADD = 32, CURVE_G2_ADD_MIXED = 33, CURVE_G2_DOUBLE = 34, CURVE_G2_IN_SUBGROUP = 35, CURVE_G2_PSI = 36,
     CURVE_G2_CLEAR_COFACTOR = 37, CURVE_G2_SSWU_ISO = 38, CURVE_G2_H2C_FINISH = 39,
     CURVE_G2_END = 40                                                // bls_g2.cu: the signature / hash kernels' build

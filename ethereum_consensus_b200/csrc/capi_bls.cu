@@ -1051,7 +1051,8 @@ int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* 
     int32_t rc = check_ready(e);
     if (rc) return rc;
     const bool fp2 = op >= FP2_EVAL_MUL && op < FP2_EVAL_END;
-    if (!(fp2 || (op >= 0 && op < FP_EVAL_N_OPS) || (op >= FPL_EVAL_SQRT_CHAIN && op < FPL_EVAL_END)) || n > (1u << 24))
+    if (!(fp2 || (op >= 0 && op < FP_EVAL_N_OPS) || (op >= FPL_EVAL_SQRT_CHAIN && op < FPL_EVAL_END) ||
+          (op >= FPD_EVAL_MUL && op < FPD_EVAL_END)) || n > (1u << 24))
         return B200_ERR_BAD_ARG;
     if (n == 0) return B200_SUCCESS;
     if (!a || !b || !out) return B200_ERR_BAD_ARG;
@@ -1080,7 +1081,8 @@ int32_t b200_curve_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_
     int32_t rc = check_ready(e);
     if (rc) return rc;
     const bool g2 = op >= CURVE_G2_ADD && op < CURVE_G2_END;
-    if (!(g2 || (op >= 0 && op < CURVE_G1_N_OPS) || op == CURVE_G1L_DOUBLE) || n > (1u << 24)) return B200_ERR_BAD_ARG;
+    if (!(g2 || (op >= 0 && op < CURVE_G1_N_OPS) || op == CURVE_G1L_DOUBLE || op == CURVE_G1_IN_SUBGROUP_ISO) || n > (1u << 24))
+        return B200_ERR_BAD_ARG;
     if (n == 0) return B200_SUCCESS;
     if (!a || !b || !out) return B200_ERR_BAD_ARG;
     const size_t bytes = size_t(n) * kCurveEvalWords * 4;

@@ -447,11 +447,15 @@ B200_API int32_t b200_vm_load_programs(const uint32_t* blob, size_t n_words);
 /* On-device self-test of the field arithmetic over `n` pseudo-random triples; *mismatches must come back 0. */
 B200_API int32_t b200_fp_selftest(uint32_t n, uint32_t seed, uint32_t* mismatches);
 /* On-device self-test of single field operations, for comparison with big integers: `op` (bls_kernels.cuh, FP_EVAL_* /
- * FP2_EVAL_*) is applied to `n` operand pairs.  a, b: n x 24 raw little-endian 32-bit limbs (Fp in the first 12, Fp2 as
- * c0 then c1); out: n x 25 (the result's limbs, then a carry / borrow / square / sign flag).  Test use only. */
+ * FP2_EVAL_* / FPD_EVAL_*) is applied to `n` operand pairs.  a, b: n x 24 raw little-endian 32-bit limbs (Fp in the first
+ * 12, Fp2 as c0 then c1); out: n x 25 (the result's limbs, then a carry / borrow / square / on-curve / sign flag).  An
+ * FpD value (the FP64 field of the per-key kernel's square root) is words 0..15 of a slot: 8 little-endian IEEE binary64
+ * limbs, limb k an integer multiple of 2^(48k), so that a record read as float64[n, 12] holds them in columns 0..7.
+ * Test use only. */
 B200_API int32_t b200_fp_eval(int32_t op, uint32_t n, const uint32_t* a, const uint32_t* b, uint32_t* out);
 /* On-device self-test of single curve stages, for comparison with a big-integer oracle: `op` (bls_kernels.cuh,
- * CURVE_G1L_* on the per-key kernel's lazily reduced field, CURVE_G2_* in the signature / hash unit) is applied to `n`
+ * CURVE_G1L_* on the per-key kernel's lazily reduced field, CURVE_G1_IN_SUBGROUP_ISO on X alone as the role-split per-key
+ * kernel checks it, CURVE_G2_* in the signature / hash unit) is applied to `n`
  * operand pairs.  a, b, out: n x 73 words: X, Y, Z as 24-word slots of raw little-endian 32-bit Montgomery limbs (Fp in
  * the first 12 words of a slot, Fp2 as c0 then c1), then a flag word (in: the affine infinity flag; out: the subgroup
  * verdict, or the infinity flag of an affine result).  Test use only. */

@@ -1,6 +1,9 @@
 // Host build of the FP64 field (fpd.cuh) and of the per-key kernel's split validation (groups.cuh), for
-// tests/test_fpd.py.  std::fma is the same IEEE binary64 fused operation as the device's DFMA, so these are the device's
-// bits.
+// tests/test_fpd.py and tests/test_fpd_device_gpu.py.  std::fma is the same IEEE binary64 fused operation as the
+// device's DFMA, and every other rounding in fpd.cuh is exact or spelled out, so these are meant to be the device's bits:
+// test_fpd_device_gpu.py compares products, squares, sums, the conversions and the square-root chain with the device
+// build limb for limb, and test_fpd.py checks that a build which contracts freely (-mfma -ffp-contract=fast) gives the
+// same bits as this one.
 #include <cstddef>
 #include <cstdint>
 

@@ -6,8 +6,9 @@ register caps), and the per-tuple G1 sum, the G2 sum and the two-launch hash_to_
 case goes through the kernels and its code (and, where there is one, its output bytes) is compared with the oracle's.
 
 Sections: a. key validation, b. signature decode + subgroup check, c. hash_to_G2 by verdict, d. equal / opposite points
-meeting in the aggregation lanes and trees, e. whole tuples (plain, chunked, RLC).  B200_G1_VARIANT and B200_PAIRING_VM are
-read once per process, so sections a, d and e run again in one child process per setting.
+meeting in the aggregation lanes and trees, e. whole tuples (plain, chunked, RLC).  B200_G1_VARIANT, B200_PAIRING_VM and
+B200_G1_SMALL_N are read once per process, so sections a, d and e run again in one child process per setting; with
+B200_G1_SMALL_N=0 every key of those sections goes through the role-split per-key kernel, not only the tiled loads.
 
     B200_SOAK_SCALE=1 (default) python -m pytest tests/test_bls_device_soak_gpu.py -m gpu -s
 """
@@ -35,8 +36,15 @@ pytestmark = pytest.mark.gpu
 SCALE = float(os.environ.get("B200_SOAK_SCALE", "1"))
 SMALL_N = 3 * 148 * 384          # bls_g1.cu g_g1_small_n: up to here the per-key kernel goes out as 128-thread CTAs
 RLC_SEED = hashlib.sha256(b"device soak rlc").digest()
+# the last: every per-key launch through the role-split kernel (k_g1_validate_split), whatever its size
 ENV_VARIANTS = [{"B200_G1_VARIANT": "0", "B200_PAIRING_VM": "1"}, {"B200_G1_VARIANT": "6", "B200_PAIRING_VM": "1"},
-                {"B200_G1_VARIANT": "7", "B200_PAIRING_VM": "0"}]
+                {"B200_G1_VARIANT": "7", "B200_PAIRING_VM": "0"},
+                {"B200_G1_VARIANT": "7", "B200_PAIRING_VM": "1", "B200_G1_SMALL_N": "0"}]
+
+
+def _env_id(e):
+    small = "-small_n_%s" % e["B200_G1_SMALL_N"] if "B200_G1_SMALL_N" in e else ""
+    return "g1_variant_%s-vm_%s%s" % (e["B200_G1_VARIANT"], e["B200_PAIRING_VM"], small)
 
 
 def _n(x):
@@ -449,7 +457,7 @@ def test_e_whole_tuples(engine, oracle_bls_c):
     assert len(set(D["want"])) >= 4
 
 
-@pytest.mark.parametrize("env", ENV_VARIANTS, ids=lambda e: "g1_variant_%s-vm_%s" % (e["B200_G1_VARIANT"], e["B200_PAIRING_VM"]))
+@pytest.mark.parametrize("env", ENV_VARIANTS, ids=_env_id)
 def test_env_variants_in_child_processes(oracle_bls_c, tmp_path, env):
     """Sections a, d and e under a per-key kernel variant / the one-thread-per-pair pairing kernels, which only the
     environment selects (read once per process): one child process per setting, inputs and oracle verdicts from here."""
@@ -476,7 +484,8 @@ def _child(path):
     _lib.init(0)
     data = pickle.loads(Path(path).read_bytes())
     rlc = os.environ.get("B200_PAIRING_VM", "1") != "0"     # the RLC entry points refuse the one-thread-per-pair kernels
-    tag = " [G1 %s, VM %s]" % (os.environ.get("B200_G1_VARIANT", "7"), os.environ.get("B200_PAIRING_VM", "1"))
+    tag = " [G1 %s, VM %s, small n %s]" % (os.environ.get("B200_G1_VARIANT", "7"), os.environ.get("B200_PAIRING_VM", "1"),
+                                          os.environ.get("B200_G1_SMALL_N", "default"))
     res = check_keys(data["keys"], tag) + check_shapes(data["shapes"], rlc, tag) + check_tuples(data["tuples"], rlc, tag)
     _assert_clean(res)
     print("CHILD_OK")

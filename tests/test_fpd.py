@@ -24,12 +24,12 @@ MASK32 = (1 << 32) - 1
 B47 = 1 << 47
 
 
-@pytest.fixture(scope="module")
-def host(tmp_path_factory):
+def build_host(out_dir, flags=("-O2", "-ffp-contract=off")):
+    """tests/host_math/fpd_host.cpp as a shared library, compiled with `flags`, loaded with its argument types."""
     src = ROOT / "tests" / "host_math" / "fpd_host.cpp"
-    lib = tmp_path_factory.mktemp("fpd") / "libfpd_host.so"
-    subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-fvisibility=hidden", "-ffp-contract=off",
-                    "-o", str(lib), str(src)], check=True)
+    lib = Path(out_dir) / "libfpd_host.so"
+    subprocess.run(["g++", *flags, "-std=c++17", "-fPIC", "-shared", "-fvisibility=hidden", "-o", str(lib), str(src)],
+                   check=True)
     L = ctypes.CDLL(str(lib))
     L.hm_fpd_op.argtypes = [ctypes.c_int, ctypes.c_uint32] + [ctypes.c_void_p] * 3
     L.hm_fpd_roundtrip.argtypes = [ctypes.c_uint32] + [ctypes.c_void_p] * 3
@@ -37,6 +37,21 @@ def host(tmp_path_factory):
     L.hm_key_validate_split.argtypes = [ctypes.c_uint32] + [ctypes.c_void_p] * 5
     L.hm_subgroup_iso.argtypes = [ctypes.c_void_p] * 4
     return L
+
+
+@pytest.fixture(scope="module")
+def host(tmp_path_factory):
+    return build_host(tmp_path_factory.mktemp("fpd"))
+
+
+def _cpu_has_fma():
+    """x86-64 with FMA3 (the -mfma build's instructions)"""
+    try:
+        lines = Path("/proc/cpuinfo").read_text().splitlines()
+    except OSError:
+        return False
+    flags = next((ln.split(":", 1)[1].split() for ln in lines if ln.startswith("flags")), [])
+    return "fma" in flags
 
 
 def _limbs(values):
@@ -145,6 +160,29 @@ def test_fpd_sqrt_chain_matches_fpl_chain(host):
     assert [v % P for v in d] == [v % P for v in l]
     squares = sum(pow(x * RINV % P, (P - 1) // 2, P) == 1 for x in xs)
     assert 50 < squares < len(xs) - 50     # both squares and non-squares
+
+
+def test_fpd_bits_do_not_depend_on_contraction(host, tmp_path):
+    """The device compiler contracts a * b + c into one FMA wherever it may (nvcc's default --fmad=true).  FpD's exactness
+    argument makes every rounding either exact or one it spells out with fpd_fma, so the bits must not change when the
+    host compiler contracts freely: -O3 -mfma -ffp-contract=fast against the -ffp-contract=off build, bit for bit."""
+    if not _cpu_has_fma():
+        pytest.skip("the CPU has no FMA instructions")
+    fast = build_host(tmp_path, ("-O3", "-mfma", "-ffp-contract=fast"))
+    da = _operands()
+    db = da[1:] + da[:1]
+    for op in (0, 1, 2):
+        off, fst = _run(host, op, da, db), _run(fast, op, da, db)
+        assert np.array_equal(off.view(np.uint64), fst.view(np.uint64)), op
+    rnd = random.Random(16)
+    xs = [0, 1, P - 1, P, 2 * P - 1] + [rnd.randrange(2 * P) for _ in range(300)]
+    a = _limbs(xs)
+    outs = []
+    for L in (host, fast):
+        d, l = np.zeros_like(a), np.zeros_like(a)
+        L.hm_fpd_sqrt_chain(len(xs), a.ctypes.data, d.ctypes.data, l.ctypes.data)
+        outs.append(d)
+    assert np.array_equal(outs[0], outs[1])
 
 
 def _torsion_cases():

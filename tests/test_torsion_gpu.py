@@ -6,8 +6,8 @@ in the per-key kernel those branches run on lazily reduced FpL, where "zero" may
 a. keys through every key entry point, b. signatures through aggregate and K = 1 tuples, c. one torsion-laden key or
 signature in an otherwise valid RLC batch, d. single curve stages through b200_curve_eval (subgroup checks without a
 decode in front, psi, cofactor clearing, the map, hash_to_G2's second half, and the FpL / Fp2 additions on their
-exceptional operands).  B200_G1_VARIANT is read once per process, so section a runs again in one child process per
-variant.
+exceptional operands).  B200_G1_VARIANT and B200_G1_SMALL_N are read once per process, so section a runs again in one
+child process per variant, and once with every per-key launch through the role-split kernel.
 
     B200_SOAK_SCALE=1 (default) python -m pytest tests/test_torsion_gpu.py -m gpu -s
 """
@@ -401,14 +401,19 @@ def test_curve_eval_rejects_unknown_ops(engine):
 
 
 # ---------------------------------------------------------------------------------------------------------- variants
-@pytest.mark.parametrize("variant", ["0", "6"])
+CHILD_ENVS = {"0": {"B200_G1_VARIANT": "0"}, "6": {"B200_G1_VARIANT": "6"},
+              "7-small_n_0": {"B200_G1_VARIANT": "7", "B200_G1_SMALL_N": "0"}}
+
+
+@pytest.mark.parametrize("variant", list(CHILD_ENVS))
 def test_a_keys_per_g1_variant_in_child_processes(oracle_bls_c, tmp_path, variant):
-    """Section a under the 256-thread / 224-register and 512-thread / 128-register per-key kernels, which only the
-    environment selects (read once per process)."""
+    """Section a under the 256-thread / 224-register and 512-thread / 128-register per-key kernels, and with every
+    launch of the default through the role-split kernel (B200_G1_SMALL_N=0), which only the environment selects (read
+    once per process)."""
     t = time.time()
     path = tmp_path / "keys.pkl"
     path.write_bytes(pickle.dumps(_keys_section(data(oracle_bls_c))))
-    env = dict(os.environ, B200_G1_VARIANT=variant)
+    env = dict(os.environ, **CHILD_ENVS[variant])
     p = subprocess.Popen([sys.executable, "-m", "tests.test_torsion_gpu", str(path)], cwd=str(ROOT), env=env,
                          stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     try:
@@ -417,7 +422,7 @@ def test_a_keys_per_g1_variant_in_child_processes(oracle_bls_c, tmp_path, varian
         p.kill()
         out = p.communicate()[0]
     print(out)
-    print(f"child B200_G1_VARIANT={variant} wall {time.time() - t:.1f} s")
+    print(f"child {CHILD_ENVS[variant]} wall {time.time() - t:.1f} s")
     assert p.returncode == 0, out
     assert "CHILD_OK" in out, out
 
@@ -426,7 +431,8 @@ def _child(path):
     from ethereum_consensus_b200 import _lib
     _lib.init(0)
     K = pickle.loads(Path(path).read_bytes())
-    _assert_clean(check_keys(K, " [G1 %s]" % os.environ.get("B200_G1_VARIANT", "7")))
+    _assert_clean(check_keys(K, " [G1 %s, small n %s]" % (os.environ.get("B200_G1_VARIANT", "7"),
+                                                           os.environ.get("B200_G1_SMALL_N", "default"))))
     print("CHILD_OK")
 
 
