@@ -802,7 +802,7 @@ static int32_t registry_fill(Engine& e, BlsState& s, size_t at, const uint8_t* h
 // the registry calls on a resident state: its Validator records in HBM and their count
 static int32_t registry_state_records(Engine& e, b200_state* h, const uint8_t** records, uint64_t* n) {
     if (state_validator_records(h, records, n)) {
-        e.last_error = "registry: the state handle is NULL, not uploaded or sharded";
+        e.last_error = "registry: the state handle is NULL or sharded";
         return B200_ERR_BAD_ARG;
     }
     if (*n > 0x7fffffffu) { e.last_error = "registry: more validators than the registry holds"; return B200_ERR_BAD_ARG; }

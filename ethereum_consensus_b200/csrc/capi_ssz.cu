@@ -59,7 +59,6 @@ struct b200_state {
     SszPlan plan;
     std::vector<uint32_t> outputs;
     DevBuf arena, fields, planbuf, selbuf, scatter;
-    bool uploaded = false;
     // ---- incremental re-hash (b200_state_update_* / b200_state_root_incremental) ----
     // Host shadow of the serialization with everything EXCEPT the five big lists filled in (their byte ranges are never
     // written or read: untouched zero pages of an anonymous mapping): small-field updates patch it and the plan is
@@ -88,25 +87,28 @@ struct b200_state {
 };
 
 namespace {
-constexpr int kBigVar[5] = {2, 3, 4, 5, 6};         // StateOffsets::var index of each big list
-constexpr uint32_t kBigElem[5] = {121, 8, 1, 1, 8};  // element size in bytes
-// first-job input covering element i of big list f: a Validator record, or the 32-byte chunk of a packed list
-inline uint32_t big_input_of(int f, uint64_t i) { return uint32_t(f == 0 ? i : (i * kBigElem[f]) / 32); }
-inline uint64_t big_count(const b200_state* h, int f) {
-    return uint64_t(h->so.var[kBigVar[f] + 1] - h->so.var[kBigVar[f]]) / kBigElem[f];
+// a single-GPU resident state: the calls that update, read or compute duties on a state take only these
+bool resident(const b200_state* h) { return h && !h->sharded; }
+// chain c of the handle's plan (ssz_plan.h: StateChain)
+StateChain chain(const b200_state* h, int c) { return state_chain(h->so, preset_of(h->preset), c); }
+// Device address of chain c's bytes on a resident handle.  Its plan stages all nine chains, and a big list's region is
+// reserved for its capacity even while the list is empty.
+uint8_t* chain_dev(const b200_state* h, int c) {
+    uint64_t field_off = 0; size_t nbytes = 0;
+    h->plan.chain_field(c, &field_off, &nbytes);
+    return static_cast<uint8_t*>(h->fields.p) + field_off;
 }
 // Elements reserved beyond a big list's length when its device regions are (re)allocated: 2^16 (one 8 MB slab of
 // Validator records) or a sixteenth of the list, whichever is larger.  Deposits then append in place for many blocks;
 // crossing the capacity relocates the list on the device.
 inline uint64_t headroom(uint64_t n) { return std::max<uint64_t>(uint64_t(1) << 16, n / 16); }
 constexpr size_t kShadowSlack = 64 << 10;   // shadow bytes beyond the reserved lists: header / summaries growth
-constexpr uint64_t kRegistryLimit = uint64_t(1) << 40;   // VALIDATOR_REGISTRY_LIMIT (both presets)
 
 size_t shadow_bytes_for(const b200_state* h) {
     size_t b = h->len + kShadowSlack;
-    for (int f = 0; f < 5; f++) b += size_t(h->cap[f] - big_count(h, f)) * kBigElem[f];
-    const size_t votes = h->so.var[2] - h->so.var[1];
-    return b + size_t(eth1_data_votes_bound(h->preset) * 72) - votes;
+    for (int f = 0; f < 5; f++) b += size_t(h->cap[f] - chain(h, f).len) * chain(h, f).elem;
+    const SmallList votes = appendable_small_list(B200_FIELD_ETH1_DATA_VOTES, preset_of(h->preset));
+    return b + size_t(votes.limit * votes.elem) - (h->so.var[2] - h->so.var[1]);
 }
 
 // Page-lock the head of the shadow up to eth1_data_votes (the fixed part and historical_roots: it never changes size),
@@ -165,6 +167,36 @@ void mark_all_small(b200_state* h) {
     h->small_dirty = true;
     h->small_ranges.emplace_back(h->shadow, h->shadow + h->so.var[2]);
     h->small_ranges.emplace_back(h->shadow + h->so.var[7], h->shadow + h->len);
+}
+
+// after a root: every dirty path, full re-hash and patched small field is in it
+void mark_clean(b200_state* h) {
+    for (auto& d : h->dirty) d.clear();
+    std::fill(h->rehash.begin(), h->rehash.end(), 0);
+    h->small_dirty = false;
+    h->small_ranges.clear();
+}
+
+// [lo, hi) of the serialization in the places that hold it: pieces of the host shadow (chain -1: everything outside the
+// five big lists, [0, var[2]) and [var[7], len)), then pieces of chains in HBM, `at` bytes into the chain.  The four big
+// vectors (chains 5..8) are held in both places.
+struct Piece {
+    int chain;
+    uint64_t x, y, at;
+};
+std::vector<Piece> split_range(const b200_state* h, uint64_t lo, uint64_t hi) {
+    std::vector<Piece> out;
+    auto add = [&](int c, uint64_t a, uint64_t b) {
+        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
+        if (x < y) out.push_back(Piece{c, x, y, x - a});
+    };
+    add(-1, 0, h->so.var[2]);
+    add(-1, h->so.var[7], h->len);
+    for (int c = 0; c < 9; c++) {
+        const StateChain L = chain(h, c);
+        add(c, L.lo, L.hi);
+    }
+    return out;
 }
 
 // grow a device buffer keeping its contents
@@ -238,13 +270,9 @@ int32_t adopt_plan(Engine& e, b200_state* h, SszPlan& np, std::vector<uint32_t>&
 
 // the registry's view of a resident state (capi_bls.cu: b200_registry_load_state / b200_registry_sync_state)
 int32_t b200::state_validator_records(const b200_state* h, const uint8_t** records, uint64_t* n) {
-    if (!h || !h->uploaded || h->sharded) return B200_ERR_BAD_ARG;
-    *records = nullptr;
-    *n = big_count(h, 0);
-    if (*n == 0) return B200_SUCCESS;
-    uint64_t field_off = 0; size_t nbytes = 0;
-    if (!h->plan.chain_field(0, &field_off, &nbytes)) return B200_ERR_BAD_ARG;
-    *records = static_cast<const uint8_t*>(h->fields.p) + field_off;
+    if (!resident(h)) return B200_ERR_BAD_ARG;
+    *n = chain(h, 0).len;
+    *records = *n ? chain_dev(h, 0) : nullptr;
     return B200_SUCCESS;
 }
 
@@ -418,7 +446,7 @@ int32_t b200_state_upload_deneb(const uint8_t* ssz, size_t len, int32_t preset, 
     std::unique_ptr<b200_state> h(new b200_state());
     if (!parse_beacon_state(ssz, len, preset, h->so)) { e.last_error = "malformed deneb BeaconState SSZ"; return B200_ERR_SSZ_MALFORMED; }
     h->len = len; h->preset = preset;
-    for (int f = 0; f < 5; f++) h->cap[f] = big_count(h.get(), f) + headroom(big_count(h.get(), f));
+    for (int f = 0; f < 5; f++) h->cap[f] = chain(h.get(), f).len + headroom(chain(h.get(), f).len);
     {
         SszPlan first;  // reads the caller's buffer
         std::vector<uint32_t> outs;
@@ -438,7 +466,6 @@ int32_t b200_state_upload_deneb(const uint8_t* ssz, size_t len, int32_t preset, 
     pin_shadow(h.get(), true);
     rc = build_beacon_state_plan(h->plan, h->shadow, len, preset, h->outputs, h->cap);  // same layout: lengths and caps
     if (rc) return rc;
-    h->uploaded = true;
     *out_handle = h.release();
     return B200_SUCCESS;
 }
@@ -459,7 +486,7 @@ int32_t b200_state_root(b200_state* h, uint8_t out[32]) {
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!h || !h->uploaded || !out) return B200_ERR_BAD_ARG;
+    if (!h || !out) return B200_ERR_BAD_ARG;
     if (h->sharded)   // every rank of the communicator calls this together: stages | ncclAllGather | finisher
         return h->plan.run(e, h->arena, h->fields, h->planbuf, COPY_NONE, h->outputs, out);
     rc = replan_if_small_dirty(e, h);  // updates made through b200_state_update_* are honoured here too
@@ -467,10 +494,7 @@ int32_t b200_state_root(b200_state* h, uint8_t out[32]) {
     rc = h->plan.run(e, h->arena, h->fields, h->planbuf, h->small_dirty ? COPY_SMALL_ONLY : COPY_NONE, h->outputs, out,
                      nullptr, nullptr, &h->small_ranges);
     if (rc) return rc;
-    for (auto& d : h->dirty) d.clear();  // a full re-hash covers every dirty path
-    std::fill(h->rehash.begin(), h->rehash.end(), 0);
-    h->small_dirty = false;
-    h->small_ranges.clear();
+    mark_clean(h);
     return B200_SUCCESS;
 }
 
@@ -487,14 +511,12 @@ int32_t b200_state_update_elements(b200_state* h, int32_t field, const uint64_t*
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!h || !h->uploaded || h->sharded || field < 0 || field > 4 || (n && (!indices || !values)) || n > 0xffffffffull) return B200_ERR_BAD_ARG;
+    if (!resident(h) || field < 0 || field > 4 || (n && (!indices || !values)) || n > 0xffffffffull) return B200_ERR_BAD_ARG;
     if (!n) return B200_SUCCESS;
-    const uint64_t count = big_count(h, field);
+    const StateChain L = chain(h, field);
     for (size_t i = 0; i < n; i++)
-        if (indices[i] >= count) { e.last_error = "state_update_elements: index beyond the list length"; return B200_ERR_BAD_ARG; }
-    uint64_t field_off = 0; size_t nbytes = 0;
-    if (!h->plan.chain_field(field, &field_off, &nbytes)) return B200_ERR_BAD_ARG;
-    const uint32_t elem = kBigElem[field];
+        if (indices[i] >= L.len) { e.last_error = "state_update_elements: index beyond the list length"; return B200_ERR_BAD_ARG; }
+    const uint32_t elem = L.elem;
     // [indices | values] through pinned staging, then a scatter kernel into the resident list
     const size_t off_vals = n * 8;
     const size_t total = off_vals + n * elem;
@@ -503,12 +525,12 @@ int32_t b200_state_update_elements(b200_state* h, int32_t field, const uint64_t*
     memcpy(e.staging.p, indices, n * 8);
     memcpy(static_cast<uint8_t*>(e.staging.p) + off_vals, values, n * elem);
     B200_CUDA_TRY(cudaMemcpyAsync(h->scatter.p, e.staging.p, total, cudaMemcpyHostToDevice, e.stream));
-    launch_scatter(static_cast<uint8_t*>(h->fields.p) + field_off, static_cast<const uint64_t*>(h->scatter.p),
+    launch_scatter(chain_dev(h, field), static_cast<const uint64_t*>(h->scatter.p),
                    static_cast<const uint8_t*>(h->scatter.p) + off_vals, uint32_t(n), elem, e.stream);
     e.launches++;
     B200_CUDA_TRY(cudaGetLastError());
     B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
-    for (size_t i = 0; i < n; i++) h->dirty[field].push_back(big_input_of(field, indices[i]));
+    for (size_t i = 0; i < n; i++) h->dirty[field].push_back(L.input_of(indices[i]));
     return B200_SUCCESS;
 }
 
@@ -524,77 +546,63 @@ int32_t b200_state_update_bytes(b200_state* h, uint64_t ssz_offset, const uint8_
 
 // b200_state_update_bytes with the engine lock held (the sync-committee rotation writes through it too)
 static int32_t update_bytes(Engine& e, b200_state* h, uint64_t ssz_offset, const uint8_t* data, size_t n) {
-    if (!h || !h->uploaded || h->sharded || (n && !data) || ssz_offset > h->len || n > h->len - ssz_offset) return B200_ERR_BAD_ARG;
+    if (!resident(h) || (n && !data) || ssz_offset > h->len || n > h->len - ssz_offset) return B200_ERR_BAD_ARG;
     if (!n) return B200_SUCCESS;
-    const uint64_t lo = ssz_offset, hi = ssz_offset + n;
-    // (1) the parts outside the big lists: patch the shadow; the variable-size offsets must not change
+    const uint64_t lo = ssz_offset;
+    const std::vector<Piece> pieces = split_range(h, lo, lo + n);
+    // (1) the shadow's pieces: patch them; the variable-size offsets must not change
     std::vector<uint8_t> saved;
-    auto patch_small = [&](uint64_t a, uint64_t b) {  // [a, b) is a small region of the serialization
-        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
-        if (x >= y) return;
-        saved.insert(saved.end(), h->shadow + x, h->shadow + y);
-        memcpy(h->shadow + x, data + (x - lo), y - x);
-        h->small_ranges.emplace_back(h->shadow + x, h->shadow + y);
-    };
-    auto restore_small = [&](uint64_t a, uint64_t b, size_t& pos) {
-        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
-        if (x >= y) return;
-        memcpy(h->shadow + x, saved.data() + pos, y - x);
-        pos += y - x;
-    };
-    patch_small(0, h->so.var[2]);
-    patch_small(h->so.var[7], h->len);
+    for (const Piece& p : pieces) {
+        if (p.chain >= 0) continue;
+        saved.insert(saved.end(), h->shadow + p.x, h->shadow + p.y);
+        memcpy(h->shadow + p.x, data + (p.x - lo), p.y - p.x);
+        h->small_ranges.emplace_back(h->shadow + p.x, h->shadow + p.y);
+    }
     if (!saved.empty()) {
         StateOffsets so2;
         bool ok = parse_beacon_state(h->shadow, h->len, h->preset, so2);
         for (int i = 0; ok && i < 10; i++) ok = so2.var[i] == h->so.var[i];
         if (!ok) {  // would move or resize a variable-size field: not an in-place update
             size_t pos = 0;
-            restore_small(0, h->so.var[2], pos);
-            restore_small(h->so.var[7], h->len, pos);
+            for (const Piece& p : pieces) {
+                if (p.chain >= 0) continue;
+                memcpy(h->shadow + p.x, saved.data() + pos, p.y - p.x);
+                pos += p.y - p.x;
+            }
             // (the ranges stay recorded: re-copying unchanged bytes is harmless)
             e.last_error = "state_update_bytes: the update changes a variable-size field's offset or length; use state_append_elements / state_set_field";
             return B200_ERR_BAD_ARG;
         }
         h->small_dirty = true;
     }
-    // (2) the parts inside big lists and inside the four big vectors (chains 5..8): copy into the resident field, mark the
-    //     covered inputs dirty
-    const uint64_t vec_lo[4] = {h->so.block_roots, h->so.state_roots, h->so.randao_mixes, h->so.slashings};
-    for (int f = 0; f < 9; f++) {
-        if (size_t(f) >= h->plan.n_chains()) break;
-        uint64_t field_off = 0; size_t nbytes = 0;
-        const bool staged = h->plan.chain_field(f, &field_off, &nbytes);
-        const uint64_t a = f < 5 ? h->so.var[kBigVar[f]] : vec_lo[f - 5];
-        const uint64_t b = f < 5 ? h->so.var[kBigVar[f] + 1] : a + nbytes;
-        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
-        if (x >= y) continue;
-        if (!staged) return B200_ERR_BAD_ARG;
-        B200_CUDA_TRY(e.staging.reserve(y - x));
-        memcpy(e.staging.p, data + (x - lo), y - x);
-        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(h->fields.p) + field_off + (x - a), e.staging.p, y - x,
-                                      cudaMemcpyHostToDevice, e.stream));
+    // (2) the pieces inside big lists and inside the four big vectors: copy into the resident chain, mark the covered
+    //     inputs dirty
+    for (const Piece& p : pieces) {
+        if (p.chain < 0) continue;
+        B200_CUDA_TRY(e.staging.reserve(p.y - p.x));
+        memcpy(e.staging.p, data + (p.x - lo), p.y - p.x);
+        B200_CUDA_TRY(cudaMemcpyAsync(chain_dev(h, p.chain) + p.at, e.staging.p, p.y - p.x, cudaMemcpyHostToDevice, e.stream));
         B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
-        const uint32_t unit = f == 0 ? 121u : 32u;
-        for (uint64_t u = (x - a) / unit; u <= (y - 1 - a) / unit; u++) h->dirty[f].push_back(uint32_t(u));
+        const uint32_t unit = chain(h, p.chain).unit;
+        for (uint64_t u = p.at / unit; u <= (p.at + (p.y - p.x) - 1) / unit; u++) h->dirty[p.chain].push_back(uint32_t(u));
     }
     return B200_SUCCESS;
 }
 
 // Field ids of the reshaping calls beyond the five big lists (include/b200_consensus.h)
-static constexpr int32_t kFieldVotes = B200_FIELD_ETH1_DATA_VOTES, kFieldSummaries = B200_FIELD_HISTORICAL_SUMMARIES,
-                         kFieldHeader = B200_FIELD_LATEST_EXECUTION_PAYLOAD_HEADER;
+static constexpr int32_t kFieldVotes = B200_FIELD_ETH1_DATA_VOTES, kFieldHeader = B200_FIELD_LATEST_EXECUTION_PAYLOAD_HEADER;
 
 // append to a big list: shadow offsets, then (past the capacity) relocation on the device, then the appended bytes H2D
 static int32_t append_big(Engine& e, b200_state* h, int f, const uint8_t* values, size_t n) {
-    const uint64_t old_n = big_count(h, f), new_n = old_n + n;
-    if (n > kRegistryLimit || new_n > kRegistryLimit) { e.last_error = "state_append_elements: beyond the list limit"; return B200_ERR_LIMIT; }
-    const uint32_t elem = kBigElem[f];
+    const StateChain L = chain(h, f);
+    const uint64_t old_n = L.len, new_n = old_n + n, limit = preset_of(h->preset).validator_registry_limit;
+    if (n > limit || new_n > limit) { e.last_error = "state_append_elements: beyond the list limit"; return B200_ERR_LIMIT; }
+    const uint32_t elem = L.elem;
     if (uint64_t(n) * elem > 0xffffffffull) { e.last_error = "state_append_elements: the serialization would exceed 4 GiB"; return B200_ERR_LIMIT; }
     const size_t old_bytes = size_t(old_n) * elem, new_bytes = size_t(new_n) * elem;
-    int32_t rc = reshape_shadow(e, h, kBigVar[f], new_bytes);
+    int32_t rc = reshape_shadow(e, h, L.var, new_bytes);
     if (rc) return rc;
-    auto undo = [&]() { reshape_shadow(e, h, kBigVar[f], old_bytes); reparse(h); };
+    auto undo = [&]() { reshape_shadow(e, h, L.var, old_bytes); reparse(h); };
     if (!reparse(h)) { undo(); return B200_ERR_SSZ_MALFORMED; }
     if (new_n > h->cap[f]) {   // relocate the list (and re-place the chains after it) with fresh headroom
         const uint64_t old_cap = h->cap[f];
@@ -605,15 +613,12 @@ static int32_t append_big(Engine& e, b200_state* h, int f, const uint8_t* values
         if (!rc) rc = adopt_plan(e, h, np, outs);
         if (rc) { h->cap[f] = old_cap; undo(); return rc; }
     }
-    uint64_t field_off = 0; size_t staged = 0;
-    if (!h->plan.chain_field(f, &field_off, &staged)) { undo(); return B200_ERR_BAD_ARG; }
     B200_CUDA_TRY(e.staging.reserve(n * elem));
     memcpy(e.staging.p, values, n * elem);
-    B200_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(h->fields.p) + field_off + old_bytes, e.staging.p, n * elem,
-                                  cudaMemcpyHostToDevice, e.stream));
+    B200_CUDA_TRY(cudaMemcpyAsync(chain_dev(h, f) + old_bytes, e.staging.p, n * elem, cudaMemcpyHostToDevice, e.stream));
     B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
     // appended inputs are dirty; the old ragged last chunk is among them when the first appended element shares it
-    for (uint64_t u = big_input_of(f, old_n); u <= big_input_of(f, new_n - 1); u++) h->dirty[f].push_back(uint32_t(u));
+    for (uint64_t u = L.input_of(old_n); u <= L.input_of(new_n - 1); u++) h->dirty[f].push_back(uint32_t(u));
     // new length mix-in and finisher ops; the finisher nodes of the lists' tops are allocated ahead of the small fields'
     // arena levels, so those move with them and are re-hashed
     mark_all_small(h);
@@ -642,19 +647,17 @@ int32_t b200_state_append_elements(b200_state* h, int32_t field, const uint8_t* 
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!h || !h->uploaded || h->sharded || (n && !values)) return B200_ERR_BAD_ARG;
+    if (!resident(h) || (n && !values)) return B200_ERR_BAD_ARG;
     if (field >= 0 && field <= 4) return n ? append_big(e, h, field, values, n) : B200_SUCCESS;
-    if (field != kFieldVotes && field != kFieldSummaries) { e.last_error = "state_append_elements: unknown field"; return B200_ERR_BAD_ARG; }
+    const SmallList l = appendable_small_list(field, preset_of(h->preset));
+    if (l.var < 0) { e.last_error = "state_append_elements: unknown field"; return B200_ERR_BAD_ARG; }
     if (!n) return B200_SUCCESS;
-    const int k = field == kFieldVotes ? 1 : 8;
-    const size_t elem = field == kFieldVotes ? 72 : 64;
-    const uint64_t limit = field == kFieldVotes ? eth1_data_votes_bound(h->preset) : historical_roots_limit(h->preset);
-    const size_t old_bytes = h->so.var[k + 1] - h->so.var[k];
-    if (n > limit || old_bytes / elem + n > limit) { e.last_error = "state_append_elements: beyond the list limit"; return B200_ERR_LIMIT; }
-    std::vector<uint8_t> buf(old_bytes + n * elem);
-    memcpy(buf.data(), h->shadow + h->so.var[k], old_bytes);
-    memcpy(buf.data() + old_bytes, values, n * elem);
-    return set_small(e, h, k, buf.data(), buf.size());
+    const size_t old_bytes = h->so.var[l.var + 1] - h->so.var[l.var];
+    if (n > l.limit || old_bytes / l.elem + n > l.limit) { e.last_error = "state_append_elements: beyond the list limit"; return B200_ERR_LIMIT; }
+    std::vector<uint8_t> buf(old_bytes + n * l.elem);
+    memcpy(buf.data(), h->shadow + h->so.var[l.var], old_bytes);
+    memcpy(buf.data() + old_bytes, values, n * l.elem);
+    return set_small(e, h, l.var, buf.data(), buf.size());
 }
 
 int32_t b200_state_set_field(b200_state* h, int32_t field, const uint8_t* ssz, size_t len) {
@@ -662,15 +665,16 @@ int32_t b200_state_set_field(b200_state* h, int32_t field, const uint8_t* ssz, s
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!h || !h->uploaded || h->sharded || (len && !ssz)) return B200_ERR_BAD_ARG;
+    if (!resident(h) || (len && !ssz)) return B200_ERR_BAD_ARG;
     if (field == kFieldVotes) {
-        if (len % 72) { e.last_error = "state_set_field: eth1_data_votes not a multiple of 72 bytes"; return B200_ERR_SSZ_MALFORMED; }
-        if (len / 72 > eth1_data_votes_bound(h->preset)) { e.last_error = "state_set_field: beyond ETH1_DATA_VOTES_BOUND"; return B200_ERR_LIMIT; }
-        return set_small(e, h, 1, ssz, len);
+        const SmallList votes = appendable_small_list(field, preset_of(h->preset));
+        if (len % votes.elem) { e.last_error = "state_set_field: eth1_data_votes not a multiple of 72 bytes"; return B200_ERR_SSZ_MALFORMED; }
+        if (len / votes.elem > votes.limit) { e.last_error = "state_set_field: beyond ETH1_DATA_VOTES_BOUND"; return B200_ERR_LIMIT; }
+        return set_small(e, h, votes.var, ssz, len);
     }
     if (field == kFieldHeader) {
         // 584 fixed bytes whose only offset (extra_data, at byte 436) is 584, then 0..32 bytes of extra_data
-        if (len < 584 || len > 584 + 32 || (uint32_t(ssz[436]) | uint32_t(ssz[437]) << 8 | uint32_t(ssz[438]) << 16 | uint32_t(ssz[439]) << 24) != 584) {
+        if (len < 584 || len > 584 + 32 || le32(ssz + 436) != 584) {
             e.last_error = "state_set_field: malformed ExecutionPayloadHeader";
             return B200_ERR_SSZ_MALFORMED;
         }
@@ -685,7 +689,7 @@ int32_t b200_state_root_incremental(b200_state* h, uint8_t out[32]) {
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!h || !h->uploaded || !out) return B200_ERR_BAD_ARG;
+    if (!h || !out) return B200_ERR_BAD_ARG;
     rc = replan_if_small_dirty(e, h);
     if (rc) return rc;
     std::vector<std::vector<uint32_t>> dirty(h->plan.n_chains());
@@ -697,10 +701,7 @@ int32_t b200_state_root_incremental(b200_state* h, uint8_t out[32]) {
     rc = h->plan.run(e, h->arena, h->fields, h->planbuf, h->small_dirty ? COPY_SMALL_ONLY : COPY_NONE, h->outputs, out,
                      &dirty, &h->selbuf, &h->small_ranges, &h->rehash);
     if (rc) return rc;
-    for (auto& d : h->dirty) d.clear();
-    std::fill(h->rehash.begin(), h->rehash.end(), 0);
-    h->small_dirty = false;
-    h->small_ranges.clear();
+    mark_clean(h);
     return B200_SUCCESS;
 }
 
@@ -740,19 +741,17 @@ int32_t b200_state_shuffled_active_indices(b200_state* h, uint64_t epoch, const 
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!h || !h->uploaded || h->sharded || !seed || !out_n) return B200_ERR_BAD_ARG;
+    if (!resident(h) || !seed || !out_n) return B200_ERR_BAD_ARG;
     *out_n = 0;
-    const uint64_t n = big_count(h, 0);
+    const uint64_t n = chain(h, 0).len;
     if (n == 0) return B200_SUCCESS;
     if (!out) return B200_ERR_BAD_ARG;
-    uint64_t field_off = 0; size_t nbytes = 0;
-    if (!h->plan.chain_field(0, &field_off, &nbytes)) return B200_ERR_BAD_ARG;
     uint64_t *d_act, *d_out;
     rc = shuffle_scratch(e, n, &d_act, &d_out);
     if (rc) return rc;
     B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
     uint64_t cnt = 0;
-    rc = active_indices_on_device(e, static_cast<const uint8_t*>(h->fields.p) + field_off, n, epoch, d_act, &cnt);
+    rc = active_indices_on_device(e, chain_dev(h, 0), n, epoch, d_act, &cnt);
     if (rc) return rc;
     rc = shuffle_on_device(e, d_act, cnt, seed, rounds, d_out);
     if (rc) return rc;
@@ -766,59 +765,10 @@ int32_t b200_state_shuffled_active_indices(b200_state* h, uint64_t epoch, const 
 
 // ---- duties on a resident state: proposer lookahead and sync committees (deneb/spec/mod.rs) ----
 namespace {
-struct DutyPreset {
-    uint64_t slots_per_epoch, epochs_per_historical_vector, epochs_per_sync_committee_period;
-    uint32_t shuffle_round_count, sync_committee_size;
-    // process_epoch
-    uint64_t slots_per_historical_root, epochs_per_slashings_vector, epochs_per_eth1_voting_period;
-    uint64_t min_per_epoch_churn_limit, max_per_epoch_activation_churn_limit, churn_limit_quotient;
-    uint64_t effective_balance_increment, max_effective_balance, ejection_balance;
-    uint64_t hysteresis_quotient, hysteresis_downward_multiplier, hysteresis_upward_multiplier;
-    uint64_t inactivity_score_bias, inactivity_score_recovery_rate, inactivity_penalty_quotient_bellatrix;
-    uint64_t proportional_slashing_multiplier_bellatrix, base_reward_factor, min_epochs_to_inactivity_penalty;
-    uint64_t max_seed_lookahead, min_validator_withdrawability_delay;
-};
-// phase0/presets/{mainnet,minimal}.rs, altair/presets/{mainnet,minimal}.rs, bellatrix/presets/{mainnet,minimal}.rs,
-// configs/{mainnet,minimal}.rs
-DutyPreset duty_preset(int preset) {
-    const bool minimal = preset == B200_PRESET_MINIMAL;
-    DutyPreset P;
-    P.slots_per_epoch = minimal ? 8 : 32;
-    P.epochs_per_historical_vector = minimal ? 64 : 65536;
-    P.epochs_per_sync_committee_period = minimal ? 8 : 256;
-    P.shuffle_round_count = minimal ? 10 : 90;
-    P.sync_committee_size = minimal ? 32 : 512;
-    P.slots_per_historical_root = minimal ? 64 : 8192;
-    P.epochs_per_slashings_vector = minimal ? 64 : 8192;
-    P.epochs_per_eth1_voting_period = minimal ? 4 : 64;
-    P.min_per_epoch_churn_limit = minimal ? 2 : 4;
-    P.max_per_epoch_activation_churn_limit = minimal ? 4 : 8;
-    P.churn_limit_quotient = minimal ? 32 : 65536;
-    P.effective_balance_increment = 1000000000ull;
-    P.max_effective_balance = 32000000000ull;
-    P.ejection_balance = 16000000000ull;
-    P.hysteresis_quotient = 4;
-    P.hysteresis_downward_multiplier = 1;
-    P.hysteresis_upward_multiplier = 5;
-    P.inactivity_score_bias = 4;
-    P.inactivity_score_recovery_rate = 16;
-    P.inactivity_penalty_quotient_bellatrix = uint64_t(1) << 24;
-    P.proportional_slashing_multiplier_bellatrix = 3;
-    P.base_reward_factor = 64;
-    P.min_epochs_to_inactivity_penalty = 4;
-    P.max_seed_lookahead = 4;
-    P.min_validator_withdrawability_delay = 256;
-    return P;
-}
 constexpr uint8_t kDomainBeaconProposer[4] = {0, 0, 0, 0}, kDomainSyncCommittee[4] = {7, 0, 0, 0};   // domains.rs:19-30
 constexpr size_t kSlotOffset = 40;   // genesis_time (8), genesis_validators_root (32), then slot
 
-uint64_t shadow_slot(const b200_state* h) {
-    const uint8_t* p = h->shadow + kSlotOffset;
-    uint64_t v = 0;
-    for (int k = 7; k >= 0; k--) v = (v << 8) | p[k];
-    return v;
-}
+uint64_t shadow_slot(const b200_state* h) { return le64(h->shadow + kSlotOffset); }
 void sha256_host(const uint8_t* data, size_t len, uint8_t out[32]) {
     Sha256Ctx c;
     sha_init(c);
@@ -828,7 +778,7 @@ void sha256_host(const uint8_t* data, size_t len, uint8_t out[32]) {
 // get_seed (deneb/spec/mod.rs:2713-2748): SHA-256(domain || le64(epoch) || randao_mixes[(epoch + EPHV - 2) mod EPHV]),
 // the mix index in wrapping u64 (EPHV divides 2^64, so the wrap does not change it); the mixes are read from the shadow
 void state_seed(const b200_state* h, uint64_t epoch, const uint8_t domain[4], uint8_t out[32]) {
-    const DutyPreset P = duty_preset(h->preset);
+    const Preset& P = preset_of(h->preset);
     const uint64_t mix = (epoch + P.epochs_per_historical_vector - 2) % P.epochs_per_historical_vector;
     uint8_t in[44];
     memcpy(in, domain, 4);
@@ -836,17 +786,15 @@ void state_seed(const b200_state* h, uint64_t epoch, const uint8_t domain[4], ui
     memcpy(in + 12, h->shadow + h->so.randao_mixes + 32 * mix, 32);
     sha256_host(in, sizeof(in), out);
 }
-bool duty_handle_ok(const b200_state* h) { return h && h->uploaded && !h->sharded; }
 
 // get_active_validator_indices(state, epoch) into the shuffle scratch: *d_act (device) holds *n_active indices, *d_out
 // (device) has room for max(N, min_out) more; *recs: the Validator records in HBM.  No active validator (the reference's
 // CollectionCannotBeEmpty, or its `i % 0` panic for the sync committee) -> B200_ERR_BAD_ARG.
 int32_t duty_active(Engine& e, b200_state* h, uint64_t epoch, uint64_t min_out, const uint8_t** recs, uint64_t** d_act,
                     uint64_t** d_out, uint64_t* n_active) {
-    const uint64_t n = big_count(h, 0);
-    uint64_t field_off = 0; size_t nbytes = 0;
-    if (n == 0 || !h->plan.chain_field(0, &field_off, &nbytes)) { e.last_error = "duties: no active validator"; return B200_ERR_BAD_ARG; }
-    *recs = static_cast<const uint8_t*>(h->fields.p) + field_off;
+    const uint64_t n = chain(h, 0).len;
+    if (n == 0) { e.last_error = "duties: no active validator"; return B200_ERR_BAD_ARG; }
+    *recs = chain_dev(h, 0);
     int32_t rc = shuffle_scratch(e, std::max(n, min_out), d_act, d_out);
     if (rc) return rc;
     rc = active_indices_on_device(e, *recs, n, epoch, *d_act, n_active);
@@ -858,7 +806,7 @@ int32_t duty_active(Engine& e, b200_state* h, uint64_t epoch, uint64_t min_out, 
 // get_next_sync_committee (deneb/spec/mod.rs:1973-2060) with the engine lock held: indices (host, SIZE) and the SyncCommittee
 // bytes (host, SIZE x 48 keys then the 48-byte aggregate; zero on a non-zero *code)
 int32_t next_sync_committee(Engine& e, b200_state* h, uint64_t* out_indices, uint8_t* out_committee, int32_t* out_code) {
-    const DutyPreset P = duty_preset(h->preset);
+    const Preset& P = preset_of(h->preset);
     const uint64_t epoch = shadow_slot(h) / P.slots_per_epoch + 1;
     uint8_t seed[32];
     state_seed(h, epoch, kDomainSyncCommittee, seed);
@@ -881,7 +829,7 @@ int32_t next_sync_committee(Engine& e, b200_state* h, uint64_t* out_indices, uin
 }
 // process_sync_committee_updates with the engine lock held (b200_state_sync_committee_updates, b200_state_process_epoch)
 int32_t sync_committee_updates(Engine& e, b200_state* h, int32_t* rotated, int32_t* out_code) {
-    const DutyPreset P = duty_preset(h->preset);
+    const Preset& P = preset_of(h->preset);
     const uint64_t next_epoch = shadow_slot(h) / P.slots_per_epoch + 1;
     if (next_epoch % P.epochs_per_sync_committee_period != 0) {
         *rotated = 0; *out_code = B200_SUCCESS;
@@ -910,7 +858,7 @@ int32_t b200_state_get_seed(b200_state* h, uint64_t epoch, const uint8_t domain_
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || !domain_type || !out) return B200_ERR_BAD_ARG;
+    if (!resident(h) || !domain_type || !out) return B200_ERR_BAD_ARG;
     state_seed(h, epoch, domain_type, out);
     return B200_SUCCESS;
 }
@@ -920,8 +868,8 @@ int32_t b200_state_proposer_indices(b200_state* h, uint64_t epoch, uint64_t* out
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || !out) return B200_ERR_BAD_ARG;
-    const DutyPreset P = duty_preset(h->preset);
+    if (!resident(h) || !out) return B200_ERR_BAD_ARG;
+    const Preset& P = preset_of(h->preset);
     if (epoch > ~uint64_t(0) / P.slots_per_epoch) { e.last_error = "proposer_indices: epoch * SLOTS_PER_EPOCH overflows u64"; return B200_ERR_BAD_ARG; }
     // get_beacon_proposer_index (deneb/spec/mod.rs:2822-2856) for every slot of the epoch: seed SHA-256(get_seed(epoch,
     // BeaconProposer) || le64(slot)), the active set and the balances being those of the epoch
@@ -954,7 +902,7 @@ int32_t b200_state_next_sync_committee(b200_state* h, uint64_t* out_indices, uin
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || !out_indices || !out_committee || !out_code) return B200_ERR_BAD_ARG;
+    if (!resident(h) || !out_indices || !out_committee || !out_code) return B200_ERR_BAD_ARG;
     return next_sync_committee(e, h, out_indices, out_committee, out_code);
 }
 
@@ -963,7 +911,7 @@ int32_t b200_state_sync_committee_updates(b200_state* h, int32_t* rotated, int32
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || !rotated || !out_code) return B200_ERR_BAD_ARG;
+    if (!resident(h) || !rotated || !out_code) return B200_ERR_BAD_ARG;
     return sync_committee_updates(e, h, rotated, out_code);
 }
 
@@ -972,16 +920,14 @@ int32_t b200_state_sync_committee_indices(b200_state* h, int32_t which, uint64_t
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || !out || (which != 0 && which != 1)) return B200_ERR_BAD_ARG;
-    const DutyPreset P = duty_preset(h->preset);
+    if (!resident(h) || !out || (which != 0 && which != 1)) return B200_ERR_BAD_ARG;
+    const Preset& P = preset_of(h->preset);
     const uint8_t* keys = h->shadow + (which ? h->so.next_sync_committee : h->so.current_sync_committee);
-    const uint64_t n = big_count(h, 0);
-    uint64_t field_off = 0; size_t nbytes = 0;
-    const uint8_t* recs = nullptr;
-    if (n && h->plan.chain_field(0, &field_off, &nbytes)) recs = static_cast<const uint8_t*>(h->fields.p) + field_off;
+    const uint64_t n = chain(h, 0).len;
+    const uint8_t* recs = n ? chain_dev(h, 0) : nullptr;
     B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
     std::vector<uint64_t> res(P.sync_committee_size);
-    rc = match_committee_keys_on_device(e, recs, recs ? n : 0, keys, P.sync_committee_size, res.data());
+    rc = match_committee_keys_on_device(e, recs, n, keys, P.sync_committee_size, res.data());
     if (rc) return rc;
     B200_CUDA_TRY(cudaEventRecord(e.ev1, e.stream));
     B200_CUDA_TRY(cudaEventSynchronize(e.ev1));
@@ -992,11 +938,6 @@ int32_t b200_state_sync_committee_indices(b200_state* h, int32_t which, uint64_t
 
 // ---- process_epoch on a resident state (deneb/spec/mod.rs:965-1003) ----
 namespace {
-uint64_t le64(const uint8_t* p) {
-    uint64_t v = 0;
-    for (int k = 7; k >= 0; k--) v = (v << 8) | p[k];
-    return v;
-}
 // floor(sqrt(x)) exactly (u64::integer_sqrt): Newton's iteration on integers from above
 uint64_t integer_sqrt(uint64_t x) {
     if (x < 2) return x;
@@ -1005,7 +946,7 @@ uint64_t integer_sqrt(uint64_t x) {
     return uint64_t(r);
 }
 // get_block_root (:2552, :2582) from the shadow's block_roots; false where the reference returns SlotOutOfRange
-bool block_root(const b200_state* h, const DutyPreset& P, uint64_t slot, uint64_t epoch, const uint8_t** root) {
+bool block_root(const b200_state* h, const Preset& P, uint64_t slot, uint64_t epoch, const uint8_t** root) {
     const uint64_t at = epoch * P.slots_per_epoch;
     if (at >= slot || slot > at + P.slots_per_historical_root) return false;
     *root = h->shadow + h->so.block_roots + 32 * (at % P.slots_per_historical_root);
@@ -1020,18 +961,14 @@ int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_cod
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || !out_code || (steps & ~uint32_t(B200_EPOCH_ALL))) return B200_ERR_BAD_ARG;
+    if (!resident(h) || !out_code || (steps & ~uint32_t(B200_EPOCH_ALL))) return B200_ERR_BAD_ARG;
     *out_code = B200_SUCCESS;
-    const DutyPreset P = duty_preset(h->preset);
-    const uint64_t n = big_count(h, 0);
+    const Preset& P = preset_of(h->preset);
+    const uint64_t n = chain(h, 0).len;
     for (int f = 1; f < 5; f++)
-        if (big_count(h, f) != n) { e.last_error = "process_epoch: the five big lists differ in length"; return B200_ERR_BAD_ARG; }
+        if (chain(h, f).len != n) { e.last_error = "process_epoch: the five big lists differ in length"; return B200_ERR_BAD_ARG; }
     uint8_t* dev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // validators, balances, participation x 2, scores
-    for (int f = 0; f < 5 && n; f++) {
-        uint64_t off = 0; size_t nbytes = 0;
-        if (!h->plan.chain_field(f, &off, &nbytes)) return B200_ERR_BAD_ARG;
-        dev[f] = static_cast<uint8_t*>(h->fields.p) + off;
-    }
+    for (int f = 0; f < 5 && n; f++) dev[f] = chain_dev(h, f);
     const uint64_t slot = shadow_slot(h), cur = slot / P.slots_per_epoch, prev = cur ? cur - 1 : 0, next = cur + 1;
     const uint64_t inc = P.effective_balance_increment;
     B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
@@ -1119,7 +1056,7 @@ int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_cod
     p.withdraw_delay = P.min_validator_withdrawability_delay;
     if (run_sync && T.n_active_next == 0) { e.last_error = "process_epoch: no active validator for the next sync committee"; return B200_ERR_BAD_ARG; }
     const uint64_t n_summaries = (h->so.var[9] - h->so.var[8]) / 64;
-    if (run_summary && n_summaries + 1 > historical_roots_limit(h->preset)) {
+    if (run_summary && n_summaries + 1 > P.historical_roots_limit) {
         e.last_error = "process_epoch: historical_summaries is full";
         return B200_ERR_LIMIT;
     }
@@ -1202,7 +1139,7 @@ int32_t b200_state_serialized_len(b200_state* h, uint64_t* out_len) {
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || !out_len) return B200_ERR_BAD_ARG;
+    if (!resident(h) || !out_len) return B200_ERR_BAD_ARG;
     *out_len = h->len;
     return B200_SUCCESS;
 }
@@ -1212,22 +1149,12 @@ int32_t b200_state_read_bytes(b200_state* h, uint64_t ssz_offset, uint8_t* out, 
     Guard g(e);
     int32_t rc = check_ready(e);
     if (rc) return rc;
-    if (!duty_handle_ok(h) || (n && !out) || ssz_offset > h->len || n > h->len - ssz_offset) return B200_ERR_BAD_ARG;
-    const uint64_t lo = ssz_offset, hi = ssz_offset + n;
-    auto from_shadow = [&](uint64_t a, uint64_t b) {
-        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
-        if (x < y) memcpy(out + (x - lo), h->shadow + x, y - x);
-    };
-    from_shadow(0, h->so.var[2]);
-    from_shadow(h->so.var[7], h->len);
-    for (int f = 0; f < 5; f++) {   // the big lists from HBM
-        const uint64_t a = h->so.var[kBigVar[f]], b = h->so.var[kBigVar[f] + 1];
-        const uint64_t x = std::max(a, lo), y = std::min(b, hi);
-        if (x >= y) continue;
-        uint64_t field_off = 0; size_t nbytes = 0;
-        if (!h->plan.chain_field(f, &field_off, &nbytes)) return B200_ERR_BAD_ARG;
-        B200_CUDA_TRY(cudaMemcpyAsync(out + (x - lo), static_cast<const uint8_t*>(h->fields.p) + field_off + (x - a), y - x,
-                                      cudaMemcpyDeviceToHost, e.stream));
+    if (!resident(h) || (n && !out) || ssz_offset > h->len || n > h->len - ssz_offset) return B200_ERR_BAD_ARG;
+    for (const Piece& p : split_range(h, ssz_offset, ssz_offset + n)) {
+        uint8_t* to = out + (p.x - ssz_offset);
+        if (p.chain < 0) memcpy(to, h->shadow + p.x, p.y - p.x);
+        else if (p.chain < 5)   // the big lists from HBM (the shadow holds the vectors)
+            B200_CUDA_TRY(cudaMemcpyAsync(to, chain_dev(h, p.chain) + p.at, p.y - p.x, cudaMemcpyDeviceToHost, e.stream));
     }
     B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
     return B200_SUCCESS;
@@ -1252,7 +1179,6 @@ int32_t b200_state_upload_deneb_sharded(const uint8_t* ssz, size_t len, int32_t 
     if (rc) return rc;
     h->len = len; h->preset = preset;
     h->sharded = true;
-    h->uploaded = true;
     *out_handle = h.release();
     return B200_SUCCESS;
 }

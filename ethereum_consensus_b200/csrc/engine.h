@@ -67,7 +67,7 @@ struct Engine {
 Engine& engine();
 
 // The Validator records (121 bytes each, back to back, pubkey first) of a single-GPU resident state in HBM: *records and
-// *n (nullptr and 0 for an empty list).  B200_ERR_BAD_ARG for a NULL, not uploaded or sharded handle.  The records move
+// *n (nullptr and 0 for an empty list).  B200_ERR_BAD_ARG for a NULL or sharded handle.  The records move
 // when the list outgrows its reserved region, so the pointer holds until the state's next call; the caller holds the
 // engine lock.
 int32_t state_validator_records(const b200_state* h, const uint8_t** records, uint64_t* n);

@@ -28,7 +28,7 @@ struct EpochParams {
     uint64_t adjusted_slashing, total_active;
     uint32_t activation_limit;    // min(MAX_PER_EPOCH_ACTIVATION_CHURN_LIMIT, L); 0 without the registry step
     uint64_t activation_epoch;    // compute_activation_exit_epoch(cur)
-    // constants of the handle's preset (capi_ssz.cu: duty_preset)
+    // constants of the handle's preset (ssz_plan.h: preset_of)
     uint64_t increment, max_effective, ejection_balance, hysteresis_down, hysteresis_up;
     uint64_t score_bias, score_recovery, inactivity_denominator, withdraw_delay;
 };

@@ -587,26 +587,79 @@ int32_t SszPlan::run(Engine& e, DevBuf& arena, DevBuf& fields, DevBuf& planbuf, 
 
 // ------------------------------------------------------------------------------------------------ BeaconState
 namespace {
-struct Preset {
-    uint64_t slots_per_historical_root, historical_roots_limit, eth1_data_votes_bound, validator_registry_limit,
-        epochs_per_historical_vector, epochs_per_slashings_vector, sync_committee_size;
-};
-// ethereum-consensus/src/phase0/presets/{mainnet.rs:5-36,82-83, minimal.rs:20-25},
-// altair/presets/{mainnet,minimal}.rs:19
-const Preset kPresets[2] = {
-    {8192, 1ull << 24, 2048, 1ull << 40, 65536, 8192, 512},
-    {64, 1ull << 24, 32, 1ull << 40, 64, 64, 32},
-};
-inline uint32_t le32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | (uint32_t(p[3]) << 24); }
-inline uint64_t le64(const uint8_t* p) { return uint64_t(le32(p)) | (uint64_t(le32(p + 4)) << 32); }
+// ethereum-consensus/src/phase0/presets/{mainnet,minimal}.rs, altair/presets/{mainnet,minimal}.rs,
+// bellatrix/presets/{mainnet,minimal}.rs, configs/{mainnet,minimal}.rs
+constexpr Preset make_preset(bool minimal) {
+    Preset P{};
+    P.slots_per_epoch = minimal ? 8 : 32;
+    P.slots_per_historical_root = minimal ? 64 : 8192;
+    P.historical_roots_limit = uint64_t(1) << 24;
+    P.eth1_data_votes_bound = minimal ? 32 : 2048;
+    P.validator_registry_limit = uint64_t(1) << 40;
+    P.epochs_per_historical_vector = minimal ? 64 : 65536;
+    P.epochs_per_slashings_vector = minimal ? 64 : 8192;
+    P.sync_committee_size = minimal ? 32 : 512;
+    P.epochs_per_sync_committee_period = minimal ? 8 : 256;
+    P.shuffle_round_count = minimal ? 10 : 90;
+    P.epochs_per_eth1_voting_period = minimal ? 4 : 64;
+    P.min_per_epoch_churn_limit = minimal ? 2 : 4;
+    P.max_per_epoch_activation_churn_limit = minimal ? 4 : 8;
+    P.churn_limit_quotient = minimal ? 32 : 65536;
+    P.effective_balance_increment = 1000000000ull;
+    P.max_effective_balance = 32000000000ull;
+    P.ejection_balance = 16000000000ull;
+    P.hysteresis_quotient = 4;
+    P.hysteresis_downward_multiplier = 1;
+    P.hysteresis_upward_multiplier = 5;
+    P.inactivity_score_bias = 4;
+    P.inactivity_score_recovery_rate = 16;
+    P.inactivity_penalty_quotient_bellatrix = uint64_t(1) << 24;
+    P.proportional_slashing_multiplier_bellatrix = 3;
+    P.base_reward_factor = 64;
+    P.min_epochs_to_inactivity_penalty = 4;
+    P.max_seed_lookahead = 4;
+    P.min_validator_withdrawability_delay = 256;
+    return P;
+}
+constexpr Preset kPresets[2] = {make_preset(false), make_preset(true)};
 }  // namespace
 
-uint64_t eth1_data_votes_bound(int preset) { return kPresets[preset ? 1 : 0].eth1_data_votes_bound; }
-uint64_t historical_roots_limit(int preset) { return kPresets[preset ? 1 : 0].historical_roots_limit; }
+const Preset& preset_of(int preset) { return kPresets[preset == B200_PRESET_MINIMAL ? 1 : 0]; }
+
+StateChain state_chain(const StateOffsets& so, const Preset& P, int c) {
+    constexpr uint32_t kElem[9] = {121, 8, 1, 1, 8, 32, 32, 32, 8};
+    StateChain L{};
+    L.elem = kElem[c];
+    L.unit = c == 0 ? 121 : 32;
+    uint64_t limit;   // elements the type holds at most
+    if (c < 5) {
+        L.var = 2 + c;
+        L.lo = so.var[L.var]; L.hi = so.var[L.var + 1];
+        limit = P.validator_registry_limit;
+    } else {
+        const size_t lo[4] = {so.block_roots, so.state_roots, so.randao_mixes, so.slashings};
+        const uint64_t n[4] = {P.slots_per_historical_root, P.slots_per_historical_root, P.epochs_per_historical_vector,
+                               P.epochs_per_slashings_vector};
+        L.var = -1;
+        L.lo = lo[c - 5]; L.hi = L.lo + n[c - 5] * L.elem;
+        limit = n[c - 5];
+    }
+    L.len = L.bytes() / L.elem;
+    L.n_inputs = (L.bytes() + L.unit - 1) / L.unit;
+    L.depth = depth_for((limit * L.elem + L.unit - 1) / L.unit);
+    return L;
+}
+
+SmallList appendable_small_list(int field, const Preset& P) {
+    SmallList l;
+    if (field == B200_FIELD_ETH1_DATA_VOTES) l = {1, 72, P.eth1_data_votes_bound};
+    if (field == B200_FIELD_HISTORICAL_SUMMARIES) l = {8, 64, P.historical_roots_limit};
+    return l;
+}
 
 bool parse_beacon_state(const uint8_t* s, size_t len, int preset, StateOffsets& so) {
     if (preset < 0 || preset > 1) return false;
-    const Preset& P = kPresets[preset];
+    const Preset& P = preset_of(preset);
     size_t fixed = 8 + 32 + 8 + 16 + 112 + 2 * 32 * P.slots_per_historical_root + 4 + 72 + 4 + 8 + 4 + 4 +
                    32 * P.epochs_per_historical_vector + 8 * P.epochs_per_slashings_vector + 4 + 4 + 1 + 3 * 40 + 4 +
                    2 * (48 * P.sync_committee_size + 48) + 4 + 8 + 8 + 4;
@@ -660,16 +713,16 @@ static uint32_t assemble_state(SszPlan& p, const uint8_t* s, const StateOffsets&
     f[2] = p.leaf_bytes(s + 40, 8);
     f[3] = p.container({p.leaf_bytes(s + 48, 4), p.leaf_bytes(s + 52, 4), p.leaf_bytes(s + 56, 8)});
     f[4] = p.container({p.leaf_bytes(s + 64, 8), p.leaf_bytes(s + 72, 8), p.leaf(s + 80), p.leaf(s + 112), p.leaf(s + 144)});
-    int d_hist = depth_for(P.slots_per_historical_root);
-    if (vec) {
-        f[5] = vec[0]; f[6] = vec[1]; f[13] = vec[2]; f[14] = vec[3];
-    } else {
+    auto vector_root = [&](int c) {   // chain c = 5..8
+        if (vec) return vec[c - 5];
+        const StateChain L = state_chain(so, P, c);
         if (chain_vectors) p.begin_chain();
-        f[5] = p.wide_chunks(p.stage_field(s + so.block_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
-        if (chain_vectors) p.begin_chain();
-        f[6] = p.wide_chunks(p.stage_field(s + so.state_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
-        if (chain_vectors) p.end_chain();
-    }
+        const uint32_t r = p.wide_chunks(p.stage_field(s + L.lo, L.bytes()), L.n_inputs, L.depth);
+        p.end_chain();
+        return r;
+    };
+    f[5] = vector_root(5);
+    f[6] = vector_root(6);
     f[7] = p.mix_in_length(p.wide_chunks(p.stage_field(s + so.var[0], sz(0)), sz(0) / 32, depth_for(P.historical_roots_limit)), sz(0) / 32);
     {
         const uint8_t* e = s + so.eth1_data;
@@ -679,13 +732,8 @@ static uint32_t assemble_state(SszPlan& p, const uint8_t* s, const StateOffsets&
     f[10] = p.leaf_bytes(s + so.eth1_deposit_index, 8);
     f[11] = big[0];
     f[12] = big[1];
-    if (!vec) {
-        if (chain_vectors) p.begin_chain();
-        f[13] = p.wide_chunks(p.stage_field(s + so.randao_mixes, 32 * P.epochs_per_historical_vector), P.epochs_per_historical_vector, depth_for(P.epochs_per_historical_vector));
-        if (chain_vectors) p.begin_chain();
-        f[14] = p.wide_chunks(p.stage_field(s + so.slashings, 8 * P.epochs_per_slashings_vector), P.epochs_per_slashings_vector / 4, depth_for(P.epochs_per_slashings_vector / 4));
-        if (chain_vectors) p.end_chain();
-    }
+    f[13] = vector_root(7);
+    f[14] = vector_root(8);
     f[15] = big[2];
     f[16] = big[3];
     f[17] = p.leaf_bytes(s + so.justification_bits, 1);
@@ -747,19 +795,17 @@ int32_t build_beacon_state_plan(SszPlan& p, const uint8_t* s, size_t len, int pr
                                 const uint64_t* caps) {
     StateOffsets so;
     if (!parse_beacon_state(s, len, preset, so)) return B200_ERR_SSZ_MALFORMED;
-    const Preset& P = kPresets[preset];
-    auto sz = [&](int i) { return size_t(so.var[i + 1] - so.var[i]); };
-    const int d_reg = depth_for(P.validator_registry_limit);
-    constexpr uint64_t kElem[5] = {121, 8, 1, 1, 8};
-    const int depth[5] = {d_reg, d_reg - 2, d_reg - 5, d_reg - 5, d_reg - 2};
+    const Preset& P = preset_of(preset);
+    StateChain L[9];
+    for (int c = 0; c < 9; c++) L[c] = state_chain(so, P, c);
+    uint32_t big[5];
     if (!caps) {   // one-shot: the staging order the pipelined Validator upload is tuned with (same chains, same root)
-        uint32_t big[5];
         for (int q = 0; q < 5; q++) {
-            const size_t nb = sz(2 + q);
             p.begin_chain();
-            const uint64_t off = p.stage_field(s + so.var[2 + q], nb);
-            const uint32_t r = q == 0 ? p.wide_records(JOB_VALIDATORS, off, nb / 121, depth[0]) : p.wide_chunks(off, (nb + 31) / 32, depth[q]);
-            big[q] = p.mix_in_length(r, nb / kElem[q]);
+            const uint64_t off = p.stage_field(s + L[q].lo, L[q].bytes());
+            const uint32_t r = q == 0 ? p.wide_records(JOB_VALIDATORS, off, L[q].n_inputs, L[q].depth)
+                                      : p.wide_chunks(off, L[q].n_inputs, L[q].depth);
+            big[q] = p.mix_in_length(r, L[q].len);
         }
         p.end_chain();
         outputs.assign(1, assemble_state(p, s, so, P, big, nullptr, true));
@@ -768,35 +814,54 @@ int32_t build_beacon_state_plan(SszPlan& p, const uint8_t* s, size_t len, int pr
     // the five big lists are chains 0..4 (B200_FIELD_* in the C ABI), the four big vectors chains 5..8 (block_roots,
     // state_roots, randao_mixes, slashings): their jobs can re-hash dirty paths only.  All nine are staged and given their
     // arena levels first, so that their places do not depend on any small variable-size field.
-    Handoff hb[5], hv[4];
-    uint64_t len_of[5];
-    for (int q = 0; q < 5; q++) {
-        const size_t nb = sz(2 + q);
-        len_of[q] = nb / kElem[q];
-        if (caps && caps[q] < len_of[q]) return B200_ERR_BAD_ARG;
-        const uint64_t cap = caps ? caps[q] : 0;
+    for (int q = 0; q < 5; q++)
+        if (caps[q] < L[q].len) return B200_ERR_BAD_ARG;
+    Handoff h[9];
+    for (int c = 0; c < 9; c++) {
+        const uint64_t cap = c < 5 ? caps[c] : 0;
         p.begin_chain();
-        const uint64_t off = p.stage_field(s + so.var[2 + q], nb, size_t(cap * kElem[q]));
-        if (q == 0) hb[q] = p.records_to_handoff(JOB_VALIDATORS, off, len_of[q], depth[q], cap);
-        else hb[q] = p.chunks_to_handoff(off, (nb + 31) / 32, depth[q], (cap * kElem[q] + 31) / 32);
+        const uint64_t off = p.stage_field(s + L[c].lo, L[c].bytes(), size_t(cap * L[c].elem));
+        if (c == 0) h[c] = p.records_to_handoff(JOB_VALIDATORS, off, L[c].len, L[c].depth, cap);
+        else h[c] = p.chunks_to_handoff(off, L[c].n_inputs, L[c].depth, (cap * L[c].elem + 31) / 32);
     }
-    const int d_hist = depth_for(P.slots_per_historical_root);
-    p.begin_chain();
-    hv[0] = p.chunks_to_handoff(p.stage_field(s + so.block_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
-    p.begin_chain();
-    hv[1] = p.chunks_to_handoff(p.stage_field(s + so.state_roots, 32 * P.slots_per_historical_root), P.slots_per_historical_root, d_hist);
-    p.begin_chain();
-    hv[2] = p.chunks_to_handoff(p.stage_field(s + so.randao_mixes, 32 * P.epochs_per_historical_vector), P.epochs_per_historical_vector,
-                                depth_for(P.epochs_per_historical_vector));
-    p.begin_chain();
-    hv[3] = p.chunks_to_handoff(p.stage_field(s + so.slashings, 8 * P.epochs_per_slashings_vector), P.epochs_per_slashings_vector / 4,
-                                depth_for(P.epochs_per_slashings_vector / 4));
     p.end_chain();
-    uint32_t big[5], vec[4];
-    for (int q = 0; q < 5; q++) big[q] = p.mix_in_length(p.finish(hb[q]), len_of[q]);
-    for (int k = 0; k < 4; k++) vec[k] = p.finish(hv[k]);
+    uint32_t vec[4];
+    for (int q = 0; q < 5; q++) big[q] = p.mix_in_length(p.finish(h[q]), L[q].len);
+    for (int k = 0; k < 4; k++) vec[k] = p.finish(h[5 + k]);
     outputs.assign(1, assemble_state(p, s, so, P, big, vec));
     return B200_SUCCESS;
+}
+
+// This rank's slices of the five big lists, staged and reduced to one root each at the lists' slice depth.
+static int32_t plan_list_slices(SszPlan& p, const uint8_t* s, const StateOffsets& so, const Preset& P, int rank, int world,
+                                uint32_t root[5]) {
+    for (int q = 0; q < 5; q++) {
+        const StateChain L = state_chain(so, P, q);
+        uint64_t first, count; int k;
+        slice_of(L.n_inputs, world, rank, &first, &count, &k);
+        // never taken for a parsed state: 4 GiB give slices of at most 2^27 chunks, and the shallowest list is 35 deep
+        if (k > L.depth) return B200_ERR_LIMIT;
+        if (q == 0) {
+            root[0] = p.wide_records(JOB_VALIDATORS, p.stage_field(s + L.lo + 121 * first, 121 * count), count, k);
+        } else {   // chunk-granular slices: starts are multiples of 2^k chunks => 32-byte aligned
+            const uint64_t b0 = std::min(L.bytes(), first * 32), b1 = std::min(L.bytes(), (first + count) * 32);
+            root[q] = p.wide_chunks(p.stage_field(s + L.lo + b0, b1 - b0), count, k);
+        }
+    }
+    return B200_SUCCESS;
+}
+
+// The five big lists' roots (length mixed in) from world x 5 slice roots: node(r, q) is rank r's root of list q.
+template <class Node>
+static void plan_list_tops(SszPlan& p, const StateOffsets& so, const Preset& P, int world, Node node, uint32_t big[5]) {
+    for (int q = 0; q < 5; q++) {
+        const StateChain L = state_chain(so, P, q);
+        uint64_t first, count; int k;
+        slice_of(L.n_inputs, world, 0, &first, &count, &k);
+        std::vector<uint32_t> nodes;
+        for (int r = 0; r < world; r++) nodes.push_back(node(r, q));
+        big[q] = p.mix_in_length(p.merkle_small(nodes, k, L.depth), L.len);
+    }
 }
 
 int32_t build_beacon_state_shard_plan(SszPlan& p, const uint8_t* s, size_t len, int preset, int rank, int world,
@@ -804,21 +869,10 @@ int32_t build_beacon_state_shard_plan(SszPlan& p, const uint8_t* s, size_t len, 
     StateOffsets so;
     if (!parse_beacon_state(s, len, preset, so)) return B200_ERR_SSZ_MALFORMED;
     if (world < 1 || (world & (world - 1)) || rank < 0 || rank >= world) return B200_ERR_BAD_ARG;
-    auto sz = [&](int i) { return size_t(so.var[i + 1] - so.var[i]); };
-    outputs.clear();
-    uint64_t first, count; int k;
-    // validators: records
-    slice_of(sz(2) / 121, world, rank, &first, &count, &k);
-    outputs.push_back(p.wide_records(JOB_VALIDATORS, p.stage_field(s + so.var[2] + 121 * first, 121 * count), count, k));
-    // packed lists: chunk-granular slices (slice starts are multiples of 2^k chunks => 32-byte aligned)
-    const int idx[4] = {3, 4, 5, 6};
-    for (int q = 0; q < 4; q++) {
-        size_t nb = sz(idx[q]);
-        uint64_t nch = (nb + 31) / 32;
-        slice_of(nch, world, rank, &first, &count, &k);
-        size_t b0 = std::min(nb, size_t(first) * 32), b1 = std::min(nb, size_t(first + count) * 32);
-        outputs.push_back(p.wide_chunks(p.stage_field(s + so.var[idx[q]] + b0, b1 - b0), count, k));
-    }
+    uint32_t root[5];
+    const int32_t rc = plan_list_slices(p, s, so, preset_of(preset), rank, world, root);
+    if (rc) return rc;
+    outputs.assign(root, root + 5);
     return B200_SUCCESS;
 }
 
@@ -829,34 +883,13 @@ int32_t build_beacon_state_sharded_plan(SszPlan& p, const uint8_t* s, size_t len
     StateOffsets so;
     if (!parse_beacon_state(s, len, preset, so)) return B200_ERR_SSZ_MALFORMED;
     if (world < 1 || (world & (world - 1)) || rank < 0 || rank >= world) return B200_ERR_BAD_ARG;
-    const Preset& P = kPresets[preset];
-    auto sz = [&](int i) { return size_t(so.var[i + 1] - so.var[i]); };
-    const int d_reg = depth_for(P.validator_registry_limit);
-    const uint64_t n_elems[5] = {sz(2) / 121, (sz(3) + 31) / 32, (sz(4) + 31) / 32, (sz(5) + 31) / 32, (sz(6) + 31) / 32};
-    const uint64_t lens[5] = {sz(2) / 121, sz(3) / 8, sz(4), sz(5), sz(6) / 8};
-    const int depth[5] = {d_reg, d_reg - 2, d_reg - 5, d_reg - 5, d_reg - 2};
-    const int var_of[5] = {2, 3, 4, 5, 6};
-    std::vector<uint32_t> local(5);
-    int kq[5];
-    for (int q = 0; q < 5; q++) {
-        uint64_t first, count;
-        slice_of(n_elems[q], world, rank, &first, &count, &kq[q]);
-        if (kq[q] > depth[q]) return B200_ERR_LIMIT;
-        if (q == 0) {
-            local[0] = p.wide_records(JOB_VALIDATORS, p.stage_field(s + so.var[2] + 121 * first, 121 * count), count, kq[0]);
-        } else {   // chunk-granular slices: starts are multiples of 2^k chunks => 32-byte aligned
-            const size_t nb = sz(var_of[q]);
-            const size_t b0 = std::min(nb, size_t(first) * 32), b1 = std::min(nb, size_t(first + count) * 32);
-            local[size_t(q)] = p.wide_chunks(p.stage_field(s + so.var[var_of[q]] + b0, b1 - b0), count, kq[q]);
-        }
-    }
-    const uint32_t remote = p.exchange(local, world);
+    const Preset& P = preset_of(preset);
+    uint32_t root[5];
+    const int32_t rc = plan_list_slices(p, s, so, P, rank, world, root);
+    if (rc) return rc;
+    const uint32_t remote = p.exchange(std::vector<uint32_t>(root, root + 5), world);
     uint32_t big[5];
-    for (int q = 0; q < 5; q++) {
-        std::vector<uint32_t> nodes;
-        for (int r = 0; r < world; r++) nodes.push_back(remote + uint32_t(r) * 5u + uint32_t(q));
-        big[q] = p.mix_in_length(p.merkle_small(nodes, kq[q], depth[q]), lens[q]);
-    }
+    plan_list_tops(p, so, P, world, [&](int r, int q) { return remote + uint32_t(r) * 5u + uint32_t(q); }, big);
     outputs.assign(1, assemble_state(p, s, so, P, big));
     return B200_SUCCESS;
 }
@@ -866,20 +899,9 @@ int32_t build_beacon_state_combine_plan(SszPlan& p, const uint8_t* s, size_t len
     StateOffsets so;
     if (!parse_beacon_state(s, len, preset, so)) return B200_ERR_SSZ_MALFORMED;
     if (world < 1 || (world & (world - 1))) return B200_ERR_BAD_ARG;
-    const Preset& P = kPresets[preset];
-    auto sz = [&](int i) { return size_t(so.var[i + 1] - so.var[i]); };
-    int d_reg = depth_for(P.validator_registry_limit);
-    const uint64_t n_elems[5] = {sz(2) / 121, (sz(3) + 31) / 32, (sz(4) + 31) / 32, (sz(5) + 31) / 32, (sz(6) + 31) / 32};
-    const uint64_t lens[5] = {sz(2) / 121, sz(3) / 8, sz(4), sz(5), sz(6) / 8};
-    const int depth[5] = {d_reg, d_reg - 2, d_reg - 5, d_reg - 5, d_reg - 2};
+    const Preset& P = preset_of(preset);
     uint32_t big[5];
-    for (int q = 0; q < 5; q++) {
-        uint64_t first, count; int k;
-        slice_of(n_elems[q], world, 0, &first, &count, &k);
-        std::vector<uint32_t> nodes;
-        for (int r = 0; r < world; r++) nodes.push_back(p.leaf(all_roots + (size_t(r) * 5 + q) * 32));
-        big[q] = p.mix_in_length(p.merkle_small(nodes, k, depth[q]), lens[q]);
-    }
+    plan_list_tops(p, so, P, world, [&](int r, int q) { return p.leaf(all_roots + (size_t(r) * 5 + q) * 32); }, big);
     outputs.assign(1, assemble_state(p, s, so, P, big));
     return B200_SUCCESS;
 }

@@ -170,6 +170,25 @@ private:
 
 int depth_for(uint64_t n);
 
+inline uint32_t le32(const uint8_t* p) { return p[0] | (p[1] << 8) | (p[2] << 16) | (uint32_t(p[3]) << 24); }
+inline uint64_t le64(const uint8_t* p) { return uint64_t(le32(p)) | (uint64_t(le32(p + 4)) << 32); }
+
+// The constants of a preset that the state plans, the duties and process_epoch read
+struct Preset {
+    uint64_t slots_per_epoch, slots_per_historical_root, historical_roots_limit, eth1_data_votes_bound,
+        validator_registry_limit, epochs_per_historical_vector, epochs_per_slashings_vector, sync_committee_size;
+    uint64_t epochs_per_sync_committee_period, shuffle_round_count;
+    // process_epoch
+    uint64_t epochs_per_eth1_voting_period, min_per_epoch_churn_limit, max_per_epoch_activation_churn_limit,
+        churn_limit_quotient;
+    uint64_t effective_balance_increment, max_effective_balance, ejection_balance;
+    uint64_t hysteresis_quotient, hysteresis_downward_multiplier, hysteresis_upward_multiplier;
+    uint64_t inactivity_score_bias, inactivity_score_recovery_rate, inactivity_penalty_quotient_bellatrix;
+    uint64_t proportional_slashing_multiplier_bellatrix, base_reward_factor, min_epochs_to_inactivity_penalty;
+    uint64_t max_seed_lookahead, min_validator_withdrawability_delay;
+};
+const Preset& preset_of(int preset);   // B200_PRESET_MAINNET or B200_PRESET_MINIMAL
+
 // deneb BeaconState (ethereum-consensus/src/deneb/beacon_state.rs:26-63): byte offsets of the
 // fixed-size fields and of the nine variable-size fields inside the SSZ serialization.
 struct StateOffsets {
@@ -183,14 +202,37 @@ struct StateOffsets {
     uint32_t var_word[9] = {0};  // byte position of each offset word in the fixed part
 };
 bool parse_beacon_state(const uint8_t* ssz, size_t len, int preset, StateOffsets& so);
+
+// The nine chains of a resident state plan: 0..4 the five big lists in B200_FIELD_* order (validators, balances,
+// previous / current epoch participation, inactivity_scores), 5..8 the four big vectors (block_roots, state_roots,
+// randao_mixes, slashings).  The sharded plans slice the five lists the same way.
+struct StateChain {
+    int var;            // StateOffsets::var index of a big list, -1 for a vector
+    uint64_t lo, hi;    // byte range in the serialization
+    uint32_t elem;      // element size in bytes
+    uint32_t unit;      // bytes per first-job input: a 121-byte Validator record or a 32-byte chunk
+    uint64_t len;       // elements
+    uint64_t n_inputs;  // first-job inputs
+    int depth;          // Merkle depth of the data (below a list's length mix-in)
+    uint64_t bytes() const { return hi - lo; }
+    uint32_t input_of(uint64_t i) const { return uint32_t(i * elem / unit); }   // the input covering element i
+};
+StateChain state_chain(const StateOffsets& so, const Preset& P, int c);
+
+// The two small lists that grow by appending (B200_FIELD_ETH1_DATA_VOTES, B200_FIELD_HISTORICAL_SUMMARIES): their
+// StateOffsets::var index, element size and limit.  var = -1 for any other field id.
+struct SmallList {
+    int var = -1;
+    uint32_t elem = 0;
+    uint64_t limit = 0;
+};
+SmallList appendable_small_list(int field, const Preset& P);
+
 // `caps` (optional, element counts of the five big lists, each >= the list's length): the lists' field regions and arena
 // levels are reserved for that many elements and are laid out, with the four big vectors, ahead of everything whose size
 // depends on a small variable-size field — a device-resident state can then grow or reshape without moving them.
 int32_t build_beacon_state_plan(SszPlan& plan, const uint8_t* ssz, size_t len, int preset, std::vector<uint32_t>& outputs,
                                 const uint64_t* caps = nullptr);
-// ETH1_DATA_VOTES_BOUND / HISTORICAL_ROOTS_LIMIT of a preset (0 mainnet, 1 minimal)
-uint64_t eth1_data_votes_bound(int preset);
-uint64_t historical_roots_limit(int preset);
 int32_t build_beacon_state_shard_plan(SszPlan& plan, const uint8_t* ssz, size_t len, int preset, int rank, int world,
                                       std::vector<uint32_t>& outputs);
 int32_t build_beacon_state_sharded_plan(SszPlan& plan, const uint8_t* ssz, size_t len, int preset, int rank, int world,
