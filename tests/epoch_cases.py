@@ -61,6 +61,95 @@ def base(n: int, epoch: int, preset: str = "mainnet", seed: int = 1, keys: bool 
     return st
 
 
+# the launch shape of csrc/epoch.cu: k_epoch_totals / k_epoch_apply run one thread per validator in CTAs of THREADS;
+# k_epoch_reduce's REDUCE_THREADS threads fold ranges of `per` consecutive CTAs; a changed-record count above
+# max(REHASH_MIN, n / 16) re-hashes the whole Validator list (capi_ssz.cu)
+THREADS, REDUCE_THREADS, REHASH_MIN = 256, 512, 4096
+
+
+@dataclass
+class Grid:
+    """Where a state's exit queue, ejections, activations and sums fall in the device's launch shape."""
+    n: int
+    nb: int             # CTAs
+    per: int            # CTAs per k_epoch_reduce thread
+    act_exit: int       # compute_activation_exit_epoch(current epoch)
+    e0: int
+    c0: int
+    L: int              # churn limit
+    limit: int          # activation churn limit
+    head: np.ndarray    # indices whose exit epoch is E0 (the c0 validators the exit-queue head counts)
+    eject: np.ndarray   # ejected indices in rank order
+    eject_epoch: np.ndarray
+    offered: np.ndarray  # activation candidates per CTA (after the eligibility update)
+    winners: np.ndarray  # activated indices
+    sums: list           # the five k_epoch_totals sums, each per CTA (Python ints)
+    pushes: int          # records k_epoch_apply and k_activation_select append to the changed list under ALL
+    threshold: int
+
+    def cta(self, i):
+        return np.asarray(i) // THREADS
+
+    def warp(self, i):   # warp inside its CTA
+        return np.asarray(i) % THREADS // 32
+
+    def lane(self, i):
+        return np.asarray(i) % 32
+
+    def rthread(self, i):   # the k_epoch_reduce thread whose range holds i's CTA
+        return self.cta(i) // self.per
+
+    def overflow(self, k):
+        """(the whole sum, the largest CTA partial, the largest k_epoch_reduce range) reach 2^64."""
+        s = self.sums[k]
+        ranges = [sum(s[t:t + self.per]) for t in range(0, self.nb, self.per)]
+        return sum(s) > U64, max(s) > U64, max(ranges) > U64
+
+    def ranks_cross(self):
+        """Ranks k (k >= 1) where the exit epoch steps up between ejection k - 1 and k."""
+        return np.nonzero(np.diff(self.eject_epoch.astype(np.int64)))[0] + 1
+
+
+def grid(st: S.SynthState) -> Grid:
+    st = eo.clone(st)
+    n = len(st.validators)
+    nb = -(-n // THREADS)
+    per = -(-nb // REDUCE_THREADS)
+    v = eo._Vector(st)
+    cur, prev = v.cur(), v.prev()
+    e0, c0, L = v.exit_queue()
+    vv = st.validators
+    eb = vv["effective_balance"].astype(np.uint64)
+    exit_ = vv["exit_epoch"].astype(np.uint64)
+    head = np.nonzero(exit_ == np.uint64(e0))[0]
+    eject = np.nonzero(v.active(cur) & (eb <= np.uint64(eo.EJECTION_BALANCE)) & (exit_ == np.uint64(FAR)))[0]
+    limit = min(eo.PRESET[st.preset]["MAX_PER_EPOCH_ACTIVATION_CHURN_LIMIT"], L)
+    slashed = vv["slashed"] != 0
+    pf, cf = st.previous_epoch_participation, st.current_epoch_participation
+    a_cur, a_prev = v.active(cur), v.active(prev)
+    masks = [a_cur] + [a_prev & ~slashed & (((pf >> f) & 1) != 0) for f in range(3)] + [a_cur & ~slashed & ((cf & 2) != 0)]
+    ebo = eb.astype(object)
+    sums = [[int(ebo[b * THREADS:(b + 1) * THREADS][m[b * THREADS:(b + 1) * THREADS]].sum()) for b in range(nb)] for m in masks]
+    reg = eo.clone(st)
+    eo._Vector(reg).registry_updates()
+    ru = reg.validators
+    elig = ru["activation_eligibility_epoch"]
+    fin = int.from_bytes(st.fixed["finalized_checkpoint"][:8], "little")
+    cand = (elig <= np.uint64(fin)) & (vv["activation_epoch"] == np.uint64(FAR))
+    offered = np.bincount(np.nonzero(cand)[0] // THREADS, minlength=nb)
+    winners = np.nonzero(ru["activation_epoch"] != vv["activation_epoch"])[0]
+    try:
+        post, _ = eo.process_epoch(st, eo.ALL)
+        pv = post.validators
+        rec = ((pv["activation_eligibility_epoch"] != vv["activation_eligibility_epoch"]) | (pv["exit_epoch"] != vv["exit_epoch"])
+               | (pv["effective_balance"] != vv["effective_balance"]))
+        pushes = int(rec.sum()) + int((pv["activation_epoch"] != vv["activation_epoch"]).sum())
+    except eo.Refused:
+        pushes = -1
+    return Grid(n, nb, per, eo.compute_activation_exit_epoch(cur), e0, c0, L, limit, head, eject, ru["exit_epoch"][eject].astype(np.uint64), offered, winners, sums,
+                pushes, max(REHASH_MIN, n // 16))
+
+
 def _flags(st, which: str, bit: int, on: bool) -> None:
     a = getattr(st, which)
     setattr(st, which, (np.where(on, a | (1 << bit), a & ~np.uint8(1 << bit))).astype(np.uint8))
@@ -80,6 +169,106 @@ def finality(rule: int, preset: str = "mainnet") -> S.SynthState:
     _flags(st, "previous_epoch_participation", 1, prev_hi)
     _flags(st, "current_epoch_participation", 1, cur_hi)
     return st
+
+
+def exits(st, idx, epoch) -> None:
+    """Validators `idx` exit at `epoch` (withdrawable MIN_VALIDATOR_WITHDRAWABILITY_DELAY later)."""
+    st.validators["exit_epoch"][idx] = epoch
+    st.validators["withdrawable_epoch"][idx] = epoch + eo.MIN_VALIDATOR_WITHDRAWABILITY_DELAY
+
+
+def ejects(st, idx) -> None:
+    st.validators["effective_balance"][idx] = eo.EJECTION_BALANCE
+
+
+def pending(st, idx, elig) -> None:
+    """Validators `idx` wait in the activation queue, eligible since `elig`."""
+    st.validators["activation_epoch"][idx] = FAR
+    st.validators["activation_eligibility_epoch"][idx] = elig
+
+
+def grid_cases() -> list:
+    """Small states whose exit-queue head, ejections, sums, activation candidates and changed-record counts sit where
+    the device's kernels pass values between lanes, warps and CTAs (csrc/epoch.cu); every one at most 4 097 validators.
+    Regime "grid:<name>"; test_epoch_cases.py asserts each shape from `grid()`."""
+    out = []
+    add = lambda name, st, refusal=None: out.append(Case(name, st, "grid:" + name, refusal))  # noqa: E731
+    # the exit-queue head with c0 < L, merged across warps and CTAs; ejection ranks stepping over a multiple of L between
+    # two CTAs.  mainnet n = 600 / 1000 / 520: L = 4, 3 / 4 / 3 CTAs (the last ragged: 88 / 232 / 8 threads)
+    st = base(600, 1000, seed=60)
+    exits(st, [33, 100, 230], 1012)                         # E0 = the largest exit, c0 = 3, warps 1, 3, 7 of CTA 0
+    exits(st, [7, 300], 990)
+    ejects(st, [255, 256, 420, 599])                        # (3 + k) / 4 steps at k = 1: thread 255 of CTA 0, 0 of CTA 1
+    add("head_c0_3_warps", st)
+    st = base(1000, 1000, seed=61)
+    exits(st, [0, 999], 1005)                               # E0 = compute_activation_exit_epoch, c0 = 2, first and last CTA
+    ejects(st, [31, 767, 768, 998])                         # (2 + k) / 4 steps at k = 2: CTA 2's last thread, CTA 3's first
+    add("head_c0_2_first_last_cta", st)
+    st = base(520, 1000, seed=62)
+    exits(st, [519], 1009)                                  # c0 = 1 at the last valid thread of the ragged CTA
+    ejects(st, [100, 200, 255, 256, 511, 512])              # (1 + k) / 4 steps at k = 3: thread 0 of CTA 1
+    add("head_c0_1_ragged", st)
+    # minimal n = 600: L = 18, c0 = 17 holders in every CTA; ranks step at k = 1 (CTA 0 -> 1) and k = 19 (CTA 1 -> 2)
+    st = base(600, 1000, "minimal", seed=63)
+    exits(st, [0, 31, 32, 63, 64, 200, 255, 256, 287, 288, 400, 511, 512, 543, 544, 598, 599], 1010)
+    ejects(st, [254] + list(range(257, 500, 14)) + [513, 514, 597])
+    add("head_c0_17_minimal", st)
+    # ejections at lanes 0 and 31, threads 0 and 255, all in the ragged last CTA, one per CTA
+    st = base(1000, 1000, seed=64)
+    ejects(st, [32, 63, 160, 191, 256, 511, 767])           # c0 = 0: E0 = compute_activation_exit_epoch
+    add("eject_lanes_threads", st)
+    st = base(1000, 1000, seed=65)
+    exits(st, [5], 1005)
+    ejects(st, [768, 769, 799, 800, 900, 999])              # c0 = 1; all in CTA 3 (232 threads), its first and last
+    add("eject_ragged_last_cta", st)
+    st = base(4096, 1000, "minimal", seed=66)                # L = 128, c0 = 126: (126 + k) / 128 steps at k = 2
+    exits(st, np.arange(126) * 32 + 7, 1011)
+    ejects(st, np.arange(16) * 256 + np.array([0, 255, 31, 32, 128, 1, 254, 63, 64, 100, 200, 17, 96, 33, 250, 255]))
+    add("eject_one_per_cta", st)
+    # get_total_balance's 128-bit sums: every CTA partial below 2^64, the fold across CTAs at 2^64 (refused) and 2^64 - 1
+    for name, total, refusal in (("sum_2p64_across_ctas", 1 << 64, "limit"), ("sum_2p64_minus_1_across_ctas", U64, None)):
+        st = base(600, 1000, seed=67)
+        eb = st.validators["effective_balance"]
+        rest = int(eb.astype(object).sum()) - 3 * int(eb[0])
+        eb[[10, 300, 590]] = [1 << 62, 1 << 63, total - rest - (1 << 62) - (1 << 63)]
+        add(name, st, refusal)
+    # previous-epoch-only overflow: validators exiting at the current epoch count in the previous-epoch flag sums only
+    st = base(600, 1000, seed=68)
+    exits(st, [20, 21, 400, 401], 1000)
+    st.validators["effective_balance"][[20, 21, 400, 401]] = [1 << 62, 1 << 62, 1 << 62, (1 << 62) + 5]
+    st.previous_epoch_participation[[20, 21, 400, 401]] = 7
+    add("overflow_previous_only", st, "limit")
+    # activation candidates (mainnet, limit 4)
+    st = base(600, 1000, seed=69)
+    pending(st, np.arange(260, 270), 990)                   # CTA 1 offers 10 at the earliest eligibility
+    pending(st, [3, 520], 992)
+    st.fixed["finalized_checkpoint"] = _cp(995, b"f")
+    add("activation_many_in_one_cta", st)
+    st = base(1000, 1000, seed=70)
+    pending(st, [900, 600, 300, 10, 257, 520], 990)         # ties across CTAs, broken by index
+    pending(st, [5, 6], 994)
+    st.fixed["finalized_checkpoint"] = _cp(995, b"f")
+    add("activation_ties_across_ctas", st)
+    st = base(1000, 1000, seed=71)
+    pending(st, [768, 999, 850, 851, 852], 985)             # the winners: all in the ragged last CTA
+    pending(st, [0, 1, 300, 700], 986)
+    st.fixed["finalized_checkpoint"] = _cp(995, b"f")
+    add("activation_last_cta_only", st)
+    st = base(600, 1000, "minimal", seed=72)
+    pending(st, [40, 599], 990)                             # a queue of 2 under limit 4
+    add("activation_short_queue", st)
+    # changed-record counts at the re-hash threshold (max(4096, n / 16) = 4096 at n = 4097): eligibility set on records
+    # with activation_eligibility_epoch = FAR and effective_balance = MAX, plus one activated record whose effective
+    # balance also changes (two pushes)
+    for count in (4096, 4097):
+        st = base(4097, 1000, seed=73)
+        st.balances[:] = 32 * ETH
+        st.validators["activation_eligibility_epoch"][1:count - 1] = FAR
+        pending(st, [4096], 990)
+        st.balances[4096] = 40 * ETH
+        st.validators["effective_balance"][4096] = 30 * ETH
+        add(f"changed_{count}", st)
+    return out
 
 
 def cases() -> list:
@@ -187,4 +376,4 @@ def cases() -> list:
     st = base(40, 7, "minimal", seed=53)
     st.validators["exit_epoch"][:] = 8
     add("refuse_no_active_next", st, "refusal", "bad_arg")
-    return out
+    return out + grid_cases()

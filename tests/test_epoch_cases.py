@@ -40,6 +40,10 @@ def test_case_hits_regime(case):
     st, r = case.st, case.regime
     cur = eo.current_epoch(st)
     v = eo._Vector(eo.clone(st))
+    if r.startswith("grid:"):
+        GRID_SHAPES[r[5:]](ec.grid(st), st)
+        if not case.refusal:
+            return
     if case.refusal:
         with pytest.raises(eo.Refused) as ei:
             eo.process_epoch(st, eo.ALL)
@@ -130,8 +134,142 @@ def test_case_hits_regime(case):
         raise AssertionError(r)
 
 
+def _step_at_cta_edges(g):
+    """The ranks where the closed form's exit epoch steps up whose two ejections lie in different CTAs."""
+    return [k for k in g.ranks_cross() if g.cta(g.eject[k - 1]) != g.cta(g.eject[k])]
+
+
+def _head(g, c0, from_largest_exit):
+    assert g.c0 == c0 == len(g.head) and 0 < c0 < g.L
+    assert (g.e0 > g.act_exit) == from_largest_exit and g.e0 >= g.act_exit
+    assert _step_at_cta_edges(g)
+
+
+def _overflow_only_across_ctas(g, k):
+    whole, cta, _ = g.overflow(k)
+    assert whole and not cta
+
+
+def _refused_under(st, bits):
+    for name, m in MASKS:
+        try:
+            eo.process_epoch(st, m)
+            refused = False
+        except eo.Refused as r:
+            assert r.kind == "limit"
+            refused = True
+        assert refused == bool(m & bits), name
+
+
+def _shape_changed(g, want):
+    assert g.pushes == want
+    assert len(g.winners) == 1   # the activated record also changes its effective balance: two pushes
+
+
+def _head_c0_3_warps(g, st):
+    _head(g, 3, True)
+    assert len(set(g.cta(g.head))) == 1 < len(set(g.warp(g.head)))
+    assert g.eject[_step_at_cta_edges(g)[0]] % ec.THREADS == 0
+
+
+def _head_c0_2_first_last_cta(g, st):
+    _head(g, 2, False)
+    assert set(g.cta(g.head)) == {0, g.nb - 1}
+
+
+def _head_c0_1_ragged(g, st):
+    _head(g, 1, True)
+    assert g.n % ec.THREADS and g.head.tolist() == [g.n - 1]
+
+
+def _head_c0_17_minimal(g, st):
+    _head(g, g.L - 1, True)
+    assert st.preset == "minimal" and set(g.cta(g.head)) == set(range(g.nb))
+    assert len(_step_at_cta_edges(g)) >= 2
+
+
+def _eject_lanes_threads(g, st):
+    assert {0, 31} <= set(g.lane(g.eject)) and {0, ec.THREADS - 1} <= set(g.eject % ec.THREADS)
+    assert len(g.eject) > g.L and g.c0 == 0 and len(set(g.cta(g.eject))) >= 3
+
+
+def _eject_ragged_last_cta(g, st):
+    assert g.n % ec.THREADS and set(g.cta(g.eject)) == {g.nb - 1} and g.c0 == 1
+    assert g.eject[0] % ec.THREADS == 0 and g.eject[-1] == g.n - 1
+    assert len(g.ranks_cross()) and not _step_at_cta_edges(g)
+
+
+def _eject_one_per_cta(g, st):
+    _head(g, g.L - 2, True)
+    assert np.bincount(g.cta(g.eject), minlength=g.nb).tolist() == [1] * g.nb
+
+
+def _sum_2p64_across_ctas(g, st):
+    _overflow_only_across_ctas(g, 0)
+    assert sum(g.sums[0]) == 1 << 64
+
+
+def _sum_2p64_minus_1_across_ctas(g, st):
+    assert sum(g.sums[0]) == ec.U64 and not g.overflow(0)[0] and g.pushes > 0
+    eb = st.validators["effective_balance"]
+    assert any(int(e) * int(s) > ec.U64 for e, s in zip(eb, st.inactivity_scores))   # the inactivity penalty wraps
+
+
+def _overflow_previous_only(g, st):
+    assert [g.overflow(k)[0] for k in range(5)] == [False, True, True, True, False]
+    for k in (1, 2, 3):
+        _overflow_only_across_ctas(g, k)
+    _refused_under(st, eo.STEP["justification_and_finalization"] | eo.STEP["rewards_and_penalties"])
+
+
+def _activation_many_in_one_cta(g, st):
+    assert g.offered.max() > g.limit == len(g.winners)
+    assert set(g.cta(g.winners)) == {int(g.offered.argmax())}
+
+
+def _activation_last_cta_only(g, st):
+    assert g.n % ec.THREADS and set(g.cta(g.winners)) == {g.nb - 1} and len(g.winners) == g.limit
+    assert g.offered[:-1].sum() > 0 and st.validators["activation_epoch"][g.n - 1] == ec.FAR
+
+
+def _activation_short_queue(g, st):
+    assert 0 < len(g.winners) == g.offered.sum() < g.limit and len(set(g.cta(g.winners))) > 1
+
+
+def _ties_across_ctas(g, st):
+    vv = st.validators
+    fin = int.from_bytes(st.fixed["finalized_checkpoint"][:8], "little")
+    q = np.nonzero((vv["activation_eligibility_epoch"] <= fin) & (vv["activation_epoch"] == ec.FAR))[0]
+    last = vv["activation_eligibility_epoch"][g.winners].max()
+    tied = q[vv["activation_eligibility_epoch"][q] == last]
+    losers = np.setdiff1d(tied, g.winners)
+    assert len(g.winners) == g.limit and len(losers) and len(set(g.cta(tied))) >= 3
+    assert losers.min() > g.winners.max() and len(set(g.cta(g.winners))) > 1
+
+
+GRID_SHAPES = {
+    "head_c0_3_warps": _head_c0_3_warps,
+    "head_c0_2_first_last_cta": _head_c0_2_first_last_cta,
+    "head_c0_1_ragged": _head_c0_1_ragged,
+    "head_c0_17_minimal": _head_c0_17_minimal,
+    "eject_lanes_threads": _eject_lanes_threads,
+    "eject_ragged_last_cta": _eject_ragged_last_cta,
+    "eject_one_per_cta": _eject_one_per_cta,
+    "sum_2p64_across_ctas": _sum_2p64_across_ctas,
+    "sum_2p64_minus_1_across_ctas": _sum_2p64_minus_1_across_ctas,
+    "overflow_previous_only": _overflow_previous_only,
+    "activation_many_in_one_cta": _activation_many_in_one_cta,
+    "activation_ties_across_ctas": _ties_across_ctas,
+    "activation_last_cta_only": _activation_last_cta_only,
+    "activation_short_queue": _activation_short_queue,
+    "changed_4096": lambda g, st: _shape_changed(g, g.threshold),
+    "changed_4097": lambda g, st: _shape_changed(g, g.threshold + 1),
+}
+
+
 def test_refusal_kinds_cover_every_rule():
     kinds = {c.name: c.refusal for c in CASES if c.refusal}
-    assert set(kinds) == {"refuse_block_root", "refuse_total_overflow", "refuse_withdrawable_overflow", "refuse_no_active_next"}
+    assert set(kinds) == {"refuse_block_root", "refuse_total_overflow", "refuse_withdrawable_overflow", "refuse_no_active_next",
+                          "sum_2p64_across_ctas", "overflow_previous_only"}
     with pytest.raises(eo.Refused):
         eo.process_epoch(CASES[0].st, 1 << 12)
