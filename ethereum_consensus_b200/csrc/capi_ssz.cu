@@ -78,11 +78,28 @@ struct b200_state {
     uint8_t* pinned_head = nullptr;   // page-locked ranges of the shadow (registration is an optimisation)
     uint8_t* pinned_tail = nullptr;
     bool sharded = false;   // b200_state_upload_deneb_sharded: this rank's slices only; root is a collective, no updates
+    // ---- beacon committees (b200_state_committee_count_per_slot ... b200_state_attesting_indices) ----
+    // Bumped by every write into the Validator records (chain 0): a cached epoch built under another generation is stale.
+    uint64_t records_gen = 0;
+    // One epoch's shuffled active list, valid while its seed (recomputed from the shadow on every call) and the records'
+    // generation are those it was built with; `pos` (the inverse map, one u32 per validator) is built on first use.
+    struct CommitteeEpoch {
+        bool used = false, pos_ready = false;
+        uint64_t epoch = 0, gen = 0, n_active = 0, cps = 0, last_use = 0;
+        uint8_t seed[32] = {0};
+        DevBuf shuffled, pos;
+    };
+    static constexpr int kCommitteeEpochs = 4;   // previous, current and next, and one more asked epoch
+    CommitteeEpoch committees[kCommitteeEpochs];
+    uint64_t committee_tick = 0;
+    DevBuf committee_work;   // per-call inputs and outputs of the committee kernels
     ~b200_state() {  // callers hold the engine lock and have selected the device
         if (pinned_head) cudaHostUnregister(pinned_head);
         if (pinned_tail) cudaHostUnregister(pinned_tail);
         free(shadow);
         arena.release(); fields.release(); planbuf.release(); selbuf.release(); scatter.release();
+        for (CommitteeEpoch& c : committees) { c.shuffled.release(); c.pos.release(); }
+        committee_work.release();
     }
 };
 
@@ -257,6 +274,7 @@ int32_t adopt_plan(Engine& e, b200_state* h, SszPlan& np, std::vector<uint32_t>&
         }
         h->arena.release(); h->fields.release();
         h->arena = na; h->fields = nf;
+        h->records_gen++;
         for (int c = 0; c < 9; c++) if (full[size_t(c)]) h->rehash[size_t(c)] = 1;
         mark_all_small(h);
     }
@@ -531,6 +549,7 @@ int32_t b200_state_update_elements(b200_state* h, int32_t field, const uint64_t*
     B200_CUDA_TRY(cudaGetLastError());
     B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
     for (size_t i = 0; i < n; i++) h->dirty[field].push_back(L.input_of(indices[i]));
+    if (field == 0) h->records_gen++;
     return B200_SUCCESS;
 }
 
@@ -585,6 +604,7 @@ static int32_t update_bytes(Engine& e, b200_state* h, uint64_t ssz_offset, const
         B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
         const uint32_t unit = chain(h, p.chain).unit;
         for (uint64_t u = p.at / unit; u <= (p.at + (p.y - p.x) - 1) / unit; u++) h->dirty[p.chain].push_back(uint32_t(u));
+        if (p.chain == 0) h->records_gen++;
     }
     return B200_SUCCESS;
 }
@@ -617,6 +637,7 @@ static int32_t append_big(Engine& e, b200_state* h, int f, const uint8_t* values
     memcpy(e.staging.p, values, n * elem);
     B200_CUDA_TRY(cudaMemcpyAsync(chain_dev(h, f) + old_bytes, e.staging.p, n * elem, cudaMemcpyHostToDevice, e.stream));
     B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+    if (f == 0) h->records_gen++;
     // appended inputs are dirty; the old ragged last chunk is among them when the first appended element shares it
     for (uint64_t u = L.input_of(old_n); u <= L.input_of(new_n - 1); u++) h->dirty[f].push_back(uint32_t(u));
     // new length mix-in and finisher ops; the finisher nodes of the lists' tops are allocated ahead of the small fields'
@@ -936,6 +957,246 @@ int32_t b200_state_sync_committee_indices(b200_state* h, int32_t which, uint64_t
     return B200_SUCCESS;
 }
 
+// ---- beacon committees on a resident state (phase0/helpers.rs:741-806, 896-974; deneb/block_processing.rs:53-100) ----
+namespace {
+constexpr uint8_t kDomainBeaconAttester[4] = {1, 0, 0, 0};   // domains.rs:19-30
+constexpr size_t kMaxAttestations = size_t(1) << 20;         // b200_state_attesting_indices' bound per call
+using CommitteeEpoch = b200_state::CommitteeEpoch;
+
+// get_committee_count_per_slot (:741-773) for n active validators
+uint64_t committees_per_slot(const Preset& P, uint64_t n) {
+    return std::max<uint64_t>(1, std::min<uint64_t>(P.max_committees_per_slot, n / P.slots_per_epoch / P.target_committee_size));
+}
+
+// The cached committee source of `epoch`: get_active_validator_indices(epoch) shuffled by get_seed(epoch, BeaconAttester)
+// on the device.  A hit needs the same seed (recomputed from the shadow) and the same records generation; a miss rebuilds
+// the least recently used entry.  Every launch is on the engine stream, so later kernels of the call see the list.
+int32_t committee_epoch(Engine& e, b200_state* h, uint64_t epoch, CommitteeEpoch** out) {
+    const Preset& P = preset_of(h->preset);
+    uint8_t seed[32];
+    state_seed(h, epoch, kDomainBeaconAttester, seed);
+    CommitteeEpoch* lru = &h->committees[0];
+    for (CommitteeEpoch& c : h->committees) {
+        if (c.used && c.epoch == epoch && c.gen == h->records_gen && !memcmp(c.seed, seed, 32)) {
+            c.last_use = ++h->committee_tick;
+            *out = &c;
+            return B200_SUCCESS;
+        }
+        if (!c.used || (lru->used && c.last_use < lru->last_use)) lru = &c;
+    }
+    CommitteeEpoch& c = *lru;
+    c.used = false;
+    c.pos_ready = false;
+    const uint64_t n = chain(h, 0).len;
+    uint64_t cnt = 0;
+    if (n) {
+        uint64_t *d_act, *d_out;
+        int32_t rc = shuffle_scratch(e, n, &d_act, &d_out);
+        if (rc) return rc;
+        rc = active_indices_on_device(e, chain_dev(h, 0), n, epoch, d_act, &cnt);
+        if (rc) return rc;
+        B200_CUDA_TRY(c.shuffled.reserve(cnt * 8 + 64));
+        rc = shuffle_on_device(e, d_act, cnt, seed, uint32_t(P.shuffle_round_count), static_cast<uint64_t*>(c.shuffled.p));
+        if (rc) return rc;
+    }
+    c.epoch = epoch;
+    c.gen = h->records_gen;
+    memcpy(c.seed, seed, 32);
+    c.n_active = cnt;
+    c.cps = committees_per_slot(P, cnt);
+    c.last_use = ++h->committee_tick;
+    c.used = true;
+    *out = &c;
+    return B200_SUCCESS;
+}
+
+// the entry's inverse position map (built on first use)
+int32_t committee_positions(Engine& e, b200_state* h, CommitteeEpoch& c) {
+    if (c.pos_ready) return B200_SUCCESS;
+    const uint64_t n = chain(h, 0).len;
+    B200_CUDA_TRY(c.pos.reserve(n * 4 + 64));
+    int32_t rc = committee_positions_on_device(e, static_cast<const uint64_t*>(c.shuffled.p), c.n_active, n, static_cast<uint32_t*>(c.pos.p));
+    if (rc) return rc;
+    c.pos_ready = true;
+    return B200_SUCCESS;
+}
+
+int32_t begin_timed(Engine& e) {
+    B200_CUDA_TRY(cudaEventRecord(e.ev0, e.stream));
+    return B200_SUCCESS;
+}
+int32_t end_timed(Engine& e) {
+    B200_CUDA_TRY(cudaEventRecord(e.ev1, e.stream));
+    B200_CUDA_TRY(cudaEventSynchronize(e.ev1));
+    B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, e.ev0, e.ev1));
+    return B200_SUCCESS;
+}
+
+// attesting_indices' work buffer: jobs | Bitlist bytes | output indices
+size_t o_bits_of(size_t n_jobs) { return (n_jobs * sizeof(AttestingJob) + 255) & ~size_t(255); }
+size_t o_out_of(size_t n_jobs, size_t n_bits_bytes) { return (o_bits_of(n_jobs) + n_bits_bytes + 255) & ~size_t(255); }
+
+// Bitlist[MAX_VALIDATORS_PER_COMMITTEE] length in bits of `len` SSZ bytes; false when malformed (no delimiter bit: empty
+// or a zero last byte, or more than `max_bits` bits)
+bool bitlist_len(const uint8_t* b, size_t len, uint64_t max_bits, uint64_t* bits) {
+    if (len == 0 || b[len - 1] == 0 || len > max_bits / 8 + 1) return false;
+    *bits = 8 * uint64_t(len - 1) + uint64_t(31 - __builtin_clz(uint32_t(b[len - 1])));
+    return *bits <= max_bits;
+}
+}  // namespace
+
+int32_t b200_state_committee_count_per_slot(b200_state* h, uint64_t epoch, uint64_t* out) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!resident(h) || !out) return B200_ERR_BAD_ARG;
+    CommitteeEpoch* c;
+    if ((rc = begin_timed(e)) || (rc = committee_epoch(e, h, epoch, &c)) || (rc = end_timed(e))) return rc;
+    *out = c->cps;
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_beacon_committees(b200_state* h, uint64_t epoch, uint64_t* out_indices, uint32_t* out_offsets, uint64_t* out_cps,
+                                     size_t* out_n) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!resident(h) || !out_indices || !out_offsets || !out_cps || !out_n) return B200_ERR_BAD_ARG;
+    const Preset& P = preset_of(h->preset);
+    CommitteeEpoch* c;
+    if ((rc = begin_timed(e)) || (rc = committee_epoch(e, h, epoch, &c))) return rc;
+    if (c->n_active == 0) { e.last_error = "beacon_committees: no active validator"; return B200_ERR_BAD_ARG; }
+    if ((rc = end_timed(e))) return rc;   // the device time of the kernels; the list then goes to the host
+    B200_CUDA_TRY(cudaMemcpyAsync(out_indices, c->shuffled.p, c->n_active * 8, cudaMemcpyDeviceToHost, e.stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+    const uint64_t count = P.slots_per_epoch * c->cps, n = c->n_active;
+    for (uint64_t k = 0; k <= count; k++) out_offsets[k] = uint32_t(n * k / count);
+    *out_cps = c->cps;
+    *out_n = size_t(n);
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_attester_duties(b200_state* h, uint64_t epoch, const uint64_t* validators, size_t n, uint64_t* out) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!resident(h) || (n && !out) || n > 0xffffffffull) return B200_ERR_BAD_ARG;
+    const Preset& P = preset_of(h->preset);
+    const uint64_t N = chain(h, 0).len;
+    if (!validators && n != N) { e.last_error = "attester_duties: validators == NULL asks for all N validators"; return B200_ERR_BAD_ARG; }
+    for (size_t i = 0; validators && i < n; i++)
+        if (validators[i] >= N) { e.last_error = "attester_duties: validator index beyond the registry"; return B200_ERR_BAD_ARG; }
+    if (epoch > shadow_slot(h) / P.slots_per_epoch + 1) { e.last_error = "attester_duties: epoch after the next epoch"; return B200_ERR_BAD_ARG; }
+    if (epoch > ~uint64_t(0) / P.slots_per_epoch) { e.last_error = "attester_duties: epoch * SLOTS_PER_EPOCH overflows u64"; return B200_ERR_BAD_ARG; }
+    if (!n) return B200_SUCCESS;
+    CommitteeEpoch* c;
+    if ((rc = begin_timed(e)) || (rc = committee_epoch(e, h, epoch, &c)) || (rc = committee_positions(e, h, *c))) return rc;
+    // work: requested indices | rows
+    const size_t o_rows = validators ? ((n * 8 + 255) & ~size_t(255)) : 0;
+    B200_CUDA_TRY(h->committee_work.reserve(o_rows + n * 40));
+    uint8_t* w = static_cast<uint8_t*>(h->committee_work.p);
+    if (validators) {
+        B200_CUDA_TRY(e.staging.reserve(n * 8));
+        memcpy(e.staging.p, validators, n * 8);
+        B200_CUDA_TRY(cudaMemcpyAsync(w, e.staging.p, n * 8, cudaMemcpyHostToDevice, e.stream));
+    }
+    rc = attester_duties_on_device(e, static_cast<const uint32_t*>(c->pos.p), validators ? reinterpret_cast<const uint64_t*>(w) : nullptr,
+                                   n, c->n_active, c->cps, P.slots_per_epoch, epoch, reinterpret_cast<uint64_t*>(w + o_rows));
+    if (rc) return rc;
+    if ((rc = end_timed(e))) return rc;
+    B200_CUDA_TRY(cudaMemcpyAsync(out, w + o_rows, n * 40, cudaMemcpyDeviceToHost, e.stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_attesting_indices(b200_state* h, size_t n_att, const uint8_t* data, const uint8_t* bits, const uint32_t* bits_offsets,
+                                     uint64_t* out_indices, uint32_t* out_offsets, int32_t* out_codes) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!resident(h) || n_att > kMaxAttestations) return B200_ERR_BAD_ARG;
+    if (!n_att) {
+        if (out_offsets) out_offsets[0] = 0;
+        e.last_kernel_ms = 0.f;
+        return B200_SUCCESS;
+    }
+    if (!data || !bits_offsets || !out_indices || !out_offsets || !out_codes) return B200_ERR_BAD_ARG;
+    if (bits_offsets[0] != 0) { e.last_error = "attesting_indices: bits_offsets[0] must be 0"; return B200_ERR_BAD_ARG; }
+    for (size_t a = 0; a < n_att; a++)
+        if (bits_offsets[a + 1] < bits_offsets[a]) { e.last_error = "attesting_indices: bits_offsets decrease"; return B200_ERR_BAD_ARG; }
+    const size_t n_bits_bytes = bits_offsets[n_att];
+    if (n_bits_bytes && !bits) return B200_ERR_BAD_ARG;
+
+    // ---- the host step: process_attestation's checks from the shadow and the cached committees ----
+    const Preset& P = preset_of(h->preset);
+    const uint64_t state_slot = shadow_slot(h), cur = state_slot / P.slots_per_epoch, prev = cur ? cur - 1 : 0;
+    if ((rc = begin_timed(e))) return rc;
+    CommitteeEpoch* ce[2] = {nullptr, nullptr};   // previous, current (built when first asked)
+    std::vector<AttestingJob> jobs;
+    uint32_t total = 0;
+    out_offsets[0] = 0;
+    for (size_t a = 0; a < n_att; a++) {
+        const uint8_t* d = data + 128 * a;
+        const uint8_t* b = bits + bits_offsets[a];
+        const size_t nb = bits_offsets[a + 1] - bits_offsets[a];
+        const uint64_t slot = le64(d), index = le64(d + 8), target = le64(d + 88);
+        uint64_t len = 0;
+        int32_t code = B200_SUCCESS;
+        CommitteeEpoch* c = nullptr;
+        if (!bitlist_len(b, nb, P.max_validators_per_committee, &len)) code = B200_ATTESTATION_MALFORMED_BITS;
+        else if (target != prev && target != cur) code = B200_ATTESTATION_INVALID_TARGET_EPOCH;
+        else if (slot / P.slots_per_epoch != target) code = B200_ATTESTATION_INVALID_SLOT;
+        else if (slot + P.min_attestation_inclusion_delay > state_slot) code = B200_ATTESTATION_NO_DELAY;   // wraps, as a release build
+        else {
+            CommitteeEpoch*& slot_entry = ce[target == cur ? 1 : 0];
+            if (!slot_entry && (rc = committee_epoch(e, h, target, &slot_entry))) return rc;
+            c = slot_entry;
+            if (index >= c->cps) code = B200_ATTESTATION_INVALID_INDEX;
+        }
+        uint32_t set = 0;
+        if (!code) {
+            const uint64_t count = P.slots_per_epoch * c->cps, k = (slot % P.slots_per_epoch) * c->cps + index;
+            const uint64_t start = c->n_active * k / count, end = c->n_active * (k + 1) / count;
+            if (len != end - start) code = B200_ATTESTATION_BITFIELD;
+            else {
+                for (size_t i = 0; i < nb; i++) set += uint32_t(__builtin_popcount(b[i]));
+                set -= 1;   // the delimiter
+                if (!set) code = B200_ATTESTATION_INDICES_EMPTY;
+                else jobs.push_back({static_cast<const uint64_t*>(c->shuffled.p) + start, uint32_t(len), bits_offsets[a], total, 0});
+            }
+        }
+        out_codes[a] = code;
+        if (!code) total += set;
+        out_offsets[a + 1] = total;
+    }
+
+    // ---- the gather on the device ----
+    if (!jobs.empty()) {
+        const size_t o_bits = o_bits_of(jobs.size()), o_out = o_out_of(jobs.size(), n_bits_bytes);
+        B200_CUDA_TRY(h->committee_work.reserve(o_out + size_t(total) * 8));
+        B200_CUDA_TRY(e.staging.reserve(o_out));
+        uint8_t* hs = static_cast<uint8_t*>(e.staging.p);
+        memcpy(hs, jobs.data(), jobs.size() * sizeof(AttestingJob));
+        memcpy(hs + o_bits, bits, n_bits_bytes);
+        uint8_t* w = static_cast<uint8_t*>(h->committee_work.p);
+        B200_CUDA_TRY(cudaMemcpyAsync(w, hs, o_out, cudaMemcpyHostToDevice, e.stream));
+        rc = attesting_indices_on_device(e, reinterpret_cast<const AttestingJob*>(w), uint32_t(jobs.size()), w + o_bits,
+                                         reinterpret_cast<uint64_t*>(w + o_out));
+        if (rc) return rc;
+    }
+    if ((rc = end_timed(e))) return rc;
+    if (!jobs.empty()) {
+        B200_CUDA_TRY(cudaMemcpyAsync(out_indices, static_cast<uint8_t*>(h->committee_work.p) + o_out_of(jobs.size(), n_bits_bytes),
+                                      size_t(total) * 8, cudaMemcpyDeviceToHost, e.stream));
+        B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
+    }
+    return B200_SUCCESS;
+}
+
 // ---- process_epoch on a resident state (deneb/spec/mod.rs:965-1003) ----
 namespace {
 // floor(sqrt(x)) exactly (u64::integer_sqrt): Newton's iteration on integers from above
@@ -1068,6 +1329,7 @@ int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_cod
         rc = epoch_apply_on_device(e, dev[0], reinterpret_cast<uint64_t*>(dev[1]), reinterpret_cast<uint64_t*>(dev[4]), dev[2], n,
                                    p, &changed, &n_changed);
         if (rc) return rc;
+        if (n_changed) h->records_gen++;
         // changed records: re-hash their paths, or the whole list once they are more than a sixteenth of it
         if (n_changed > std::max<uint64_t>(4096, n / 16)) {
             h->rehash[0] = 1;

@@ -337,6 +337,83 @@ __global__ void __launch_bounds__(kThreads) k_match_committee_keys(const uint8_t
     }
 }
 
+// ---- beacon committees over an epoch's cached shuffled active list (phase0/helpers.rs:459-483, 741-806) ----
+// Committee k of C = SLOTS_PER_EPOCH x committees_per_slot is positions [n k / C, n (k + 1) / C) of the list.
+// k_committee_positions inverts the list: pos[shuffled[p]] = p over a map pre-filled with kNotActive.  A duty row is then
+// arithmetic on p: the committee holding p is k = ((p + 1) C - 1) / n, the largest k with n k / C <= p, so never an empty
+// one; (p + 1) C fits u64 (C <= 2048, p < 2^31).
+__global__ void __launch_bounds__(kThreads) k_committee_positions(const uint64_t* __restrict__ shuffled, uint64_t n,
+                                                                    uint32_t* __restrict__ pos) {
+    const uint64_t p = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (p < n) pos[shuffled[p]] = uint32_t(p);
+}
+// AttestationDuty rows (slot, committee_index, committee_length, committees_at_slot, validator_committee_index) for
+// validators[r] (nullptr: r itself); UINT64_MAX x 5 for a validator not active at the epoch
+__global__ void __launch_bounds__(kThreads) k_attester_duties(const uint32_t* __restrict__ pos, const uint64_t* __restrict__ validators,
+                                                                uint64_t n_rows, uint64_t n, uint64_t cps, uint64_t spe,
+                                                                uint64_t epoch, uint64_t* __restrict__ out) {
+    const uint64_t r = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (r >= n_rows) return;
+    const uint32_t p = pos[validators ? validators[r] : r];
+    uint64_t* row = out + r * 5;
+    if (p == kNotActive) {
+#pragma unroll
+        for (int f = 0; f < 5; f++) row[f] = ~uint64_t(0);
+        return;
+    }
+    const uint64_t c = spe * cps;
+    const uint64_t k = ((uint64_t(p) + 1) * c - 1) / n;
+    const uint64_t start = n * k / c, end = n * (k + 1) / c;
+    row[0] = epoch * spe + k / cps;
+    row[1] = k % cps;
+    row[2] = end - start;
+    row[3] = cps;
+    row[4] = p - start;
+}
+
+// get_attesting_indices + get_indexed_attestation's sort (phase0/helpers.rs:896-974), one CTA per attestation that passed
+// the host's checks: the set bits of its committee slice are compacted by warp ballot into shared memory (committee order
+// is lost, the sort restores a canonical one), padded with UINT64_MAX to a power of two and bitonic-sorted ascending, then
+// written at the job's prefix-summed offset.  A committee member appears once, so the sorted set is the sorted list.
+constexpr int kAttThreads = 256;
+__global__ void __launch_bounds__(kAttThreads) k_attesting_indices(const AttestingJob* __restrict__ jobs, const uint8_t* __restrict__ bits,
+                                                                     uint64_t* __restrict__ out) {
+    __shared__ uint64_t s[kMaxCommitteeBits];
+    __shared__ uint32_t count;
+    const AttestingJob j = jobs[blockIdx.x];
+    const uint32_t lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) count = 0;
+    __syncthreads();
+    const uint8_t* b = bits + j.bits_off;
+    for (uint32_t i0 = 0; i0 < j.len; i0 += kAttThreads) {   // uniform trip count: whole warps reach the ballot
+        const uint32_t i = i0 + threadIdx.x;
+        const bool set = i < j.len && ((b[i >> 3] >> (i & 7)) & 1u);
+        const uint32_t m = __ballot_sync(0xffffffffu, set);
+        uint32_t base = 0;
+        if (lane == 0 && m) base = atomicAdd(&count, uint32_t(__popc(m)));
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (set) s[base + __popc(m & ((1u << lane) - 1u))] = j.committee[i];
+    }
+    __syncthreads();
+    const uint32_t n = count;
+    uint32_t size = 1;
+    while (size < n) size <<= 1;
+    for (uint32_t i = n + threadIdx.x; i < size; i += kAttThreads) s[i] = ~uint64_t(0);
+    __syncthreads();
+    for (uint32_t k = 2; k <= size; k <<= 1)
+        for (uint32_t d = k >> 1; d > 0; d >>= 1) {
+            for (uint32_t i = threadIdx.x; i < size; i += kAttThreads) {
+                const uint32_t l = i ^ d;
+                if (l > i) {
+                    const uint64_t a = s[i], c = s[l];
+                    if ((a > c) == ((i & k) == 0)) { s[i] = c; s[l] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    for (uint32_t i = threadIdx.x; i < n; i += kAttThreads) out[uint64_t(j.out_off) + i] = s[i];
+}
+
 }  // namespace
 
 struct ShuffleScratch {
@@ -528,6 +605,36 @@ int32_t match_committee_keys_on_device(Engine& e, const uint8_t* recs_dev, uint6
         memcpy(&v, hs + o_out + 8 * size_t(k), 8);
         out[k] = v ? v - 1 : ~uint64_t(0);
     }
+    return B200_SUCCESS;
+}
+
+int32_t committee_positions_on_device(Engine& e, const uint64_t* shuffled_dev, uint64_t n_active, uint64_t n_validators, uint32_t* pos_dev) {
+    if (n_active > n_validators || n_validators > (uint64_t(1) << 32)) { e.last_error = "committee positions: bad list sizes"; return B200_ERR_BAD_ARG; }
+    cudaStream_t st = e.stream;
+    if (n_validators) B200_CUDA_TRY(cudaMemsetAsync(pos_dev, 0xff, n_validators * 4, st));
+    if (n_active) {
+        k_committee_positions<<<unsigned((n_active + kThreads - 1) / kThreads), kThreads, 0, st>>>(shuffled_dev, n_active, pos_dev);
+        e.launches++;
+        B200_CUDA_TRY(cudaGetLastError());
+    }
+    return B200_SUCCESS;
+}
+
+int32_t attester_duties_on_device(Engine& e, const uint32_t* pos_dev, const uint64_t* validators_dev, uint64_t n_rows, uint64_t n_active,
+                                  uint64_t cps, uint64_t slots_per_epoch, uint64_t epoch, uint64_t* out_dev) {
+    if (!n_rows) return B200_SUCCESS;
+    k_attester_duties<<<unsigned((n_rows + kThreads - 1) / kThreads), kThreads, 0, e.stream>>>(pos_dev, validators_dev, n_rows, n_active,
+                                                                                                cps, slots_per_epoch, epoch, out_dev);
+    e.launches++;
+    B200_CUDA_TRY(cudaGetLastError());
+    return B200_SUCCESS;
+}
+
+int32_t attesting_indices_on_device(Engine& e, const AttestingJob* jobs_dev, uint32_t n_jobs, const uint8_t* bits_dev, uint64_t* out_dev) {
+    if (!n_jobs) return B200_SUCCESS;
+    k_attesting_indices<<<n_jobs, kAttThreads, 0, e.stream>>>(jobs_dev, bits_dev, out_dev);
+    e.launches++;
+    B200_CUDA_TRY(cudaGetLastError());
     return B200_SUCCESS;
 }
 }  // namespace b200

@@ -619,6 +619,10 @@ constexpr Preset make_preset(bool minimal) {
     P.min_epochs_to_inactivity_penalty = 4;
     P.max_seed_lookahead = 4;
     P.min_validator_withdrawability_delay = 256;
+    P.target_committee_size = minimal ? 4 : 128;
+    P.max_committees_per_slot = minimal ? 4 : 64;
+    P.max_validators_per_committee = 2048;
+    P.min_attestation_inclusion_delay = 1;
     return P;
 }
 constexpr Preset kPresets[2] = {make_preset(false), make_preset(true)};

@@ -186,6 +186,8 @@ struct Preset {
     uint64_t inactivity_score_bias, inactivity_score_recovery_rate, inactivity_penalty_quotient_bellatrix;
     uint64_t proportional_slashing_multiplier_bellatrix, base_reward_factor, min_epochs_to_inactivity_penalty;
     uint64_t max_seed_lookahead, min_validator_withdrawability_delay;
+    // beacon committees (phase0/helpers.rs:741-806) and process_attestation (deneb/block_processing.rs:53-100)
+    uint64_t target_committee_size, max_committees_per_slot, max_validators_per_committee, min_attestation_inclusion_delay;
 };
 const Preset& preset_of(int preset);   // B200_PRESET_MAINNET or B200_PRESET_MINIMAL
 

@@ -195,6 +195,68 @@ B200_API int32_t b200_state_next_sync_committee(b200_state* handle, uint64_t* ou
 B200_API int32_t b200_state_sync_committee_updates(b200_state* handle, int32_t* rotated, int32_t* out_code);
 B200_API int32_t b200_state_sync_committee_indices(b200_state* handle, int32_t which, uint64_t* out);
 
+/* Beacon committees on a device-resident state (single-GPU handles; a NULL, not uploaded or sharded handle gets
+ * B200_ERR_BAD_ARG and is left as it was): who attests where, and who signed an attestation, computed where the Validator
+ * records are.  These calls read the state and never write it.  Preset constants follow the handle's preset:
+ * SLOTS_PER_EPOCH 32 / 8, TARGET_COMMITTEE_SIZE 128 / 4, MAX_COMMITTEES_PER_SLOT 64 / 4, SHUFFLE_ROUND_COUNT 90 / 10
+ * (mainnet / minimal); MAX_VALIDATORS_PER_COMMITTEE 2048 and MIN_ATTESTATION_INCLUSION_DELAY 1 in both.
+ * An epoch's committees are the slices [n k / C, n (k + 1) / C), k = 0 .. C - 1 with C = SLOTS_PER_EPOCH x cps, of its n
+ * active validators shuffled by get_seed(epoch, BeaconAttester = {1,0,0,0}) (compute_committee, phase0/helpers.rs:459-483);
+ * get_beacon_committee(slot, index) (:775-806) is committee k = (slot mod SLOTS_PER_EPOCH) x cps + index of slot's epoch,
+ * and cps = get_committee_count_per_slot = max(1, min(MAX_COMMITTEES_PER_SLOT, n / SLOTS_PER_EPOCH / TARGET_COMMITTEE_SIZE))
+ * (:741-773).  A committee is empty when n < C.
+ * The handle caches the shuffled active lists of the last four epochs asked, in HBM.  An entry is used only while its
+ * epoch's seed (recomputed from the host copy on every call) and the Validator records are what it was built from: any
+ * write into the records (b200_state_update_elements or b200_state_update_bytes on them, an append to the validator list,
+ * a relocation, or a b200_state_process_epoch that changes a record) makes every entry stale.  A cached epoch costs no
+ * shuffle.  b200_last_kernel_ms: the device time of the call's kernels, without the copy of the results to the host.
+ *  - b200_state_committee_count_per_slot: *out = cps of `epoch` (1 when no validator is active).
+ *  - b200_state_beacon_committees: every committee of `epoch`: out_indices (room for n entries; the registry length always
+ *    suffices) receives the shuffled active list, out_offsets (SLOTS_PER_EPOCH x cps + 1 <= 2049 entries) the committee
+ *    bounds, *out_cps and *out_n = n.  No active validator at `epoch` -> B200_ERR_BAD_ARG.
+ *  - b200_state_attester_duties: get_committee_assignment of the validator guide for each of the n validators named
+ *    (validators == NULL with n == the registry length: every validator), as out[5 i .. 5 i + 4] = the AttestationDuty
+ *    fields slot, committee_index, committee_length, committees_at_slot, validator_committee_index; a validator not
+ *    active at `epoch` gets five UINT64_MAX.  B200_ERR_BAD_ARG before any work: an index >= the registry length, NULL with
+ *    another n, n > 2^32 - 1, an epoch after the state's next epoch (the guide's `assert epoch <= next_epoch`), or an
+ *    epoch x SLOTS_PER_EPOCH that overflows u64.
+ *  - b200_state_attesting_indices: for n_att attestations, data (n_att x 128 bytes, SSZ AttestationData) and the SSZ
+ *    Bitlist[MAX_VALIDATORS_PER_COMMITTEE] aggregation_bits of attestation a at bytes [bits_offsets[a], bits_offsets[a+1])
+ *    of `bits`: the attesting_indices of get_indexed_attestation (:896-974), the committee members whose bit is set in
+ *    ascending order, as out_indices[out_offsets[a] .. out_offsets[a+1]) (out_offsets: n_att + 1 entries; out_indices: room
+ *    for the sum of the Bitlists' lengths in bits), and out_codes[a].  An attestation that fails gets its code and an empty
+ *    slice.  The checks run in deneb process_attestation's order (deneb/block_processing.rs:53-100), after the Bitlist's
+ *    decoding and before is_valid_indexed_attestation's emptiness test; the source checkpoint (participation flags) and
+ *    the signature are not checked here:
+ *      B200_ATTESTATION_MALFORMED_BITS        no delimiter bit (no bytes, or a zero last byte), or more than 2048 bits;
+ *      B200_ATTESTATION_INVALID_TARGET_EPOCH  target.epoch neither the previous nor the current epoch (InvalidTargetEpoch);
+ *      B200_ATTESTATION_INVALID_SLOT          target.epoch != compute_epoch_at_slot(slot) (InvalidSlot);
+ *      B200_ATTESTATION_NO_DELAY              slot + MIN_ATTESTATION_INCLUSION_DELAY > state.slot, the sum wrapping in u64 as
+ *                                             a release build computes it (NoDelay);
+ *      B200_ATTESTATION_INVALID_INDEX         index >= get_committee_count_per_slot(target.epoch) (InvalidIndex);
+ *      B200_ATTESTATION_BITFIELD              the Bitlist's length != the committee's length (Bitfield);
+ *      B200_ATTESTATION_INDICES_EMPTY         no bit set (InvalidIndexedAttestation::AttestingIndicesEmpty).
+ *    These codes are neither blst codes nor engine errors.  B200_ERR_BAD_ARG before any work: a NULL pointer (bits may be
+ *    NULL when bits_offsets[n_att] == 0), bits_offsets not starting at 0 or decreasing, or n_att > 2^20.  n_att == 0
+ *    succeeds and sets out_offsets[0] = 0 when out_offsets is not NULL. */
+enum {
+    B200_ATTESTATION_INVALID_TARGET_EPOCH = 0x201,
+    B200_ATTESTATION_INVALID_SLOT = 0x202,
+    B200_ATTESTATION_NO_DELAY = 0x203,
+    B200_ATTESTATION_INVALID_INDEX = 0x204,
+    B200_ATTESTATION_BITFIELD = 0x205,
+    B200_ATTESTATION_INDICES_EMPTY = 0x206,
+    B200_ATTESTATION_MALFORMED_BITS = 0x207
+};
+B200_API int32_t b200_state_committee_count_per_slot(b200_state* handle, uint64_t epoch, uint64_t* out);
+B200_API int32_t b200_state_beacon_committees(b200_state* handle, uint64_t epoch, uint64_t* out_indices, uint32_t* out_offsets,
+                                              uint64_t* out_cps, size_t* out_n);
+B200_API int32_t b200_state_attester_duties(b200_state* handle, uint64_t epoch, const uint64_t* validators, size_t n,
+                                            uint64_t* out /* n x 5 */);
+B200_API int32_t b200_state_attesting_indices(b200_state* handle, size_t n_att, const uint8_t* data, const uint8_t* bits,
+                                              const uint32_t* bits_offsets, uint64_t* out_indices, uint32_t* out_offsets,
+                                              int32_t* out_codes);
+
 /* Epoch processing on a device-resident state (single-GPU handles, as the duties above).  Sub-steps of deneb
  * process_epoch (deneb/spec/mod.rs:991-1002), in the reference's order: */
 #define B200_EPOCH_JUSTIFICATION_AND_FINALIZATION  (1u << 0)
