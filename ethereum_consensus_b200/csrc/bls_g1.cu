@@ -7,17 +7,11 @@
 //                 5-round shared-memory tree of Jacobian additions; lane 0 normalises to affine.
 // Squarings (~75 % of this kernel's products) use the dedicated PTX square (222 wide MADs instead of 288).  It pays
 // with 256-thread CTAs at 224 registers; with the 168-register cap the square's wider live range spills, and at ptxas'
-// default level it loses to predicate spills.  -DB200_G1_SQR_VIA_MUL restores squares-by-product.
-#if defined(B200_G1_SQR_VIA_MUL)
-#define B200_FP_SQR_VIA_MUL 1
-#endif
+// default level it loses to predicate spills.
 // Products as by-value function CALLS (operands and result in registers, 0-byte frames) instead of ~70 inlined copies:
 // the inlined kernel is 0.5 MB of straight-line code, far beyond the instruction caches, and only pays at 8 warps per SM
-// where the warps stay in step.  With calls the kernel body is about a third of that and 12 warps per SM
-// win.  -DB200_G1_INLINE_MUL restores the inlined products.
-#if !defined(B200_G1_INLINE_MUL)
+// where the warps stay in step.  With calls the kernel body is about a third of that and 12 warps per SM win.
 #define B200_FP_MUL_CALL 1
-#endif
 // fp_pow's window table in dynamic shared memory (fp.cuh): every kernel here that can reach fp_pow is launched through
 // with_pow_tab() below.  Thread-local storage made the per-key kernel's speed depend on what else the process had run.
 #define B200_POW_TAB_SMEM 1
@@ -42,26 +36,17 @@ __device__ __forceinline__ void g1_validate_body(const uint8_t* __restrict__ key
     codes[i] = rc;
     if (rc == BLS_SUCCESS) out[i] = p;
 }
-// Default (variant 7): 384 threads capped at 168 registers = 12 warps per SM (with call-based products, see the top of
-// this file).  Variant 0: 256-thread CTAs at 224 registers (8 warps per SM, no spills).  Variant 6: 512 threads at 128
-// registers = 16 warps per SM.  The register budgets follow from the SM's 64 K-entry register file;
-// B200_G1_VARIANT selects a variant at run time for A/B runs.  (__maxnreg__ cannot be combined with __launch_bounds__.)
-__global__ void __maxnreg__(224) k_g1_validate_main(const uint8_t* __restrict__ keys, uint32_t n, G1Aff* __restrict__ out,
-                                                    int32_t* __restrict__ codes) {
-    g1_validate_body(keys, n, out, codes);
-}
+// 168 registers = 12 warps per SM (with call-based products, see the top of this file); 256-thread CTAs at 224
+// registers (8 warps per SM, no spills) measured slower (DESIGN.md §4).  The register budgets follow from the SM's
+// 64 K-entry register file.  (__maxnreg__ cannot be combined with __launch_bounds__.)
+// (Occupancies between 8 and 12 warps per SM do not exist for this kernel: the register file is handed out in units of
+// four warps, so 9-, 10- and 11-warp CTAs at 224 / 200 / 184 registers all fail to launch — measured, "too many
+// resources requested" — and the choice is 8 warps at <= 256 registers or 12 warps at <= 168.)
 __global__ void __maxnreg__(168) k_g1_validate_r168(const uint8_t* __restrict__ keys, uint32_t n, G1Aff* __restrict__ out,
                                                     int32_t* __restrict__ codes) {
     g1_validate_body(keys, n, out, codes);
 }
-// (Occupancies between 8 and 12 warps per SM do not exist for this kernel: the register file is handed out in units of
-// four warps, so 9-, 10- and 11-warp CTAs at 224 / 200 / 184 registers all fail to launch — measured, "too many
-// resources requested" — and the choice is 8 warps at <= 256 registers or 12 warps at <= 168.)
-__global__ void __maxnreg__(128) k_g1_validate_r128(const uint8_t* __restrict__ keys, uint32_t n, G1Aff* __restrict__ out,
-                                                    int32_t* __restrict__ codes) {
-    g1_validate_body(keys, n, out, codes);
-}
-// The default launch of 384-thread CTAs (variant 7): the same 168-register budget split by role, so that both multiply
+// The default launch of 384-thread CTAs: the same 168-register budget split by role, so that both multiply
 // pipes of an SM work on the same keys.  Warps 0-7 run the subgroup checks of the CTA's 256 keys on the integer pipe
 // (g1_in_subgroup_iso, which needs x only); warps 8-11 run their square roots on the FP64 pipe (g1_y_from_x_fpd), two
 // keys per thread, one after the other.  One barrier, then each integer thread merges its key's code in the
@@ -407,11 +392,7 @@ static size_t with_pow_tab(K kernel, unsigned threads) {
 // no pow table: no dynamic shared memory, and the carve-out asks for all of the SM's unified L1 / shared array as L1,
 // where the 168-register kernel's stack frames (384 threads x 280 B at 12 warps per SM) have to stay.
 template <class K>
-static size_t k1_smem(K kernel, unsigned threads) {
-#if defined(B200_G1_CANONICAL_FP)
-    return with_pow_tab(kernel, threads);   // fp_sqrt -> fp_pow
-#else
-    (void)threads;
+static size_t k1_smem(K kernel) {
     static const void* done[4];
     static int n_done = 0;
     const void* key = reinterpret_cast<const void*>(kernel);
@@ -420,30 +401,20 @@ static size_t k1_smem(K kernel, unsigned threads) {
     cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 0);
     if (n_done < 4) done[n_done++] = key;
     return 0;
-#endif
 }
-// tuning knob (B200_G1_VARIANT): 7: 384 threads, 168 registers (default); 0: 256 threads, 224 registers; 6: 512 threads, 128 registers
-static int g_g1_variant = 7;
 static uint32_t g_g1_small_n = 3u * 148u * 384u;   // B200_G1_SMALL_N overrides (0: always 384-thread CTAs)
 void set_g1_small_n(uint32_t n) { g_g1_small_n = n; }
-void set_g1_variant(int v) { if (v >= 0 && v <= 7) g_g1_variant = v; }
 void launch_g1_validate(const uint8_t* keys, uint32_t n, G1Aff* out, int32_t* codes, void* stream, int cta) {
     if (!n) return;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (g_g1_variant) {
-    case 6: k_g1_validate_r128<<<(n + 511) / 512, 512, k1_smem(k_g1_validate_r128, 512), st>>>(keys, n, out, codes); break;
-    case 0: k_g1_validate_main<<<(n + 255) / 256, 256, k1_smem(k_g1_validate_main, 256), st>>>(keys, n, out, codes); break;
-    default:
-        // 12 warps per SM either way; below ~3 full waves of 384-thread CTAs the keys go out as three 128-thread CTAs per
-        // SM of the unsplit kernel, so that the last, partial wave spreads over all SMs instead of leaving most of them
-        // idle; larger launches run the role-split kernel
-        if (cta == 128 || (cta != 384 && n <= g_g1_small_n))
-            k_g1_validate_r168<<<(n + 127) / 128, 128, k1_smem(k_g1_validate_r168, 128), st>>>(keys, n, out, codes);
-        else
-            k_g1_validate_split<<<(n + kSplitIntThreads - 1) / kSplitIntThreads, kSplitThreads,
-                                  k1_smem(k_g1_validate_split, kSplitThreads), st>>>(keys, n, out, codes);
-        break;
-    }
+    // 12 warps per SM either way; below ~3 full waves of 384-thread CTAs the keys go out as three 128-thread CTAs per SM
+    // of the unsplit kernel, so that the last, partial wave spreads over all SMs instead of leaving most of them idle;
+    // larger launches run the role-split kernel
+    if (cta == 128 || (cta != 384 && n <= g_g1_small_n))
+        k_g1_validate_r168<<<(n + 127) / 128, 128, k1_smem(k_g1_validate_r168), st>>>(keys, n, out, codes);
+    else
+        k_g1_validate_split<<<(n + kSplitIntThreads - 1) / kSplitIntThreads, kSplitThreads, k1_smem(k_g1_validate_split),
+                              st>>>(keys, n, out, codes);
 }
 // The registry's key staging from a resident state: the 48-byte public key at the head of each 121-byte Validator record,
 // packed back to back so that K1 reads every key as three 16-byte words.  Records sit at odd byte offsets: byte loads.

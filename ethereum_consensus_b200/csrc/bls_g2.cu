@@ -7,10 +7,6 @@
 // warps per SM, so the only thing that matters is the length of one thread's dependent chain — and at T = 4096 the 3-5 KB
 // stack frames of the earlier build (Fp2 products as calls, 128 registers) overflowed L1.  In strict mode they hide under the
 // per-key kernel either way; in registry mode the step waits for them.
-// -DB200_G2_FP2_CALLS / -DB200_G2_MAXREG=128 restore the earlier build.
-#if defined(B200_G2_FP2_CALLS)
-#define B200_FP2_NOINLINE 1
-#endif
 #define B200_TOWER_NOINLINE 1   // (a build with the curve routines inlined as well returned wrong verdicts on the GPU — not investigated, not offered)
 #include <cuda_runtime.h>
 
@@ -28,11 +24,7 @@ namespace {
 // With Fp2 products as calls, more registers in the caller meant more saves / restores around every product.  Round 2 inlines the Fp2 products and lifts the cap
 // (see the top of this file).
 constexpr int kSmallCta = 32;
-#if !defined(B200_G2_MAXREG)
-#define B200_G2_MAXREG 255
-#endif
-#define B200_G2_BOUNDS __maxnreg__(B200_G2_MAXREG)
-__global__ void B200_G2_BOUNDS k_g2_sig_decode(const uint8_t* __restrict__ sigs, uint32_t n, G2Aff* __restrict__ out,
+__global__ void __maxnreg__(255) k_g2_sig_decode(const uint8_t* __restrict__ sigs, uint32_t n, G2Aff* __restrict__ out,
                                                        int32_t* __restrict__ sig_code) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -52,7 +44,7 @@ __global__ void B200_G2_BOUNDS k_g2_sig_decode(const uint8_t* __restrict__ sigs,
 
 // hash_to_G2 in two launches: the two SSWU maps of a message are independent (2n threads), then one thread per message
 // adds them, clears the cofactor and normalises.
-__global__ void B200_G2_BOUNDS k_hash_to_g2_map(const uint8_t* __restrict__ msgs, const uint32_t* __restrict__ moff,
+__global__ void __maxnreg__(255) k_hash_to_g2_map(const uint8_t* __restrict__ msgs, const uint32_t* __restrict__ moff,
                                                         uint32_t n, G2Jac* __restrict__ tmp) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= 2 * n) return;
@@ -61,7 +53,7 @@ __global__ void B200_G2_BOUNDS k_hash_to_g2_map(const uint8_t* __restrict__ msgs
     hash_to_g2_map(q, msgs + moff[m], size_t(moff[m + 1] - moff[m]), int(i & 1));
     tmp[i] = q;
 }
-__global__ void B200_G2_BOUNDS k_hash_to_g2_finish(const G2Jac* __restrict__ tmp, uint32_t n, G2Aff* __restrict__ out) {
+__global__ void __maxnreg__(255) k_hash_to_g2_finish(const G2Jac* __restrict__ tmp, uint32_t n, G2Aff* __restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const G2Jac q0 = tmp[2 * i], q1 = tmp[2 * i + 1];
@@ -106,7 +98,7 @@ __device__ __forceinline__ void load_cg(G2Jac& q, const G2Jac* p) {
 // precedence over group-check errors (every signature is decoded before any is checked, as blst's aggregate does), else
 // the chunk sums are added, normalised and compressed.  A failed or empty group's 96 bytes are zero.  Every group, empty
 // ones included, has at least one chunk.
-__global__ void B200_G2_BOUNDS k_g2_aggregate(const G2Aff* __restrict__ sigs, const int32_t* __restrict__ sig_code,
+__global__ void __maxnreg__(255) k_g2_aggregate(const G2Aff* __restrict__ sigs, const int32_t* __restrict__ sig_code,
                                               const uint32_t* __restrict__ off, const uint32_t* __restrict__ chunk_group,
                                               const uint32_t* __restrict__ chunk_off, uint32_t n_chunks, uint32_t chunk,
                                               G2Jac* part, int32_t* part_code, uint32_t* done, uint8_t* __restrict__ out96,
@@ -176,7 +168,7 @@ __global__ void B200_G2_BOUNDS k_g2_aggregate(const G2Aff* __restrict__ sigs, co
 
 // Fp2 self-test against big integers (b200_fp_eval): compiled here so that it runs this unit's inlined Fp2 products,
 // register cap and ptxas level
-__global__ void B200_G2_BOUNDS k_fp2_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
+__global__ void __maxnreg__(255) k_fp2_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
                                           uint32_t* __restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -209,7 +201,7 @@ __device__ __forceinline__ void curve2_load(G2Jac& p, const uint32_t* w) {
         p.z.c0.l[k] = w[48 + k]; p.z.c1.l[k] = w[60 + k];
     }
 }
-__global__ void B200_G2_BOUNDS k_curve2_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
+__global__ void __maxnreg__(255) k_curve2_eval(int32_t op, uint32_t n, const uint32_t* __restrict__ a, const uint32_t* __restrict__ b,
                                              uint32_t* __restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;

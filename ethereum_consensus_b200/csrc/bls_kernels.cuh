@@ -21,7 +21,6 @@ enum : uint32_t { TUPLE_FLAG_EMPTY = 1u, TUPLE_FLAG_AGG_INF = 2u };
 enum : int32_t { SIG_OK = 0, SIG_NOT_IN_GROUP = -1 };  // >0: blst decode error code
 
 // K1: key_validate every 48-byte public key -> affine point + blst code
-void set_g1_variant(int v);
 void set_g1_small_n(uint32_t n);
 void set_small_cta(int threads);
 void set_vm_team16_max(uint32_t n);

@@ -2,11 +2,6 @@
 // scheduled Fp2 programs of tools/gen_pairing_vm.py (Miller loop, final exponentiation) on a shared-memory register
 // file.  Replaces the one-thread-per-pair kernels of bls_pairing.cu on the batch path: those expose only 2T threads
 // (a latency floor of tens of ms at T = 4096); here 16x more lanes work on the same tuples, products stay inlined PTX.
-// -DB200_VM_MUL_CALL: field products as by-value function calls (fp.cuh) instead of ~15 inlined copies per kernel
-// (141 KB of straight-line code per VM kernel -> instruction-fetch stalls; see DESIGN.md §4)
-#if defined(B200_VM_MUL_CALL)
-#define B200_FP_MUL_CALL 1
-#endif
 #include <cuda_runtime.h>
 
 #include <algorithm>

@@ -113,7 +113,6 @@ static void read_env(BlsState& s, int* side_prio, int* pair_prio) {
         for (const char* c = k.name; *c; c++) var += char(toupper(static_cast<unsigned char>(*c)));
         if (const char* v = getenv(var.c_str())) k.set(s, atoll(v));
     }
-    if (const char* v = getenv("B200_G1_VARIANT")) set_g1_variant(atoi(v));
     if (const char* v = getenv("B200_G1_SMALL_N")) set_g1_small_n(uint32_t(atol(v)));
     if (const char* v = getenv("B200_PAIRING_VM")) s.use_vm = atoi(v) != 0;
     if (const char* v = getenv("B200_BLS_TRACE")) s.trace = atoi(v) != 0;

@@ -314,9 +314,6 @@ int32_t b200_init(int32_t device) {
     B200_CUDA_TRY(cudaEventCreate(&e.ev1));
     for (auto& ev : e.ev_copy) B200_CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     e.device = device;
-    const char* a = getenv("B200_SSZ_MINB_VALIDATORS");
-    const char* b = getenv("B200_SSZ_MINB_STAGE");
-    set_ssz_tuning(a ? atoi(a) : 0, b ? atoi(b) : 0);
     e.ready = true;
     return ensure_zero_nodes(e);
 }

@@ -64,8 +64,8 @@ B200_HD bool fp_geq_raw(const Fp& a, const Fp& b) {
 // Raw 384-bit add / subtract.  On the device: hardware carry chains (add.cc / addc.cc -> one IADD3.X per limb); the
 // portable 64-bit emulation below compiles to THREE dependent instructions per limb (IADD3 + IADD3.X + LOP3, several of them
 // IMAD.X / IMAD.IADD on the FMA pipe the products need), which made a plain Fp2 addition ~150 SASS instructions in the
-// pairing VM's light rounds.  -DB200_FP_ADD_PORTABLE restores the emulation on the device (A/B).  Outputs may alias inputs:
-// asm operands are distinct PTX virtual registers.
+// pairing VM's light rounds.  The emulation stays the host's code and the device self-test's reference.  Outputs may
+// alias inputs: asm operands are distinct PTX virtual registers.
 B200_HD uint32_t fp_sub_raw_portable(Fp& r, const Fp& a, const Fp& b) {
     uint64_t borrow = 0;
 #pragma unroll
@@ -86,8 +86,7 @@ B200_HD uint32_t fp_add_raw_portable(Fp& r, const Fp& a, const Fp& b) {
     }
     return uint32_t(carry);
 }
-#if defined(__CUDA_ARCH__) && !defined(B200_FP_PORTABLE) && !defined(B200_FP_ADD_PORTABLE)
-#define B200_FP_ADD_PTX 1
+#if defined(__CUDA_ARCH__)
 // r = a - b (mod 2^384), returns the borrow (0 / 1)
 __device__ __forceinline__ uint32_t fp_sub_raw(Fp& r, const Fp& a, const Fp& b) {
     uint32_t c;
@@ -249,7 +248,7 @@ namespace b200 {
 // B200_FP_MUL_CALL: emit them as real functions taking/returning Fp BY VALUE — the ABI keeps all 36 limbs in
 // registers (0-byte stack frame), so a call costs ~40 register moves but every warp of the kernel shares one ~13 KB
 // instruction footprint instead of hundreds of inlined copies (the per-key kernel was instruction-fetch limited).
-#if defined(__CUDA_ARCH__) && !defined(B200_FP_PORTABLE)
+#if defined(__CUDA_ARCH__)
 #if defined(B200_FP_MUL_CALL)
 static __device__ __noinline__ Fp fp_mul_call(Fp a, Fp b) {
     Fp out;
@@ -259,11 +258,7 @@ static __device__ __noinline__ Fp fp_mul_call(Fp a, Fp b) {
 }
 static __device__ __noinline__ Fp fp_sqr_call(Fp a) {
     Fp out;
-#if defined(B200_FP_SQR_VIA_MUL)
-    fp_mul_ptx_core(out.l, a.l, a.l);
-#else
     fp_sqr_ptx_core(out.l, a.l);   // dedicated square: 222 wide multiply-adds instead of 288
-#endif
     fp_reduce_once(out);
     return out;
 }
@@ -278,11 +273,7 @@ B200_HD void fp_mul(Fp& r, const Fp& a, const Fp& b) {
 }
 B200_HD void fp_sqr(Fp& r, const Fp& a) {
     Fp out;
-#if defined(B200_FP_SQR_VIA_MUL)
-    fp_mul_ptx_core(out.l, a.l, a.l);
-#else
     fp_sqr_ptx_core(out.l, a.l);
-#endif
     fp_reduce_once(out);
     r = out;
 }
@@ -489,9 +480,9 @@ B200_HD void fp_inv_kaliski(Fp& out, const Fp& a) {
     const Fp r2 = B200_FP_R2;
     fp_mul(out, tt, r2);                              // y 2^j
 }
-// Device: Kaliski (-DB200_FP_INV_FERMAT restores the exponentiation); host: the exponentiation (reference for the tests)
+// Device: Kaliski; host: the exponentiation (reference for the tests)
 B200_HD void fp_inv(Fp& r, const Fp& a) {
-#if defined(__CUDA_ARCH__) && !defined(B200_FP_INV_FERMAT)
+#if defined(__CUDA_ARCH__)
     fp_inv_kaliski(r, a);
 #else
     fp_inv_fermat(r, a);

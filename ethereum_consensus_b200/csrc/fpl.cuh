@@ -47,25 +47,17 @@ B200_HD void f_neg(FpL& r, const FpL& a) {
     f_sub(r, z, a);   // 0 -> 0, otherwise 2p - a in (0, 2p)
 }
 #if defined(__CUDA_ARCH__) && defined(B200_FP_MUL_CALL)
-// A/B knob (-DB200_G1_CALL_MUL): the two products as real functions, operands and result by value in registers — one
+// B200_FP_MUL_CALL (fp.cuh): the two products as real functions, operands and result by value in registers — one
 // ~4 KB copy of each instead of ~70 inlined copies (the per-key kernel is 0.5 MB of straight-line code otherwise)
 static __device__ __noinline__ Fp fpl_mul_call(Fp a, Fp b) { Fp out; fp_mul_ptx_core(out.l, a.l, b.l); return out; }
-static __device__ __noinline__ Fp fpl_sqr_call(Fp a) {
-    Fp out;
-#if defined(B200_FP_SQR_VIA_MUL)
-    fp_mul_ptx_core(out.l, a.l, a.l);
-#else
-    fp_sqr_ptx_core(out.l, a.l);
-#endif
-    return out;
-}
+static __device__ __noinline__ Fp fpl_sqr_call(Fp a) { Fp out; fp_sqr_ptx_core(out.l, a.l); return out; }
 #endif
 // products without the final conditional subtraction: [0, 2p) x [0, 2p) -> [0, 1.41 p)
 B200_HD void f_mul(FpL& r, const FpL& a, const FpL& b) {
     Fp out;
 #if defined(__CUDA_ARCH__) && defined(B200_FP_MUL_CALL)
     out = fpl_mul_call(a.v, b.v);
-#elif defined(__CUDA_ARCH__) && !defined(B200_FP_PORTABLE)
+#elif defined(__CUDA_ARCH__)
     fp_mul_ptx_core(out.l, a.v.l, b.v.l);
 #else
     fp_mul_emul_core(out.l, a.v.l, b.v.l);   // host: the C emulation of the very same instruction list
@@ -76,18 +68,10 @@ B200_HD void f_sqr(FpL& r, const FpL& a) {
     Fp out;
 #if defined(__CUDA_ARCH__) && defined(B200_FP_MUL_CALL)
     out = fpl_sqr_call(a.v);
-#elif defined(__CUDA_ARCH__) && !defined(B200_FP_PORTABLE)
-#if defined(B200_FP_SQR_VIA_MUL)
-    fp_mul_ptx_core(out.l, a.v.l, a.v.l);
-#else
+#elif defined(__CUDA_ARCH__)
     fp_sqr_ptx_core(out.l, a.v.l);
-#endif
-#else
-#if defined(B200_FP_SQR_VIA_MUL)
-    fp_mul_emul_core(out.l, a.v.l, a.v.l);
 #else
     fp_sqr_emul_core(out.l, a.v.l);
-#endif
 #endif
     r.v = out;
 }
@@ -113,7 +97,7 @@ B200_HD void fpl_reduce_4p(Fp& r) {
 B200_HD Fp fpl_mul_sub_mul_core(const Fp& a, const Fp& b, const Fp& c, const Fp& d) {
     Fp nd, out;
     fp_sub_raw(nd, fp_2p(), d);
-#if defined(__CUDA_ARCH__) && !defined(B200_FP_PORTABLE)
+#if defined(__CUDA_ARCH__)
     fp_mul_add_mul_ptx_core(out.l, a.l, b.l, c.l, nd.l);
 #else
     fp_mul_add_mul_emul_core(out.l, a.l, b.l, c.l, nd.l);
@@ -122,7 +106,7 @@ B200_HD Fp fpl_mul_sub_mul_core(const Fp& a, const Fp& b, const Fp& c, const Fp&
 }
 B200_HD Fp fpl_mul_sub_8sqr_core(const Fp& a, const Fp& b, const Fp& c) {
     Fp out;
-#if defined(__CUDA_ARCH__) && !defined(B200_FP_PORTABLE)
+#if defined(__CUDA_ARCH__)
     fp_mul_sub_8sqr_ptx_core(out.l, a.l, b.l, c.l);
 #else
     fp_mul_sub_8sqr_emul_core(out.l, a.l, b.l, c.l);

@@ -56,20 +56,7 @@ B200_HD int32_t g1_uncompress(G1Aff& out, const uint8_t b[48]) {
     return BLS_SUCCESS;
 }
 
-// phi(P) == -[z^2]P  (Scott 2021; beta chosen by tools/gen_bls_consts.py so that this holds on G1)
-B200_HD bool g1_in_subgroup(const G1Aff& p) {
-    if (p.inf) return true;
-    G1Jac t, t2;
-    jac_mul_u64(t, p.x, p.y, B200_Z_ABS);
-    jac_mul_u64_jac(t2, t, B200_Z_ABS);
-    const Fp beta = B200_FP_BETA;
-    Fp bx, ny;
-    fp_mul(bx, p.x, beta);
-    fp_neg(ny, p.y);
-    return jac_eq_aff(t2, bx, ny);
-}
-
-// ---- the same two steps on lazily reduced field elements (fpl.cuh): what the per-key kernel runs ----------------
+// ---- decompression and subgroup check on lazily reduced field elements (fpl.cuh): what the per-key kernel runs ------
 // decompression: identical checks and codes as g1_uncompress; y = (x^3 + 4)^((p+1)/4) with no reduction inside the chain,
 // a fixed addition chain whose temporaries are registers (no pow table: the kernel's L1 stays free for its stack)
 B200_HD int32_t g1_uncompress_lazy(G1Aff& out, const uint8_t b[48]) {
@@ -94,7 +81,8 @@ B200_HD int32_t g1_uncompress_lazy(G1Aff& out, const uint8_t b[48]) {
     out.x = x; out.y = y;
     return BLS_SUCCESS;
 }
-// phi(P) == -[z^2]P on FpL (the templated Jacobian formulas of curve.cuh, every intermediate in [0, 2p))
+// phi(P) == -[z^2]P (Scott 2021; beta chosen by tools/gen_bls_consts.py so that this holds on G1), on FpL (the
+// templated Jacobian formulas of curve.cuh, every intermediate in [0, 2p))
 B200_HD bool g1_in_subgroup_lazy(const G1Aff& p) {
     if (p.inf) return true;
     const FpL px = fpl_from_fp(p.x), py = fpl_from_fp(p.y);
@@ -153,19 +141,12 @@ B200_HD int32_t g1_key_validate_code(int32_t parse_rc, uint32_t inf, bool on_cur
     return in_group ? BLS_SUCCESS : BLS_POINT_NOT_IN_GROUP;
 }
 
-// blst `PublicKey::key_validate`.  -DB200_G1_CANONICAL_FP selects the fully reduced arithmetic (round 1's path).
+// blst `PublicKey::key_validate`
 B200_HD int32_t g1_key_validate(G1Aff& out, const uint8_t b[48]) {
-#if defined(B200_G1_CANONICAL_FP)
-    int32_t rc = g1_uncompress(out, b);
-    if (rc) return rc;
-    if (out.inf) return BLS_PK_IS_INFINITY;
-    if (!g1_in_subgroup(out)) return BLS_POINT_NOT_IN_GROUP;
-#else
     int32_t rc = g1_uncompress_lazy(out, b);
     if (rc) return rc;
     if (out.inf) return BLS_PK_IS_INFINITY;
     if (!g1_in_subgroup_lazy(out)) return BLS_POINT_NOT_IN_GROUP;
-#endif
     return BLS_SUCCESS;
 }
 

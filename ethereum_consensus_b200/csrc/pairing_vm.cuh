@@ -11,35 +11,26 @@ namespace b200 {
 
 enum VmOp : uint32_t { VM_NOP = 0, VM_MUL, VM_SQR, VM_MULFP, VM_INV, VM_ADD, VM_SUB, VM_NEG, VM_DBL, VM_CONJ, VM_MULXI, VM_COPY, VM_LDC };
 
-// register-file accessors: dense array of Fp2 (host) or 25-word-strided shared memory (device, bank-conflict free)
+// register-file accessors: dense array of Fp2 (host) or 28-word-strided shared memory (device)
 struct VmRfDense {
     Fp2* p;
     B200_HD Fp2 load(uint32_t i) const { return p[i]; }
     B200_HD void store(uint32_t i, const Fp2& v) const { p[i] = v; }
 };
-// Slot stride in words.  28 (default) / 24: 16-byte aligned slots moved with 128-bit LDS/STS; 25 (round 1, -DB200_VM_SLOT_WORDS=25):
-// scalar LDS/STS, conflict-free for any slot pattern.  28 had the shortest Miller loop and final exponentiation of the three.
-// 16-byte aligned slots moved with 128-bit LDS/STS — 6 + 6 + 6 wide accesses per light op instead of 24 + 24 + 24.
-#if !defined(B200_VM_SLOT_WORDS)
-#define B200_VM_SLOT_WORDS 28
-#endif
-constexpr int kVmSlotWords = B200_VM_SLOT_WORDS;
-// -DB200_VM_SLOT_PAD4 (A/B): 24-word slots with 16 bytes of padding after every fourth (100 B per slot on average instead of 112):
-// any 8 consecutive slots still fall into 8 different 16-byte bank groups, and 12 % more teams fit an SM.
-#if defined(B200_VM_SLOT_PAD4)
-B200_HD constexpr uint32_t vm_slot_word(uint32_t i) { return i * 24u + (i >> 2) * 4u; }
-B200_HD constexpr uint32_t vm_team_words(uint32_t n_slots) { return n_slots * 24u + ((n_slots + 3u) >> 2) * 4u; }
-#else
+// Slot stride in words: 16-byte aligned slots moved with 128-bit LDS/STS — 6 + 6 + 6 wide accesses per light op instead
+// of 24 + 24 + 24.  Of the strides 24 and 28 (128-bit accesses) and 25 (scalar accesses, conflict-free for any slot
+// pattern), 28 had the shortest Miller loop and final exponentiation.
+constexpr int kVmSlotWords = 28;
+static_assert(kVmSlotWords % 4 == 0, "slots are moved as 16-byte words");
 B200_HD constexpr uint32_t vm_slot_word(uint32_t i) { return i * uint32_t(kVmSlotWords); }
 B200_HD constexpr uint32_t vm_team_words(uint32_t n_slots) { return n_slots * uint32_t(kVmSlotWords); }
-#endif
 constexpr int kVmMaxSmemBytes = 227 * 1024;          // opt-in dynamic shared memory per CTA on sm_90 (H100)
 constexpr uint32_t kVmBlobMagic = 0xB200564Du;       // run-time program blobs (vm_load_programs)
 struct VmRfStrided {
     uint32_t* p;
     B200_HD Fp2 load(uint32_t i) const {
         Fp2 v;
-#if defined(__CUDA_ARCH__) && (B200_VM_SLOT_WORDS % 4 == 0)
+#if defined(__CUDA_ARCH__)
         const uint4* q = reinterpret_cast<const uint4*>(p + vm_slot_word(i));
 #pragma unroll
         for (int k = 0; k < 3; k++) {
@@ -55,7 +46,7 @@ struct VmRfStrided {
         return v;
     }
     B200_HD void store(uint32_t i, const Fp2& v) const {
-#if defined(__CUDA_ARCH__) && (B200_VM_SLOT_WORDS % 4 == 0)
+#if defined(__CUDA_ARCH__)
         uint4* q = reinterpret_cast<uint4*>(p + vm_slot_word(i));
 #pragma unroll
         for (int k = 0; k < 3; k++) {

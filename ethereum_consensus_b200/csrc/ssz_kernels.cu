@@ -104,8 +104,7 @@ __device__ __forceinline__ void validator_root(const uint32_t* smem, uint32_t ba
     hash_pair_words(ab, x, root);
 }
 
-template <int MINB>
-__global__ void __launch_bounds__(kStageThreads, MINB) k_validator_roots(const __grid_constant__ Job jb) {
+__global__ void __launch_bounds__(kStageThreads, 4) k_validator_roots(const __grid_constant__ Job jb) {
     __shared__ __align__(16) uint32_t smem[(kStageThreads * 121 + 16) / 4 + 4];
     const uint32_t blk = blockIdx.x;
     // stage 256 x 121 B (30 976 B, a multiple of 16) with coalesced 16-byte loads
@@ -123,8 +122,7 @@ __global__ void __launch_bounds__(kStageThreads, MINB) k_validator_roots(const _
     store_node(jb.dst + (first + threadIdx.x) * 8, root);
 }
 
-template <int MINB>
-__global__ void __launch_bounds__(kStageThreads, MINB) k_merkle_stage(const __grid_constant__ StageDesc sd) {
+__global__ void __launch_bounds__(kStageThreads, 4) k_merkle_stage(const __grid_constant__ StageDesc sd) {
     // locate this block's job (njobs is small; block_begin ascending)
     int j = 0;
 #pragma unroll 1
@@ -333,33 +331,15 @@ __global__ void __launch_bounds__(kFinisherThreads) k_merkle_finisher(uint32_t* 
 
 }  // namespace
 
-// occupancy knobs (registers per thread vs resident warps); set once from B200_SSZ_MINB_{VALIDATORS,STAGE}
-int g_minb_validators = 4;
-int g_minb_stage = 4;
-void set_ssz_tuning(int minb_validators, int minb_stage) {
-    if (minb_validators >= 2 && minb_validators <= 4) g_minb_validators = minb_validators;
-    if (minb_stage >= 2 && minb_stage <= 4) g_minb_stage = minb_stage;
-}
-
 void launch_validators(const Job& jb, void* stream) {
     if (jb.n_in == 0) return;
     const uint32_t nblocks = uint32_t((jb.n_in + kStageThreads - 1) / kStageThreads);
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (g_minb_validators) {
-    case 2: k_validator_roots<2><<<nblocks, kStageThreads, 0, st>>>(jb); break;
-    case 4: k_validator_roots<4><<<nblocks, kStageThreads, 0, st>>>(jb); break;
-    default: k_validator_roots<3><<<nblocks, kStageThreads, 0, st>>>(jb); break;
-    }
+    k_validator_roots<<<nblocks, kStageThreads, 0, static_cast<cudaStream_t>(stream)>>>(jb);
 }
 
 void launch_stage(const StageDesc& sd, void* stream) {
     if (sd.nblocks == 0) return;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (g_minb_stage) {
-    case 2: k_merkle_stage<2><<<sd.nblocks, kStageThreads, 0, st>>>(sd); break;
-    case 4: k_merkle_stage<4><<<sd.nblocks, kStageThreads, 0, st>>>(sd); break;
-    default: k_merkle_stage<3><<<sd.nblocks, kStageThreads, 0, st>>>(sd); break;
-    }
+    k_merkle_stage<<<sd.nblocks, kStageThreads, 0, static_cast<cudaStream_t>(stream)>>>(sd);
 }
 
 void launch_coop(const CoopDesc& cd, void* stream) {

@@ -80,7 +80,6 @@ enum FinKind : uint32_t { FIN_HASH = 0, FIN_COPY = 1 };
 constexpr int kFinisherThreads = 1024;
 constexpr int kMaxWaves = 256;
 
-void set_ssz_tuning(int minb_validators, int minb_stage);
 void launch_validators(const Job& jb, void* stream);
 void launch_stage(const StageDesc& sd, void* stream);
 // dirty-path variants: thread t handles output sel[t] (JOB_VALIDATORS or JOB_REDUCE only)

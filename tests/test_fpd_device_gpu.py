@@ -472,7 +472,7 @@ def test_split_slots_small_calls_in_child_process(oracle_bls_c, tmp_path):
     want_pairs(oracle_bls_c, D, CHILD_NS)
     path = tmp_path / "pool.pkl"
     path.write_bytes(pickle.dumps(D))
-    env = dict(os.environ, B200_G1_VARIANT="7", B200_G1_SMALL_N="0")
+    env = dict(os.environ, B200_G1_SMALL_N="0")
     p = subprocess.Popen([sys.executable, "-m", "tests.test_fpd_device_gpu", str(path)], cwd=str(ROOT), env=env,
                          stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     try:

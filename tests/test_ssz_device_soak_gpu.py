@@ -6,8 +6,8 @@ Sections: a. merkleize / packed / Validator lists at the planner's boundary size
 0..300; b. whole-state roots (one-shot, resident, shard_roots + combine_roots for world 1..64); c. incremental update
 scripts on resident states; d. malformed encodings on every entry point; e. shuffling and active indices, also on a
 resident state whose validators changed; f. two resident handles of different presets updated alternately, with one-shot
-calls in between.  B200_SSZ_FOLD, B200_SSZ_MINB_VALIDATORS and B200_SSZ_MINB_STAGE are read once per process, so
-sections a, b, c and f run again in one child process per setting.  The cases come from tests/ssz_soak_cases.py.
+calls in between.  B200_SSZ_FOLD is read once per process, so sections a, b, c and f run again in a child process
+with it off.  The cases come from tests/ssz_soak_cases.py.
 
     B200_SOAK_SCALE=1 (default) python -m pytest tests/test_ssz_device_soak_gpu.py -m gpu -s
 """
@@ -34,8 +34,7 @@ from tests import ssz_soak_cases as sc  # noqa: E402
 pytestmark = pytest.mark.gpu
 NT = os.cpu_count() or 1
 WORLDS = [1, 2, 4, 8, 16, 32, 64]
-ENV_VARIANTS = [{"B200_SSZ_FOLD": "0"}, {"B200_SSZ_MINB_VALIDATORS": "2"}, {"B200_SSZ_MINB_VALIDATORS": "3"},
-                {"B200_SSZ_MINB_STAGE": "2"}, {"B200_SSZ_MINB_STAGE": "3"}]
+ENV_VARIANTS = [{"B200_SSZ_FOLD": "0"}]
 REJECT = "reject"
 
 
@@ -439,9 +438,8 @@ def test_e_shuffling_and_active_indices(engine, oracle_ssz_c):
 
 @pytest.mark.parametrize("env", ENV_VARIANTS, ids=lambda e: "-".join(f"{k[5:].lower()}_{v}" for k, v in e.items()))
 def test_env_variants_in_child_processes(oracle_ssz_c, tmp_path, env):
-    """Sections a, b, c and f with the fold into k_merkle_coop off, or with the register-capped k_validator_roots<2|3> /
-    k_merkle_stage<2|3>, which only the environment selects (read once per process): one child process per setting,
-    oracle roots from here."""
+    """Sections a, b, c and f with the fold into k_merkle_coop off, which only the environment selects (read once per
+    process): one child process per setting, oracle roots from here."""
     t = time.time()
     path = tmp_path / "wants.pkl"
     path.write_bytes(pickle.dumps(wants(oracle_ssz_c)))

@@ -20,7 +20,7 @@ for line in sass.splitlines():
         counts[cur][m.group(1).split(".")[0]] += 1
 ALU = {"LOP3", "SHF", "IADD3", "IADD", "PRMT", "VIADD", "LEA", "IMAD", "MOV", "SEL"}
 for fn, c in counts.items():
-    if "k_validator_rootsILi4" not in fn:
+    if "17k_validator_rootsE" not in fn:   # the dense kernel, not k_validator_roots_sparse
         continue
     alu = sum(v for k, v in c.items() if k in ALU)
     core = sum(v for k, v in c.items() if k in ("LOP3", "SHF", "IADD3", "VIADD", "IADD"))

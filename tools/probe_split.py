@@ -28,5 +28,5 @@ for split, first_cta, small_cta in CONFIGS:
         assert got.tolist() == want
         if i >= 2:
             dev.append(crypto.last_kernel_ms()); wall.append(dt)
-    print(f"T={T} K={K} G1_VARIANT={os.environ.get('B200_G1_VARIANT', 'default')} key_split={split} k1_first_cta={first_cta} small_cta={small_cta or 'auto'}: device {min(dev):.2f} ms | end-to-end wall {min(wall):.2f} ms "
+    print(f"T={T} K={K} key_split={split} k1_first_cta={first_cta} small_cta={small_cta or 'auto'}: device {min(dev):.2f} ms | end-to-end wall {min(wall):.2f} ms "
           f"(median {sorted(wall)[len(wall)//2]:.2f}) | per-key kernels {crypto.last_dominant_kernel_ms():.2f} ms", flush=True)
