@@ -226,7 +226,9 @@ def h2c_data(O):
 
 def _shapes():
     """Multisets of key indices (index, sign) that make equal or opposite points meet in k_g1_aggregate's lanes (lane j sums
-    positions j, j + 32, ...) and in its 5-level tree (level s adds lane j + s into lane j), and in k_g2_sum_compress."""
+    positions j, j + 32, ...) and in its 5-level tree (level s adds lane j + s into lane j), and in k_g2_aggregate: these
+    groups are far below 256 x SMs signatures, so its chunks are 32 signatures (one per lane) and the points meet in a
+    chunk's butterfly (round s adds lane j ^ s into lane j) and in the finisher's sum of the chunk partials."""
     out = []
     for K in (2, 32, 33, 64, 512, 2048):
         out.append((f"[P] * {K}", [(7, 1)] * K))
