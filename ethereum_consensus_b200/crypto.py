@@ -461,7 +461,9 @@ def pairing_eval(op: str, a, b=None) -> np.ndarray:
 
 
 def tune(knob: str, value: int) -> None:
-    """Launch-shape knobs of the batch pipeline (include/b200_consensus.h, b200_tune): never change a result."""
+    """Launch-shape knobs of the batch pipeline (include/b200_consensus.h, b200_tune): never change a result.
+
+    The knobs are "bls_small_cta", "vm_team16_max" and "vm_cta"; any other name raises EngineError (B200_ERR_BAD_ARG)."""
     _lib.check(_lib.lib().b200_tune(knob.encode(), int(value)), f"tune({knob})")
 
 

@@ -187,19 +187,17 @@ __global__ void k_g1_compress_groups(const G1Aff* __restrict__ agg, const int32_
     if (rc == BLS_SUCCESS) g1_compress(o, agg[g]);
     else for (int k = 0; k < 48; k++) o[k] = 0;
 }
-// aggregate_verify batches: one thread per key of the call, its pair's G1 operand (launch_g1_pair_operands).  Keys that
-// failed validation are converted as well; their tuples are dead and no pairing kernel reads them.
+// aggregate_verify batches: one thread per key of the call, its pair's G1 operand for the pairing VM
+// (launch_g1_pair_operands).  Keys that failed validation are converted as well; their tuples are dead and no pairing
+// kernel reads them.
 __global__ void k_g1_pair_operands(const G1Aff* __restrict__ keys, const uint32_t* __restrict__ index, uint32_t n,
-                                   G1Pre* __restrict__ pre, G1Aff* __restrict__ aff) {
+                                   G1Pre* __restrict__ pre) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const G1Aff a = keys[index ? index[i] : i];
-    if (pre) {
-        G1Pre p;
-        p.xz = a.x; p.y = a.y; p.z3 = fp_one(); p.inf = a.inf;
-        pre[i] = p;
-    }
-    if (aff) aff[i] = a;
+    G1Pre p;
+    p.xz = a.x; p.y = a.y; p.z3 = fp_one(); p.inf = a.inf;
+    pre[i] = p;
 }
 __global__ void k_neg_g1(G1Aff* out, G1Pre* out_pre) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -443,9 +441,9 @@ void launch_g1_aggregate(const G1Aff* keys, const int32_t* key_codes, const uint
                      static_cast<cudaStream_t>(stream)>>>(
         keys, key_codes, index, off, n_tuples, agg, agg_pre, pk_code, flags, extra_flags, agg_jac, tuple_flags);
 }
-void launch_g1_pair_operands(const G1Aff* keys, const uint32_t* index, uint32_t n, G1Pre* pre, G1Aff* aff, void* stream) {
+void launch_g1_pair_operands(const G1Aff* keys, const uint32_t* index, uint32_t n, G1Pre* pre, void* stream) {
     if (!n) return;
-    k_g1_pair_operands<<<(n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(keys, index, n, pre, aff);
+    k_g1_pair_operands<<<(n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(keys, index, n, pre);
 }
 void launch_g1_compress_groups(const G1Aff* agg, const int32_t* pk_code, const uint32_t* flags, uint32_t n_groups, uint8_t* out48,
                                int32_t* out_code, void* stream) {

@@ -245,8 +245,8 @@ __global__ void __maxnreg__(255) k_curve2_eval(int32_t op, uint32_t n, const uin
 }  // namespace
 
 constexpr size_t kPowTab = 0;  // thread-local table here (see above)
-// CTA size of the signature / message kernels: 32 spreads them over all SMs (lowest latency when they run alone, before
-// the per-key kernel); larger CTAs pack them onto few SMs for runs UNDER the per-key kernel (B200_SMALL_ORDER=0)
+// CTA size of the signature / message kernels: 32 spreads them over all SMs (lowest latency when they run alone, without
+// a per-key kernel); larger CTAs pack them onto few SMs for runs UNDER the per-key kernel
 static int g_small_cta = kSmallCta;
 void set_small_cta(int threads) { if (threads >= 32 && threads <= 512 && threads % 32 == 0) g_small_cta = threads; }
 

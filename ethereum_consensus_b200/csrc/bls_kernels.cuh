@@ -40,8 +40,8 @@ void launch_g1_aggregate(const G1Aff* keys, const int32_t* key_codes, const uint
                          uint32_t n_tuples, G1Aff* agg, G1Pre* agg_pre, int32_t* pk_code, uint32_t* flags,
                          uint32_t extra_flags, void* stream, G1Jac* agg_jac = nullptr, const uint32_t* tuple_flags = nullptr);
 // aggregate_verify batches: the G1 operand of key i's pair, keys[i] (or keys[index[i]] when index is non-null), as the VM
-// Miller kernel's G1Pre (x, y, 1) into pre[i] and / or as the affine point into aff[i] (either may be null)
-void launch_g1_pair_operands(const G1Aff* keys, const uint32_t* index, uint32_t n, G1Pre* pre, G1Aff* aff, void* stream);
+// Miller kernel's G1Pre (x, y, 1) into pre[i]
+void launch_g1_pair_operands(const G1Aff* keys, const uint32_t* index, uint32_t n, G1Pre* pre, void* stream);
 // RLC whole-batch check (bls_rlc.cu): scale per tuple, fold 32 -> 1 per launch, sum -> affine
 void launch_rlc_scale(const G1Jac* agg, const G2Aff* sig, const int32_t* pk_code, const uint32_t* flags, const int32_t* sig_code,
                       const uint32_t* seed_words, uint64_t t0, uint32_t n, G1Pre* out_g1, G2Jac* out_g2, int32_t* bad, void* stream);

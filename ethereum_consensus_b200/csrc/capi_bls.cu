@@ -13,9 +13,9 @@
 // Every entry point describes its work as one Batch; run_verify() runs it through these phases, in this order:
 //   reserve_buffers  grow-only device buffers
 //   stage_small      the small index arrays, built on the host, one pinned copy to the device (stream A)
-//   key_phase        the key copy and K1, and where K3 / K4 go: one key range (keys_one_range, with the split key copy of
-//                    big strict batches) or several (keys_chunked, which also queues each range's K2 -> K5 -> K6)
-//   pairing_tail     K5 / K6 per tuple: lane-parallel VM or one thread per pair   | or rlc_tail: the whole-batch check
+//   key_phase        the key copy and K1 (two launches when big strict batches split the key copy), K3 / K4 right behind
+//                    K1's first launch, K2
+//   pairing_tail     K5 / K6 per tuple                                          | or rlc_tail: the whole-batch check
 //   readback         verdicts to the host, event times; then the B200_BLS_TRACE line
 #include <algorithm>
 #include <cctype>
@@ -35,22 +35,8 @@ namespace b200 {
 
 struct BlsState {
     cudaStream_t sb = nullptr, sc = nullptr;  // signatures / messages: run under the per-key kernel
-    // Chunked strict batches (OFF by default): the per-key kernel goes out in `chunks` key ranges on the engine stream, and
-    // each range's aggregate -> Miller loops -> final exponentiation chain runs on `sd` UNDER the next range's per-key
-    // kernel (B200_BLS_CHUNKS, 1 = one range; B200_BLS_CHUNK_MIN_TUPLES; B200_BLS_CHUNK_K1_CTA = 128 | 384).
-    // At T = 4096 x K = 512 every extra range made the step slower.  The pairing chain does not fit under the per-key
-    // kernel: its CTAs need the registers / shared memory of a retiring per-key CTA, both kernels then run at reduced
-    // occupancy, and the per-key kernel loses more than the chain it hides.
-    static constexpr uint32_t kMaxChunks = 16;
-    cudaStream_t sd = nullptr, se = nullptr;   // se: odd key ranges, so that range c+1's CTAs fill range c's draining tail
-    cudaEvent_t ev_ck[kMaxChunks] = {nullptr}, ev_join = nullptr;
-    uint32_t chunks = 1, chunk_min_tuples = 2048;
-    int chunk_k1_cta = 128;
-    bool chunk_alt = true;
-    bool key_split = true;   // B200_BLS_KEY_SPLIT / b200_tune("bls_key_split")
-    // CTA size of the first (4-wave) per-key launch of a split batch, the one the signature / message kernels run under: as three
-    // 128-thread CTAs per SM a side kernel's CTA displaces a third of an SM's per-key work instead of all of it
-    int k1_first_cta = 128;
+    cudaStream_t se = nullptr;   // split key copy: the second part of the keys and their per-key launch (ev_e: done)
+    cudaEvent_t ev_e = nullptr;
     cudaEvent_t ev_in = nullptr, ev_b = nullptr, ev_c = nullptr, ev_k0 = nullptr, ev_k1 = nullptr, ev_d0 = nullptr, ev_d1 = nullptr;
     DevBuf keys, key_aff, key_code, g1pts, g1pre, pk_code, flags, sigs, g2pts, sig_code, msgs, small, f, out, h2c_tmp, gath;
     // RLC whole-batch check (bls_rlc.cu): Jacobian aggregates, scaled points, reduction ping-pong, zeros, indices, exchange
@@ -68,20 +54,16 @@ struct BlsState {
     float last_dominant_ms = 0.f;
     bool trace = false;          // B200_BLS_TRACE=1: per-phase CUDA-event timings on stderr
     cudaEvent_t ev_t[8] = {nullptr};
-    // B200_SMALL_ORDER: where the signature / message kernels go relative to the per-key kernel K1: 0 (default) under it on
-    // high-priority streams, 1 before it, 2 after it.  With the call-based
-    // per-key kernel (a fifth of the code, 12 warps/SM) the overlap beats running them first, with 128-thread CTAs at
+    // The signature / message kernels run under the per-key kernel K1 on high-priority streams.  With the call-based per-key
+    // kernel (a fifth of the code, 12 warps/SM) that overlap beats running them before K1, with 128-thread CTAs at
     // T = 4096 and 32-thread CTAs at T = 256.  B200_BLS_SMALL_CTA overrides the CTA size (default: 32 up to 1 024 tuples, else 128).
-    int small_order = 0;
     int small_cta_override = 0;
-    bool use_vm = true;  // lane-parallel pairing kernels (B200_PAIRING_VM=0 selects the one-thread-per-pair kernels)
 
     // only a bls_state() that fails part-way destroys one: a completed state lives as long as the process
     ~BlsState() {
-        for (cudaStream_t st : {sb, sc, sd, se}) if (st) cudaStreamDestroy(st);
-        for (cudaEvent_t ev : ev_ck) if (ev) cudaEventDestroy(ev);
+        for (cudaStream_t st : {sb, sc, se}) if (st) cudaStreamDestroy(st);
         for (cudaEvent_t ev : ev_t) if (ev) cudaEventDestroy(ev);
-        for (cudaEvent_t ev : {ev_join, ev_in, ev_b, ev_c, ev_k0, ev_k1, ev_d0, ev_d1}) if (ev) cudaEventDestroy(ev);
+        for (cudaEvent_t ev : {ev_e, ev_in, ev_b, ev_c, ev_k0, ev_k1, ev_d0, ev_d1}) if (ev) cudaEventDestroy(ev);
         cudaFree(d_negg1);
         cudaFree(d_negg1_pre);
     }
@@ -94,48 +76,35 @@ struct Knob {
     void (*set)(BlsState&, int64_t);
 };
 static const Knob kKnobs[] = {
-    {"bls_chunks", [](BlsState& s, int64_t v) { s.chunks = uint32_t(std::max<int64_t>(1, v)); }},
-    {"bls_chunk_min_tuples", [](BlsState& s, int64_t v) { s.chunk_min_tuples = uint32_t(std::max<int64_t>(2, v)); }},
-    {"bls_chunk_k1_cta", [](BlsState& s, int64_t v) { s.chunk_k1_cta = int(v); }},
-    {"bls_chunk_alt", [](BlsState& s, int64_t v) { s.chunk_alt = v != 0; }},
-    {"bls_key_split", [](BlsState& s, int64_t v) { s.key_split = v != 0; }},
-    {"bls_k1_first_cta", [](BlsState& s, int64_t v) { s.k1_first_cta = (v == 128) ? 128 : 384; }},
     {"bls_small_cta", [](BlsState& s, int64_t v) { s.small_cta_override = int(v); }},
     {"vm_team16_max", [](BlsState&, int64_t v) { set_vm_team16_max(uint32_t(std::max<int64_t>(0, v))); }},
     {"vm_cta", [](BlsState&, int64_t v) { set_vm_cta(int(v)); }},
 };
 
-// The knobs' environment variables, then the settings b200_tune does not take: kernel variants, the pairing kernels,
-// tracing, the side kernels' order and the streams' priorities are fixed for the process at first use.
-static void read_env(BlsState& s, int* side_prio, int* pair_prio) {
+// The knobs' environment variables, then the settings b200_tune does not take: the per-key launch size up to which
+// k_g1_validate goes out as 128-thread CTAs, and tracing, are fixed for the process at first use.
+static void read_env(BlsState& s) {
     for (const Knob& k : kKnobs) {
         std::string var = "B200_";
         for (const char* c = k.name; *c; c++) var += char(toupper(static_cast<unsigned char>(*c)));
         if (const char* v = getenv(var.c_str())) k.set(s, atoll(v));
     }
     if (const char* v = getenv("B200_G1_SMALL_N")) set_g1_small_n(uint32_t(atol(v)));
-    if (const char* v = getenv("B200_PAIRING_VM")) s.use_vm = atoi(v) != 0;
     if (const char* v = getenv("B200_BLS_TRACE")) s.trace = atoi(v) != 0;
-    if (const char* v = getenv("B200_SMALL_ORDER")) s.small_order = atoi(v);
-    if (const char* v = getenv("B200_SMALL_STREAM_PRIORITY")) *side_prio = atoi(v);   // A/B knob
-    *pair_prio = *side_prio;
-    if (const char* v = getenv("B200_PAIR_STREAM_PRIORITY")) *pair_prio = atoi(v);
 }
 
 static int32_t bls_state(Engine& e, BlsState** out) {
     if (!e.bls) {
         std::unique_ptr<BlsState> s(new BlsState());   // freed if a step below fails; the next call starts over
         for (auto& ev : s->ev_t) B200_CUDA_TRY(cudaEventCreate(&ev));
-        // High priority only matters for B200_SMALL_ORDER=0 (dispatch under the per-key kernel as its CTAs retire).
-        int prio_lo = 0, prio = 0, prio_d = 0;
-        B200_CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio));          // highest priority
-        read_env(*s, &prio, &prio_d);
+        read_env(*s);
+        // signatures / messages at the highest priority: their CTAs dispatch under the per-key kernel as its CTAs retire
+        int prio_lo = 0, prio = 0;
+        B200_CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio));
         B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->sb, cudaStreamNonBlocking, prio));
         B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->sc, cudaStreamNonBlocking, prio));
-        B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->sd, cudaStreamNonBlocking, prio_d));
         B200_CUDA_TRY(cudaStreamCreateWithPriority(&s->se, cudaStreamNonBlocking, prio_lo));
-        for (auto& ev : s->ev_ck) B200_CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        B200_CUDA_TRY(cudaEventCreateWithFlags(&s->ev_join, cudaEventDisableTiming));
+        B200_CUDA_TRY(cudaEventCreateWithFlags(&s->ev_e, cudaEventDisableTiming));
         B200_CUDA_TRY(cudaEventCreateWithFlags(&s->ev_c, cudaEventDisableTiming));
         B200_CUDA_TRY(cudaEventCreateWithFlags(&s->ev_in, cudaEventDisableTiming));
         B200_CUDA_TRY(cudaEventCreateWithFlags(&s->ev_b, cudaEventDisableTiming));
@@ -269,17 +238,14 @@ struct VerifyRun {
     const cudaStream_t sa = e.stream;
     // set by stage_small: word offsets in s.small, the pair arrays on the device, the pinned area results come back to
     size_t o_koff = 0, o_index = 0, o_moff = 0, o_tflags = 0, o_two = 0;
-    std::vector<FoldLevel> fold;   // MODE_AGGREGATE_BATCH with the VM: the levels of the segmented Gt product
+    std::vector<FoldLevel> fold;   // MODE_AGGREGATE_BATCH: the levels of the segmented Gt product
     const uint32_t *d_small = nullptr, *d_g1i = nullptr, *d_g2i = nullptr, *d_ptu = nullptr, *d_poff = nullptr;
     int32_t* h_out = nullptr;
-    bool chunked = false;   // set by key_phase: the pairing chain is already queued on stream D
 
     int32_t run(int32_t* out_codes);
     int32_t reserve_buffers();
     int32_t stage_small();
     int32_t key_phase();
-    int32_t keys_chunked(uint32_t n_chunks);
-    int32_t keys_one_range(uint32_t k_split);
     int32_t launch_small();
     void pairing_tail();
     int32_t rlc_tail();
@@ -287,11 +253,11 @@ struct VerifyRun {
 };
 
 int32_t VerifyRun::run(int32_t* out_codes) {
-    if (b.rlc && (!fa || !s.use_vm)) return B200_ERR_BAD_ARG;
+    if (b.rlc && !fa) return B200_ERR_BAD_ARG;
     int32_t rc;
     if ((rc = reserve_buffers()) || (rc = stage_small()) || (rc = key_phase())) return rc;
     if (b.rlc) return rlc_tail();
-    if (!chunked) pairing_tail();   // chunked: every range's Miller loops and final exponentiations are already queued (joined)
+    pairing_tail();
     if ((rc = readback(h_out + 4, s.out.p, size_t(T) * 4))) return rc;
     if (s.trace) {
         float a = 0, b1 = 0, c = 0, d = 0, f2 = 0, g2 = 0;
@@ -309,7 +275,6 @@ int32_t VerifyRun::reserve_buffers() {
     B200_CUDA_TRY(s.keys.reserve(size_t(n_keys) * 48 + 64));
     B200_CUDA_TRY(s.key_aff.reserve(size_t(n_keys + 1) * sizeof(G1Aff)));
     B200_CUDA_TRY(s.key_code.reserve(size_t(n_keys + 1) * 4));
-    B200_CUDA_TRY(s.g1pts.reserve(size_t(n_g1) * sizeof(G1Aff)));
     B200_CUDA_TRY(s.g1pre.reserve(size_t(n_g1) * sizeof(G1Pre)));
     B200_CUDA_TRY(s.pk_code.reserve(size_t(T + 1) * 4));
     B200_CUDA_TRY(s.flags.reserve(size_t(T + 1) * 4));
@@ -377,13 +342,12 @@ int32_t VerifyRun::stage_small() {
         for (uint32_t t = 0; t < T; t++) small.push_back(av_shape_ok(b, t) ? 0u : uint32_t(TUPLE_FLAG_EMPTY));
         o_two = small.size();
         for (uint32_t t = 0; t <= T; t++) small.push_back(2 * t);
-        if (s.use_vm) {   // level 0 reads the Miller values, with pair_tuple as its map
-            fold = plan_fold(small, o_g1i + 3 * size_t(n_pairs), T, o_g1i + 2 * size_t(n_pairs), true);
-            uint32_t most = 0;
-            for (const FoldLevel& l : fold) most = std::max(most, l.n_out);
-            B200_CUDA_TRY(s.fold_a.reserve((size_t(most) + 1) * sizeof(Fp12)));
-            B200_CUDA_TRY(s.fold_b.reserve((size_t(most) + 1) * sizeof(Fp12)));
-        }
+        // level 0 reads the Miller values, with pair_tuple as its map
+        fold = plan_fold(small, o_g1i + 3 * size_t(n_pairs), T, o_g1i + 2 * size_t(n_pairs), true);
+        uint32_t most = 0;
+        for (const FoldLevel& l : fold) most = std::max(most, l.n_out);
+        B200_CUDA_TRY(s.fold_a.reserve((size_t(most) + 1) * sizeof(Fp12)));
+        B200_CUDA_TRY(s.fold_b.reserve((size_t(most) + 1) * sizeof(Fp12)));
     } else {
         for (uint32_t i = 0; i + 1 < n_pairs; i++) { g1i[i] = i; g2i[i] = i; ptu[i] = 0; }
         if (n_pairs) { g1i[n_pairs - 1] = n_keys; g2i[n_pairs - 1] = n_msgs; ptu[n_pairs - 1] = 0; }
@@ -405,106 +369,35 @@ int32_t VerifyRun::stage_small() {
     return B200_SUCCESS;
 }
 
-// Key copy and K1, with the signature / message kernels placed by B200_SMALL_ORDER.  The one place that picks the shape:
-// several key ranges (b200_tune("bls_chunks")), one range with the key copy split in two, or one plain range.
+// Key copy and K1, the signature / message kernels right behind K1's first launch, K2, and the join
 int32_t VerifyRun::key_phase() {
     const bool have_k1 = n_keys != 0;
-    const uint32_t n_chunks = (fa && !b.rlc && s.use_vm && have_k1 && !registry && s.small_order == 0 && !b.force_fail_shape &&
-                               s.chunks > 1 && T >= s.chunk_min_tuples) ? std::min(s.chunks, BlsState::kMaxChunks) : 1u;
     // Big strict batches: the first kSplitWaves full waves of the per-key kernel start as soon as THEIR keys have arrived; the rest of
     // the key bytes (~90 MB at T = 4096) cross PCIe on stream E under that first launch, and the second launch follows them there
-    // (two streams, so its CTAs fill the first launch's draining tail).  b200_tune("bls_key_split", 0) restores the single copy.
+    // (two streams, so its CTAs fill the first launch's draining tail).
     // The split point is a fixed key count (4 x 148 x 384), not whole waves of this GPU: on an H100 (132 SMs) sizing it and the
     // thresholds below from the SM count made the T = 4096 step ~1 % slower.
     constexpr uint32_t kSplitWaves = 4, kSplitKeys = kSplitWaves * 148u * 384u;
-    const uint32_t k_split = (s.key_split && have_k1 && !registry && n_chunks == 1 && s.small_order == 0 && n_keys >= 4u * kSplitKeys)
-                                 ? kSplitKeys : n_keys;
+    const uint32_t k_split = (have_k1 && !registry && n_keys >= 4u * kSplitKeys) ? kSplitKeys : n_keys;
     if (n_keys) B200_CUDA_TRY(cudaMemcpyAsync(s.keys.p, b.keys, size_t(k_split) * 48, cudaMemcpyHostToDevice, sa));
     B200_CUDA_TRY(cudaEventRecord(s.ev_k0, sa));
     // packed CTAs only when there is a big per-key kernel to run under; alone (registry mode, small batches) they spread
-    set_small_cta(s.small_cta_override ? s.small_cta_override : ((have_k1 && n_keys >= 148u * 384u && s.small_order == 0 && T > 1024) ? 128 : 32));
-    if (have_k1 && s.small_order == 1) {   // signatures / messages first, the per-key kernel only afterwards
-        int32_t rc = launch_small();
-        if (rc) return rc;
-        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_b, 0));
-        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_c, 0));
-    }
+    set_small_cta(s.small_cta_override ? s.small_cta_override : ((have_k1 && n_keys >= 148u * 384u && T > 1024) ? 128 : 32));
     // ---- stream A: public keys
     B200_CUDA_TRY(cudaEventRecord(s.ev_d0, sa));
-    chunked = n_chunks > 1;
-    return chunked ? keys_chunked(n_chunks) : keys_one_range(k_split);
-}
-
-// Chunked strict batch: tuple range c's keys are validated on stream A while range c-1's aggregate -> Miller ->
-// final-exponentiation chain (latency-bound: ~1/3 of the IMAD pipe when alone) runs on stream D in the slots the
-// per-key kernel's retiring 128-thread CTAs leave.  Same kernels, same per-tuple arithmetic, same code vector.
-int32_t VerifyRun::keys_chunked(uint32_t n_chunks) {
-    cudaStream_t sd = s.sd;
-    uint32_t tb[BlsState::kMaxChunks + 1];
-    for (uint32_t c = 0; c <= n_chunks; c++) tb[c] = uint32_t(uint64_t(T) * c / n_chunks);
-    B200_CUDA_TRY(cudaStreamWaitEvent(s.se, s.ev_k0, 0));   // the key bytes
-    for (uint32_t c = 0; c < n_chunks; c++) {
-        const uint32_t k0 = b.key_off[tb[c]], k1 = b.key_off[tb[c + 1]];
-        cudaStream_t sk = ((c & 1u) && s.chunk_alt) ? s.se : sa;
-        launch_g1_validate(static_cast<const uint8_t*>(s.keys.p) + size_t(k0) * 48, k1 - k0, static_cast<G1Aff*>(s.key_aff.p) + k0,
-                           static_cast<int32_t*>(s.key_code.p) + k0, sk, s.chunk_k1_cta);
-        if (k1 > k0) e.launches++;
-        B200_CUDA_TRY(cudaEventRecord(s.ev_ck[c], sk));
-        if (c == 0) {   // signature / message kernels right behind the first range, as in the one-range flow
-            int32_t rc = launch_small();
-            if (rc) return rc;
-        }
-    }
-    if (s.chunk_alt)
-        for (uint32_t c = 1; c < n_chunks; c += 2) B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_ck[c], 0));
-    B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
-    B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_in, 0));   // the small index arrays
-    B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_b, 0));
-    B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_c, 0));
-    B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sd));
-    int32_t* d_pk = static_cast<int32_t*>(s.pk_code.p);
-    uint32_t* d_fl = static_cast<uint32_t*>(s.flags.p);
-    const int32_t* d_sc = static_cast<const int32_t*>(s.sig_code.p);
-    for (uint32_t c = 0; c < n_chunks; c++) {
-        const uint32_t t0 = tb[c], nt = tb[c + 1] - tb[c];
-        if (!nt) continue;
-        B200_CUDA_TRY(cudaStreamWaitEvent(sd, s.ev_ck[c], 0));
-        launch_g1_aggregate(static_cast<const G1Aff*>(s.key_aff.p), static_cast<const int32_t*>(s.key_code.p), nullptr, d_small + o_koff + t0,
-                            nt, nullptr, static_cast<G1Pre*>(s.g1pre.p) + t0, d_pk + t0, d_fl + t0, 0u, sd, nullptr);
-        // pair-indexed arrays start at 2 t0 (values are absolute); tuple-indexed code arrays are read through pair_tuple
-        launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i + 2 * t0, static_cast<const G2Aff*>(s.g2pts.p), d_g2i + 2 * t0,
-                         d_ptu + 2 * t0, d_pk, d_fl, d_sc, 2 * nt, static_cast<Fp12*>(s.f.p) + 2 * size_t(t0), sd);
-        // f BASE + absolute pair offsets; tuple-indexed arrays start at t0
-        launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff + t0, d_pk + t0, d_fl + t0, d_sc + t0, nt,
-                        static_cast<int32_t*>(s.out.p) + t0, sd);
-        e.launches += 3;
-    }
-    B200_CUDA_TRY(cudaEventRecord(s.ev_join, sd));
-    B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_join, 0));
-    if (s.trace) { cudaEventRecord(s.ev_t[0], sa); cudaEventRecord(s.ev_t[1], sa); cudaEventRecord(s.ev_t[2], sa); cudaEventRecord(s.ev_t[3], sa); }
-    return B200_SUCCESS;
-}
-
-// One key range: K1 (two launches when the key copy is split at k_split), the signature / message kernels, K2, and the join
-int32_t VerifyRun::keys_one_range(uint32_t k_split) {
-    const bool have_k1 = n_keys != 0;
-    G1Aff* d_g1 = static_cast<G1Aff*>(s.g1pts.p);
     const G1Aff* key_aff = registry ? static_cast<const G1Aff*>(s.reg_aff.p) : static_cast<const G1Aff*>(s.key_aff.p);
     const int32_t* key_code = registry ? static_cast<const int32_t*>(s.reg_code.p) : static_cast<const int32_t*>(s.key_code.p);
     // where the per-key kernel writes: the call's own arrays, or (registry + extra keys) the tail behind the reg_n resident keys
     G1Aff* k1_aff = registry ? static_cast<G1Aff*>(s.reg_aff.p) + s.reg_n : static_cast<G1Aff*>(s.key_aff.p);
     int32_t* k1_code = registry ? static_cast<int32_t*>(s.reg_code.p) + s.reg_n : static_cast<int32_t*>(s.key_code.p);
     if (have_k1) {
-        launch_g1_validate(static_cast<const uint8_t*>(s.keys.p), k_split, k1_aff, k1_code, sa, k_split < n_keys ? s.k1_first_cta : 0);
+        // the first launch of a split copy, the one the signature / message kernels run under, in 128-thread CTAs: as three
+        // CTAs per SM a side kernel's CTA displaces a third of an SM's per-key work instead of all of it
+        launch_g1_validate(static_cast<const uint8_t*>(s.keys.p), k_split, k1_aff, k1_code, sa, k_split < n_keys ? 128 : 0);
         e.launches++;
     }
-    if (!(have_k1 && s.small_order == 1)) {
-        if (have_k1 && s.small_order == 2) {  // strictly after the per-key kernel
-            B200_CUDA_TRY(cudaEventRecord(s.ev_in, sa));
-        }
-        int32_t rc = launch_small();
-        if (rc) return rc;
-    }
+    int32_t rc = launch_small();
+    if (rc) return rc;
     if (k_split < n_keys) {   // the remaining keys: copy strictly after the first part's (one PCIe link), then their launch
         B200_CUDA_TRY(cudaStreamWaitEvent(s.se, s.ev_k0, 0));
         B200_CUDA_TRY(cudaMemcpyAsync(static_cast<uint8_t*>(s.keys.p) + size_t(k_split) * 48, b.keys + size_t(k_split) * 48,
@@ -512,29 +405,24 @@ int32_t VerifyRun::keys_one_range(uint32_t k_split) {
         launch_g1_validate(static_cast<const uint8_t*>(s.keys.p) + size_t(k_split) * 48, n_keys - k_split, k1_aff + k_split,
                            k1_code + k_split, s.se, 384);
         e.launches++;
-        B200_CUDA_TRY(cudaEventRecord(s.ev_ck[0], s.se));
-        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_ck[0], 0));
+        B200_CUDA_TRY(cudaEventRecord(s.ev_e, s.se));
+        B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_e, 0));
     }
     B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
     if (s.trace) cudaEventRecord(s.ev_t[0], sa);
     launch_g1_aggregate(key_aff, key_code, registry ? d_small + o_index : nullptr, d_small + o_koff, (fa || avb) ? T : 1,
-                        (fa && !s.use_vm) ? d_g1 : nullptr, (fa && s.use_vm) ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
+                        nullptr, fa ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
                         static_cast<int32_t*>(s.pk_code.p), static_cast<uint32_t*>(s.flags.p),
                         b.force_fail_shape ? uint32_t(TUPLE_FLAG_EMPTY) : 0u, sa, b.rlc ? static_cast<G1Jac*>(s.rlc_jac.p) : nullptr,
                         avb ? d_small + o_tflags : nullptr);
     e.launches++;
     if (fa) {
-        B200_CUDA_TRY(cudaMemcpyAsync(d_g1 + T, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
         B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
-    } else if (avb && (s.use_vm || registry)) {
-        // every key's pair operand (the VM's G1Pre, or the registry's points gathered for the one-thread kernels), -g1 behind them
-        const bool pre = s.use_vm;
-        launch_g1_pair_operands(key_aff, registry ? d_small + o_index : nullptr, n_ops, pre ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
-                                pre ? nullptr : d_g1, sa);
+    } else if (avb) {   // every key's pair operand for the VM, -g1 behind them
+        launch_g1_pair_operands(key_aff, registry ? d_small + o_index : nullptr, n_ops, static_cast<G1Pre*>(s.g1pre.p), sa);
         if (n_ops) e.launches++;
-        if (pre) B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + n_ops, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
-        else B200_CUDA_TRY(cudaMemcpyAsync(d_g1 + n_ops, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
-    } else {   // the pairs read the key array itself (pairing_tail)
+        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + n_ops, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
+    } else {   // MODE_AGGREGATE: the pairs read the key array itself (pairing_tail)
         B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Aff*>(s.key_aff.p) + n_keys, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
     }
     // ---- join, pairing
@@ -560,17 +448,18 @@ int32_t VerifyRun::launch_small() {
     return B200_SUCCESS;
 }
 
-// Miller loops and final exponentiations per tuple on stream A: the lane-parallel VM, or one thread per pair
+// Miller loops and final exponentiations per tuple on stream A: the lane-parallel VM for the batches, one thread per pair
+// for the single aggregate_verify
 void VerifyRun::pairing_tail() {
     const G2Aff* d_g2 = static_cast<const G2Aff*>(s.g2pts.p);
     const int32_t* d_pk = static_cast<const int32_t*>(s.pk_code.p);
     const uint32_t* d_fl = static_cast<const uint32_t*>(s.flags.p);
     const int32_t* d_sc = static_cast<const int32_t*>(s.sig_code.p);
-    if (fa && s.use_vm) {
+    if (fa) {
         launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
         if (s.trace) cudaEventRecord(s.ev_t[3], sa);
         launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
-    } else if (avb && s.use_vm) {
+    } else if (avb) {
         // n_t + 1 Miller values per tuple, folded level by level to the two per tuple the final exponentiation reads
         launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
         if (s.trace) cudaEventRecord(s.ev_t[3], sa);
@@ -587,8 +476,7 @@ void VerifyRun::pairing_tail() {
     } else {
         // aggregate_verify pairs the keys themselves: len(msgs) != len(pks) or no keys was flagged EMPTY by K2 -> VERIFY_FAIL
         // after the decoding checks
-        const G1Aff* pair_g1 = static_cast<const G1Aff*>((fa || (avb && registry)) ? s.g1pts.p : s.key_aff.p);
-        launch_miller(pair_g1, d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
+        launch_miller(static_cast<const G1Aff*>(s.key_aff.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
         launch_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
     }
     e.launches += (n_pairs ? 1 : 0) + (T ? 1 : 0);
@@ -602,7 +490,6 @@ int32_t VerifyRun::readback(void* h_dst, const void* d_src, size_t bytes) {
     B200_CUDA_TRY(cudaStreamSynchronize(sa));
     B200_CUDA_TRY(cudaStreamSynchronize(s.sb));
     B200_CUDA_TRY(cudaStreamSynchronize(s.sc));
-    if (chunked) B200_CUDA_TRY(cudaStreamSynchronize(s.sd));
     B200_CUDA_TRY(cudaEventElapsedTime(&e.last_kernel_ms, s.ev_k0, s.ev_k1));
     B200_CUDA_TRY(cudaEventElapsedTime(&s.last_dominant_ms, s.ev_d0, s.ev_d1));
     return B200_SUCCESS;
@@ -710,7 +597,6 @@ static int32_t run_verify(Engine& e, BlsState& s, const Batch& b, int32_t* out_c
         cudaStreamSynchronize(e.stream);
         cudaStreamSynchronize(s.sb);
         cudaStreamSynchronize(s.sc);
-        cudaStreamSynchronize(s.sd);
         cudaStreamSynchronize(s.se);
         cudaGetLastError();
     }

@@ -492,14 +492,11 @@ B200_API float b200_last_dominant_kernel_ms(void);
 B200_API int32_t b200_measure_int_peak(int32_t kind, double* gops);
 /* Scheduling knobs of the BLS batch pipeline, settable at run time (the same names, upper-cased with a B200_ prefix, are
  * read from the environment when the pipeline is first used).  They change launch shapes only, never a result:
- *   "bls_chunks" (key ranges per strict batch, 1 = off), "bls_chunk_min_tuples", "bls_chunk_k1_cta" (128 | 384),
- *   "bls_chunk_alt" (0 | 1: alternate key ranges over two streams), "bls_key_split" (0 | 1: big strict batches copy most
- *   of their keys under the first waves of the per-key kernel), "bls_k1_first_cta" (128 | 384: CTA size of those first waves),
  *   "bls_small_cta" (0 = by batch size | 32 | 64 | 128: CTA size of the signature / message kernels), "vm_team16_max",
  *   "vm_cta" (32 | 64 | 128).
- * An environment value goes through the same rule as the value passed here: B200_BLS_K1_FIRST_CTA other than 128 means 384,
- * a negative B200_VM_TEAM16_MAX means 0, and B200_BLS_SMALL_CTA is the only name of that knob.
- * Unknown knob -> B200_ERR_BAD_ARG. */
+ * An environment value goes through the same rule as the value passed here: a negative B200_VM_TEAM16_MAX means 0, and
+ * B200_BLS_SMALL_CTA is the only name of that knob.
+ * Unknown knob -> B200_ERR_BAD_ARG; so are the names of the key-range, split-copy and first-wave knobs earlier versions took. */
 B200_API int32_t b200_tune(const char* knob, int64_t value);
 /* Replaces the scheduled Miller-loop / final-exponentiation programs of one team size (8 or 16 lanes) of the lane-parallel
  * pairing kernels with another SCHEDULE of the same formulas: `blob` is what `tools/gen_pairing_vm.py <team> ... --blob F`

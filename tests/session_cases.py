@@ -542,9 +542,7 @@ def build_session(seed: int = 0x5E55, scale: float = SCALE) -> Session:
     settings("bls_small_cta", 128)
     strict(b, ragged)
     settings("bls_small_cta", 0, tags=[("restore",)])
-    settings("bls_k1_first_cta", 384)
     strict(b, big_side)
-    settings("bls_k1_first_cta", 128, tags=[("restore",)])
     b.add("settings", "vm_load_programs", dict(blob=alt_blob), None, writes={"knobs"})
     strict(b, pairs_2048)
     rlc(rlc_true[3], seed_b)

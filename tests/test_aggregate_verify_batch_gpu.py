@@ -2,8 +2,8 @@
 single call b200_aggregate_verify and the C oracle agree code for code: the golden cases as one batch, every crafted tuple,
 shuffled, and closed-form batches of 256 x 64 (8-lane programs), 1 x 2048 (one fold over three levels) and 4096 x 1.  Also:
 both team sizes and every vm_cta; the registry path equals the strict path, keys appended after the load and keys that
-failed validation included; the one-thread pairing kernels (B200_PAIRING_VM=0, in a child process); the segmented Gt
-product value by value (b200_pairing_eval); one engine interleaving this call with the other families; every refusal,
+failed validation included; the indexed call refused in a process that never loaded a registry (a child process); the
+segmented Gt product value by value (b200_pairing_eval); one engine interleaving this call with the other families; every refusal,
 each followed by a good call; and the launches per call shape."""
 from __future__ import annotations
 
@@ -35,8 +35,6 @@ STRICT_4096x1 = 1 + 1 + 2 + 1 + 1 + 1 + 0 + 1        # two Miller values per tup
 STRICT_256x64 = 1 + 1 + 2 + 1 + 1 + 1 + 2 + 1        # 65 values per tuple: in up to three pieces, then one level more
 STRICT_SHAPE_ONLY = 1 + 1 + 2 + 1 + 1 + 0 + 0 + 1    # no tuple has a pairing: no Miller loop, no level
 REGISTRY_1x4 = STRICT_1x4 - 1                         # no K1
-VM0_STRICT_1x4 = 1 + 1 + 2 + 1 + 1 + 1                # one thread per pair: the keys themselves, Miller, final
-VM0_REGISTRY_1x4 = 1 + 2 + 1 + 1 + 1 + 1              # K3, K4, K2, the registry points gathered, Miller, final
 
 
 @pytest.fixture(scope="module")
@@ -200,7 +198,7 @@ def _load(path):
 
 
 def _child(path):
-    """B200_PAIRING_VM=0 (set by the parent): refusal without a registry, then the codes and launches of each path."""
+    """A fresh process: refusal without a registry, then the codes of the strict and the registry path."""
     from ethereum_consensus_b200 import _lib, crypto
     _lib.init(0)
     tuples = _load(path)
@@ -212,31 +210,26 @@ def _child(path):
     res = {"no_registry": L.b200_aggregate_verify_batch_indexed(_lib.ptr(idx), _lib.ptr(np.array(koff, dtype=np.uint32)), _lib.ptr(flat),
                                                                 _lib.ptr(moff), _lib.ptr(g), _lib.ptr(_arr(sigs)), 2, _lib.ptr(out))}
     res["codes"] = _batch(tuples)
-    four = [t for t in tuples if len(t["pks"]) == 4 and len(t["msgs"]) == 4][:1]
-    res["strict_1x4"] = list(_counted(_batch, four))
     keys = _registry_keys(tuples)
     reg = crypto.Registry(_arr(b"".join(keys[:20])))
     reg.append(_arr(b"".join(keys[20:])))
     where = {k: i for i, k in enumerate(keys)}
     res["registry"] = _registry_batch(reg, where, tuples)
-    res["registry_1x4"] = list(_counted(_registry_batch, reg, where, four))
     print("RESULT " + json.dumps(res))
 
 
-def test_without_pairing_vm(engine, cases, tmp_path):
-    """The one-thread-per-pair kernels (k_miller + k_final) take the batch's multi-pair tuples through pair_off."""
+def test_indexed_call_without_registry_in_child_process(engine, cases, tmp_path):
+    """b200_aggregate_verify_batch_indexed answers B200_ERR_BAD_ARG until a registry is loaded; this process may have one."""
     from ethereum_consensus_b200 import _lib
     path = tmp_path / "cases.json"
     _dump(cases, path)
     p = subprocess.run([sys.executable, "-m", "tests.test_aggregate_verify_batch_gpu", str(path)], cwd=str(ROOT), capture_output=True,
-                       text=True, env=dict(os.environ, B200_PAIRING_VM="0"), timeout=1200)
+                       text=True, timeout=1200)
     assert p.returncode == 0, p.stdout + p.stderr
     res = json.loads(next(ln for ln in p.stdout.splitlines() if ln.startswith("RESULT "))[7:])
     want = [t["want"] for t in cases]
     assert res["no_registry"] == _lib.ERR_BAD_ARG
     assert res["codes"] == want and res["registry"] == want
-    assert res["strict_1x4"] == [[av.SUCCESS], VM0_STRICT_1x4]
-    assert res["registry_1x4"] == [[av.SUCCESS], VM0_REGISTRY_1x4]
 
 
 def test_fold_segments_value_by_value(engine):

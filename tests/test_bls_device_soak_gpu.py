@@ -6,9 +6,9 @@ register caps), and the per-tuple G1 sum, the G2 sum and the two-launch hash_to_
 case goes through the kernels and its code (and, where there is one, its output bytes) is compared with the oracle's.
 
 Sections: a. key validation, b. signature decode + subgroup check, c. hash_to_G2 by verdict, d. equal / opposite points
-meeting in the aggregation lanes and trees, e. whole tuples (plain, chunked, RLC).  B200_PAIRING_VM and B200_G1_SMALL_N are
-read once per process, so sections a, d and e run again in one child process per setting; with B200_G1_SMALL_N=0 every
-key of those sections goes through the role-split per-key kernel, not only the tiled loads.
+meeting in the aggregation lanes and trees, e. whole tuples (plain, RLC).  B200_G1_SMALL_N is read once per process, so
+sections a, d and e run again in a child process with B200_G1_SMALL_N=0: every key of those sections goes through the
+role-split per-key kernel, not only the tiled loads.
 
     B200_SOAK_SCALE=1 (default) python -m pytest tests/test_bls_device_soak_gpu.py -m gpu -s
 """
@@ -36,14 +36,12 @@ pytestmark = pytest.mark.gpu
 SCALE = float(os.environ.get("B200_SOAK_SCALE", "1"))
 SMALL_N = 3 * 148 * 384          # bls_g1.cu g_g1_small_n: up to here the per-key kernel goes out as 128-thread CTAs
 RLC_SEED = hashlib.sha256(b"device soak rlc").digest()
-# the last: every per-key launch through the role-split kernel (k_g1_validate_split), whatever its size
-ENV_VARIANTS = [{"B200_PAIRING_VM": "0"},
-                {"B200_PAIRING_VM": "1", "B200_G1_SMALL_N": "0"}]
+# every per-key launch through the role-split kernel (k_g1_validate_split), whatever its size
+ENV_VARIANTS = [{"B200_G1_SMALL_N": "0"}]
 
 
 def _env_id(e):
-    small = "-small_n_%s" % e["B200_G1_SMALL_N"] if "B200_G1_SMALL_N" in e else ""
-    return "vm_%s%s" % (e["B200_PAIRING_VM"], small)
+    return "small_n_%s" % e["B200_G1_SMALL_N"]
 
 
 def _n(x):
@@ -324,7 +322,7 @@ def check_keys(D, tag=""):
     return res
 
 
-def check_shapes(D, rlc, tag=""):
+def check_shapes(D, tag=""):
     from ethereum_consensus_b200 import crypto
     res = []
     tup, want = D["tuples"], D["want"]
@@ -346,34 +344,25 @@ def check_shapes(D, rlc, tag=""):
     res.append(("d. eth_aggregate_public_keys" + tag, *report("d. shapes: eth_aggregate_public_keys" + tag, D["agg_want"], got)))
     got = [_code(crypto.aggregate, [f[96 * j: 96 * j + 96] for j in range(len(f) // 96)]) for f in D["sig_sets"]]
     res.append(("d. aggregate (signatures)" + tag, *report("d. shapes: aggregate(signatures)" + tag, D["sig_want"], got)))
-    if rlc:
-        ok = [t for t, w in zip(tup, want) if w == 0]
-        got = [crypto.fast_aggregate_verify_batch_all(*_pack(tup), seed=RLC_SEED), crypto.fast_aggregate_verify_batch_all(*_pack(ok), seed=RLC_SEED)]
-        res.append(("d. RLC" + tag, *report("d. shapes: fast_aggregate_verify_batch_all" + tag, [all(w == 0 for w in want), True], got)))
+    ok = [t for t, w in zip(tup, want) if w == 0]
+    got = [crypto.fast_aggregate_verify_batch_all(*_pack(tup), seed=RLC_SEED), crypto.fast_aggregate_verify_batch_all(*_pack(ok), seed=RLC_SEED)]
+    res.append(("d. RLC" + tag, *report("d. shapes: fast_aggregate_verify_batch_all" + tag, [all(w == 0 for w in want), True], got)))
     return res
 
 
-def check_tuples(D, rlc, tag=""):
+def check_tuples(D, tag=""):
     from ethereum_consensus_b200 import crypto
     res = []
     tup, want = D["tuples"], D["want"]
-    args = _pack(tup)
-    res.append(("e. strict batch" + tag, *report("e. tuples: strict batch" + tag, want, crypto.fast_aggregate_verify_batch(*args).tolist())))
-    try:
-        crypto.tune("bls_chunks", 5); crypto.tune("bls_chunk_min_tuples", 2)
-        got = crypto.fast_aggregate_verify_batch(*args).tolist()
-    finally:
-        crypto.tune("bls_chunks", 1); crypto.tune("bls_chunk_min_tuples", 2048)
-    res.append(("e. chunked" + tag, *report("e. tuples: 5 chunks" + tag, want, got)))
-    if rlc:
-        ok = [t for t, w in zip(tup, want) if w == 0]
-        wants, gots = [True], [crypto.fast_aggregate_verify_batch_all(*_pack(ok), seed=RLC_SEED)]
-        for kind in range(1, sc.N_TUPLE_KINDS):
-            bad = next((t for t, w, k in zip(tup, want, D["kind"]) if k == kind and w != 0), None)
-            if bad is not None:
-                wants.append(False)
-                gots.append(crypto.fast_aggregate_verify_batch_all(*_pack(ok[:40] + [bad] + ok[40:80]), seed=RLC_SEED))
-        res.append(("e. RLC" + tag, *report("e. tuples: batch_all, valid and each class" + tag, wants, gots)))
+    res.append(("e. strict batch" + tag, *report("e. tuples: strict batch" + tag, want, crypto.fast_aggregate_verify_batch(*_pack(tup)).tolist())))
+    ok = [t for t, w in zip(tup, want) if w == 0]
+    wants, gots = [True], [crypto.fast_aggregate_verify_batch_all(*_pack(ok), seed=RLC_SEED)]
+    for kind in range(1, sc.N_TUPLE_KINDS):
+        bad = next((t for t, w, k in zip(tup, want, D["kind"]) if k == kind and w != 0), None)
+        if bad is not None:
+            wants.append(False)
+            gots.append(crypto.fast_aggregate_verify_batch_all(*_pack(ok[:40] + [bad] + ok[40:80]), seed=RLC_SEED))
+    res.append(("e. RLC" + tag, *report("e. tuples: batch_all, valid and each class" + tag, wants, gots)))
     return res
 
 
@@ -443,7 +432,7 @@ def test_c_hash_to_g2(engine, oracle_bls_c):
 def test_d_aggregation_edge_cases(engine, oracle_bls_c):
     t = time.time()
     D = shapes_data(oracle_bls_c)
-    res = check_shapes(D, rlc=True)
+    res = check_shapes(D)
     print(f"d. wall {time.time() - t:.1f} s")
     _assert_clean(res, {"d. strict batch": 30})
     assert 0 in D["want"] and any(w != 0 for w in D["want"])   # both verdicts occur among the shapes
@@ -452,7 +441,7 @@ def test_d_aggregation_edge_cases(engine, oracle_bls_c):
 def test_e_whole_tuples(engine, oracle_bls_c):
     t = time.time()
     D = tuples_data(oracle_bls_c)
-    res = check_tuples(D, rlc=True)
+    res = check_tuples(D)
     print(f"e. wall {time.time() - t:.1f} s")
     _assert_clean(res, {"e. strict batch": _min(3000)})
     assert len(set(D["want"])) >= 4
@@ -460,9 +449,8 @@ def test_e_whole_tuples(engine, oracle_bls_c):
 
 @pytest.mark.parametrize("env", ENV_VARIANTS, ids=_env_id)
 def test_env_variants_in_child_processes(oracle_bls_c, tmp_path, env):
-    """Sections a, d and e with every per-key launch through the role-split kernel / under the one-thread-per-pair
-    pairing kernels, which only the environment selects (read once per process): one child process per setting, inputs
-    and oracle verdicts from here."""
+    """Sections a, d and e with every per-key launch through the role-split kernel, which only the environment selects
+    (read once per process): one child process per setting, inputs and oracle verdicts from here."""
     t = time.time()
     data = {"keys": keys_data(oracle_bls_c), "shapes": shapes_data(oracle_bls_c), "tuples": tuples_data(oracle_bls_c)}
     path = tmp_path / "soak.pkl"
@@ -485,9 +473,8 @@ def _child(path):
     from ethereum_consensus_b200 import _lib
     _lib.init(0)
     data = pickle.loads(Path(path).read_bytes())
-    rlc = os.environ.get("B200_PAIRING_VM", "1") != "0"     # the RLC entry points refuse the one-thread-per-pair kernels
-    tag = " [VM %s, small n %s]" % (os.environ.get("B200_PAIRING_VM", "1"), os.environ.get("B200_G1_SMALL_N", "default"))
-    res = check_keys(data["keys"], tag) + check_shapes(data["shapes"], rlc, tag) + check_tuples(data["tuples"], rlc, tag)
+    tag = " [small n %s]" % os.environ.get("B200_G1_SMALL_N", "default")
+    res = check_keys(data["keys"], tag) + check_shapes(data["shapes"], tag) + check_tuples(data["tuples"], tag)
     _assert_clean(res)
     print("CHILD_OK")
 

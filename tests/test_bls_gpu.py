@@ -86,24 +86,21 @@ def test_fast_aggregate_verify_batch_all_golden(engine):
     assert got.tolist() == want.tolist()
 
 
-def test_chunked_pipeline_same_codes_on_ragged_golden_batch(engine):
-    """The strict batch in 2..16 key ranges (per-key kernel of range c+1 over range c's pairing chain), the VM kernels at
-    every CTA size: launch shapes only — the golden codes (ragged K, empty tuples, every failure kind) must not move."""
+def test_vm_launch_shapes_same_codes_on_ragged_golden_batch(engine):
+    """The strict batch with the VM kernels at every CTA size, with and without 16-lane teams: launch shapes only — the
+    golden codes (ragged K, empty tuples, every failure kind) must not move."""
     pks, off, msgs, sigs, want = _batch_inputs(list(reversed(FAV)), reps=3)
     try:
-        crypto.tune("bls_chunk_min_tuples", 2)
-        for chunks, alt, cta, vm_cta in ((1, 1, 128, 128), (2, 1, 128, 64), (3, 0, 384, 32), (5, 1, 384, 128), (16, 1, 128, 128), (64, 0, 128, 64)):
-            crypto.tune("bls_chunks", chunks); crypto.tune("bls_chunk_alt", alt)
-            crypto.tune("bls_chunk_k1_cta", cta); crypto.tune("vm_cta", vm_cta)
+        for vm_cta in (32, 64, 128):
+            crypto.tune("vm_cta", vm_cta)
             for team16_max in (0, 1 << 20):
                 crypto.tune("vm_team16_max", team16_max)
                 got = crypto.fast_aggregate_verify_batch(pks, off, msgs, sigs)
-                assert got.tolist() == want.tolist(), (chunks, alt, cta, vm_cta, team16_max)
+                assert got.tolist() == want.tolist(), (vm_cta, team16_max)
         with pytest.raises(Exception):
             crypto.tune("no_such_knob", 1)
     finally:
-        for k, v in (("bls_chunks", 1), ("bls_chunk_min_tuples", 2048), ("bls_chunk_alt", 1), ("bls_chunk_k1_cta", 128), ("vm_cta", 32), ("bls_k1_first_cta", 128), ("bls_small_cta", 0),
-                     ("vm_team16_max", 2048)):
+        for k, v in (("vm_cta", 32), ("bls_small_cta", 0), ("vm_team16_max", 2048)):
             crypto.tune(k, v)
 
 

@@ -3,13 +3,8 @@ it launches (b200_launch_count).  Which phases run, on how many key ranges and i
 so a launch count that moves means a path changed; the codes say it still computes the same thing.
 
 Launch names: K1 per-key validation, K3 signature decode, K4 hash_to_G2 (two kernels: map, finish), K2 per-tuple
-aggregate, K5 Miller loops, K6 final exponentiations.  The B200_SMALL_ORDER and B200_PAIRING_VM settings are read once
-per process, so each runs the shared shapes in a child process."""
+aggregate, K5 Miller loops, K6 final exponentiations."""
 import json
-import os
-import subprocess
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -18,7 +13,6 @@ from ethereum_consensus_b200 import _lib, crypto, parallel
 from tests.test_bls_gpu import FAV, GOLDEN, _batch_inputs, _call
 
 pytestmark = pytest.mark.gpu
-ROOT = Path(__file__).resolve().parent.parent
 
 # batch of fast-aggregate tuples with keys: K1 + K3 + K4 (2) + K2 + K5 + K6
 STRICT = 1 + 1 + 2 + 1 + 1 + 1
@@ -26,8 +20,6 @@ STRICT = 1 + 1 + 2 + 1 + 1 + 1
 REGISTRY = 1 + 2 + 1 + 1 + 1
 # big strict batch (>= 4 x 227 328 keys): K1 on the first 227 328 keys, a second K1 on the rest behind their copy
 SPLIT = STRICT + 1
-# golden batch in 5 key ranges: K1 per range + K3 + K4 (2) under the first range + K2, K5, K6 per range (T = 37, no range empty)
-CHUNKED5 = 5 * 1 + 3 + 5 * 3
 # RLC tail: K_scale, the signature folds (ceil(n / 32) per level), K_finish, K5 on T + 1 pairs, the Gt folds, K_one, K6
 def rlc(t):
     def folds(n):
@@ -49,8 +41,9 @@ AGG_PUBKEYS = 3        # K1 + aggregate + compress
 CASES = [c for c in FAV if len(c["msg"]) == 64]
 VALID = [c for c in CASES if c["code"] == 0]
 BIG_T, BIG_K = 1776, 512
-KNOB_DEFAULTS = {"bls_chunks": 1, "bls_chunk_min_tuples": 2048, "bls_chunk_k1_cta": 128, "bls_chunk_alt": 1, "bls_key_split": 1,
-                 "bls_k1_first_cta": 128, "bls_small_cta": 0, "vm_team16_max": 2048, "vm_cta": 32}
+KNOB_DEFAULTS = {"bls_small_cta": 0, "vm_team16_max": 2048, "vm_cta": 32}
+# knobs earlier versions took; b200_tune refuses them like any unknown name
+RETIRED_KNOBS = ("bls_chunks", "bls_chunk_min_tuples", "bls_chunk_k1_cta", "bls_chunk_alt", "bls_key_split", "bls_k1_first_cta")
 
 
 def _launches() -> int:
@@ -94,7 +87,7 @@ def _case(section, name):
 
 
 def shared_shapes() -> dict:
-    """The call shapes every process setting runs: name -> (codes, launches)."""
+    """One call of each shape: name -> (codes, launches)."""
     crypto.fast_aggregate_verify_batch(*_batch_inputs(FAV)[:4])   # first use builds the pipeline's state (2 launches)
     res = {}
     codes, n = _counted(crypto.fast_aggregate_verify_batch, *_batch_inputs(FAV)[:4])
@@ -129,12 +122,10 @@ def shared_shapes() -> dict:
     return res
 
 
-def check_shared(res: dict, split: bool, big_codes=None):
+def check_shared(res: dict):
     want = [c["code"] for c in CASES]
     assert res["strict"] == [want, STRICT]
-    assert res["big"][1] == (SPLIT if split else STRICT)
-    if big_codes is not None:
-        assert res["big"][0] == big_codes
+    assert res["big"][1] == SPLIT
     assert res["registry_load"][1] == 1
     assert res["registry"] == [want, REGISTRY]
     assert res["mixed"] == [want, STRICT]
@@ -150,7 +141,7 @@ def check_shared(res: dict, split: bool, big_codes=None):
 
 @pytest.fixture
 def knobs(engine):
-    """Every knob at its default around the test (the counts below assume one key range and the split key copy)."""
+    """Every knob at its default around the test."""
     for k, v in KNOB_DEFAULTS.items():
         crypto.tune(k, v)
     yield
@@ -166,24 +157,7 @@ def default_shapes(engine):
 
 
 def test_shared_shapes_default_process(default_shapes):
-    check_shared(default_shapes, split=True)
-
-
-def test_split_key_copy_matches_single_copy(knobs, default_shapes):
-    big = _big_batch()
-    codes, n = _counted(crypto.fast_aggregate_verify_batch, *big)
-    assert (codes.tolist(), n) == (default_shapes["big"][0], SPLIT)
-    crypto.tune("bls_key_split", 0)
-    codes, n = _counted(crypto.fast_aggregate_verify_batch, *big)
-    assert (codes.tolist(), n) == (default_shapes["big"][0], STRICT)
-
-
-def test_chunked_golden_batch(knobs):
-    want = [c["code"] for c in CASES]
-    crypto.tune("bls_chunks", 5)
-    crypto.tune("bls_chunk_min_tuples", 2)
-    codes, n = _counted(crypto.fast_aggregate_verify_batch, *_batch_inputs(FAV)[:4])
-    assert (codes.tolist(), n) == (want, CHUNKED5)
+    check_shared(default_shapes)
 
 
 def test_whole_batch_calls(knobs):
@@ -214,23 +188,7 @@ def test_sharded_calls_world1(knobs):
 def test_tune_accepts_every_documented_knob(engine):
     for k, v in KNOB_DEFAULTS.items():
         crypto.tune(k, v)
-    with pytest.raises(_lib.EngineError) as e:
-        crypto.tune("no_such_knob", 1)
-    assert e.value.code == _lib.ERR_BAD_ARG
-
-
-@pytest.mark.parametrize("env,split", [({"B200_SMALL_ORDER": "1"}, False), ({"B200_SMALL_ORDER": "2"}, False),
-                                       ({"B200_PAIRING_VM": "0"}, True)], ids=["small_order1", "small_order2", "pairing_vm0"])
-def test_shared_shapes_under_env(default_shapes, env, split):
-    """The signature / message kernels before (1) or after (2) the per-key kernel, which also turns the split key copy
-    off; the one-thread-per-pair pairing kernels (B200_PAIRING_VM=0): same codes, same launches per phase."""
-    p = subprocess.run([sys.executable, "-m", "tests.test_bls_host_pipeline_gpu"], cwd=str(ROOT), capture_output=True, text=True,
-                       env=dict(os.environ, **env), timeout=900)
-    assert p.returncode == 0, p.stdout + p.stderr
-    line = next(ln for ln in p.stdout.splitlines() if ln.startswith("SHAPES "))
-    check_shared(json.loads(line[len("SHAPES "):]), split=split, big_codes=default_shapes["big"][0])
-
-
-if __name__ == "__main__":
-    _lib.init(0)
-    print("SHAPES " + json.dumps(shared_shapes()))
+    for k in ("no_such_knob", *RETIRED_KNOBS):
+        with pytest.raises(_lib.EngineError) as e:
+            crypto.tune(k, 1)
+        assert e.value.code == _lib.ERR_BAD_ARG, k

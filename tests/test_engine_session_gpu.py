@@ -5,8 +5,6 @@ step of the same family) through the CUDA library, every answer against the orac
 a. the session in script order (this process);
 b. the same session in a seeded topological shuffle (dependent steps keep their order) in a child process; every answer
    equal to a's; a step that differs is replayed alone, with the steps it depends on, in a fresh child process;
-c. a child process with B200_PAIRING_VM=0: the session without its RLC steps, and the RLC entry points refused with
-   B200_ERR_BAD_ARG;
 d. four worker threads that never called b200_init, each with its own resident handle, running the session's state steps
    on it and a share of the one-shot, shuffle and batch steps, all at once; they read the registry and change nothing
    shared.  Every answer equal to a's.
@@ -15,7 +13,6 @@ d. four worker threads that never called b200_init, each with its own resident h
 """
 from __future__ import annotations
 
-import os
 import pickle
 import subprocess
 import sys
@@ -256,12 +253,12 @@ def sequential(engine):
     return got, wall
 
 
-def _child(mode, tmp_path, payload, env=None):
+def _child(mode, tmp_path, payload):
     path = tmp_path / f"{mode}.pkl"
     path.write_bytes(pickle.dumps(payload))
     out = tmp_path / f"{mode}.out.pkl"
     p = subprocess.run([sys.executable, "-m", "tests.test_engine_session_gpu", mode, str(path), str(out)], cwd=str(ROOT),
-                       env=dict(os.environ, **(env or {})), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
+                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
                        timeout=CHILD_TIMEOUT)
     print(p.stdout[-4000:])
     assert p.returncode == 0, p.stdout[-4000:]
@@ -305,24 +302,6 @@ def test_b_shuffled_order_in_a_child(sequential, tmp_path):
           f"wall {time.time() - t:.1f} s")
     assert not differ, f"{len(differ)} answers depend on the order, first at step {differ[0]}"
     assert not mismatches(s.steps, got_b)
-
-
-# ---------------------------------------------------------------------------------------------------------- c
-def test_c_without_the_pairing_vm(sequential, tmp_path):
-    s = session()
-    got_a, _ = sequential
-    keep = [x.i for x in s.steps if x.family != "rlc"]
-    rlc = [x.i for x in s.steps if x.family == "rlc"]
-    t = time.time()
-    got_c = _child("run", tmp_path, dict(steps=s.steps, init=s.init_state, order=keep + rlc[:1] + rlc[-1:]),
-                   env={"B200_PAIRING_VM": "0"})
-    differ = [i for i in keep if got_c[i] != got_a[i]]
-    for i in differ[:5]:
-        _print_context(s.steps, keep, i, got_c)
-    refusals = [got_c[i] for i in (rlc[:1] + rlc[-1:])]
-    print(f"c. B200_PAIRING_VM=0: {len(keep)} steps, mismatches {len(differ)}; RLC answers {refusals}; wall {time.time() - t:.1f} s")
-    assert not differ, f"{len(differ)} answers differ without the pairing VM, first at step {differ[0]}"
-    assert refusals == [sn.refused(sn.ERR_BAD_ARG)] * 2
 
 
 # ---------------------------------------------------------------------------------------------------------- d

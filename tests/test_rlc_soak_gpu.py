@@ -14,7 +14,6 @@ again under each pairing-VM launch shape (vm_cta 32 / 64 / 128, vm_team16_max 0)
 from __future__ import annotations
 
 import os
-import pickle
 import subprocess
 import sys
 import time
@@ -171,19 +170,6 @@ def test_bc_under_vm_launch_shapes(engine, oracle_bls_c, knob, value):
     _assert_clean(res)
 
 
-def test_rlc_refused_without_the_pairing_vm(oracle_bls_c, tmp_path):
-    """With B200_PAIRING_VM=0 (one thread per pair) the RLC entry points answer B200_ERR_BAD_ARG, never a boolean."""
-    _, M, fam = soak(oracle_bls_c)
-    c = next(c for c in fam["A"] if "A:crafted" in c.tags)
-    path = tmp_path / "rlc.pkl"
-    path.write_bytes(pickle.dumps({"args": [np.ascontiguousarray(a) for a in M.pack(c.batch)], "seed": rc.SEED}))
-    p = subprocess.run([sys.executable, "-m", "tests.test_rlc_soak_gpu", str(path)], cwd=str(ROOT), capture_output=True, text=True,
-                       env=dict(os.environ, B200_PAIRING_VM="0"), timeout=600)
-    print(p.stdout)
-    assert p.returncode == 0, p.stdout + p.stderr
-    assert "CHILD_OK" in p.stdout
-
-
 def _gpu_count():
     try:
         out = subprocess.run(["nvidia-smi", "-L"], capture_output=True, text=True, timeout=60).stdout
@@ -203,31 +189,3 @@ def test_crafted_batch_on_two_ranks(oracle_bls_c, oracle_ssz_c, tmp_path):
     ranks = run_ranks(tmp_path / "box", 2, transport="nccl", devices=[0, 1], sections=["rlc"])
     n, bad = check(ranks, data, sections={"rlc"})
     assert not bad, "\n".join(bad[:40])
-
-
-def _child(path):
-    from ethereum_consensus_b200 import _lib, crypto, parallel
-    _lib.init(0)
-    data = pickle.loads(Path(path).read_bytes())
-    args, seed = data["args"], data["seed"]
-    pks, off, msgs, sigs = args
-    parallel.comm_init(0, 1)
-    reg = crypto.Registry(pks)
-    calls = [lambda: crypto.fast_aggregate_verify_batch_all(*args, seed=seed),
-             lambda: crypto.fast_aggregate_verify_batch_all(*args),
-             lambda: crypto.fast_aggregate_verify_batch_all(*args, seed=seed, sharded=True),
-             lambda: reg.verify_batch_all(np.arange(int(off[-1]), dtype=np.uint32), off, msgs, sigs, seed=seed)]
-    for i, call in enumerate(calls):
-        try:
-            r = call()
-        except _lib.EngineError as e:
-            assert e.code == _lib.ERR_BAD_ARG, (i, hex(e.code))
-            print(f"entry point {i}: engine error 0x{e.code:x}")
-        else:
-            raise AssertionError(f"entry point {i} answered {r!r} without the pairing VM")
-    assert crypto.fast_aggregate_verify_batch(*args).tolist() == [5] * (len(off) - 1)   # the strict path still works
-    print("CHILD_OK")
-
-
-if __name__ == "__main__":
-    _child(sys.argv[1])

@@ -147,12 +147,12 @@ def test_census_every_refusal_is_followed_by_its_family(session):
 def test_census_settings_rlc_singles_ssz_shuffles_evals(session):
     steps = session.steps
     tunes = [(s.args["knob"], s.args["value"]) for s in steps if s.op == "tune"]
-    for kv in (("vm_cta", 64), ("vm_cta", 128), ("vm_team16_max", 0), ("bls_small_cta", 128), ("bls_k1_first_cta", 384)):
+    for kv in (("vm_cta", 64), ("vm_cta", 128), ("vm_team16_max", 0), ("bls_small_cta", 128)):
         assert kv in tunes, kv
     last = {}
     for k, v in tunes:
         last[k] = v
-    assert last == {"vm_cta": 32, "vm_team16_max": sn.VM_TEAM16_MAX, "bls_small_cta": 0, "bls_k1_first_cta": 128}
+    assert last == {"vm_cta": 32, "vm_team16_max": sn.VM_TEAM16_MAX, "bls_small_cta": 0}
     loads = [s for s in steps if s.op == "vm_load_programs"]
     assert len(loads) == 3 and [("restore",) in s.tags for s in loads] == [False, True, True]
     assert any(s.family in ("strict", "rlc") for s in steps[loads[0].i:loads[1].i])

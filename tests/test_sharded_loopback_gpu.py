@@ -3,8 +3,7 @@ loopback communicator (b200_comm_init_loopback).  The cases (tests/sharded_cases
 split: strict verify against the C oracle's codes, the RLC check against the exponent model with the global tuple index,
 the sharded state roots against the C oracle, the host all-gathers, and the refusals.  Every rank must return the expected
 values, identical across ranks, with exactly one collective per sharded call and none per refusal.  World 2 runs again
-without the pairing VM (B200_PAIRING_VM=0: the strict call on the one-thread kernels, the RLC call refused) and with
-team-8 Miller loops at every batch size (B200_VM_TEAM16_MAX=0).
+with team-8 Miller loops at every batch size (B200_VM_TEAM16_MAX=0).
 
 The parent process builds the cases and never touches the GPU; each group of workers runs under a timeout and is killed
 and reaped on any failure."""
@@ -24,8 +23,7 @@ from tests import sharded_cases as sh
 pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parent.parent
 WORKER = ROOT / "tests" / "mp_loopback_worker.py"
-ERR_BAD_ARG = 0x102
-CONFIGS = [(w, {}) for w in sh.WORLDS] + [(2, {"B200_PAIRING_VM": "0"}), (2, {"B200_VM_TEAM16_MAX": "0"})]
+CONFIGS = [(w, {}) for w in sh.WORLDS] + [(2, {"B200_VM_TEAM16_MAX": "0"})]
 
 
 def _compute_mode():
@@ -69,7 +67,7 @@ def run_ranks(box: Path, world: int, transport: str = "loopback", env=None, devi
     return out
 
 
-def expected(data, vm=True):
+def expected(data):
     """{name: (value, return code, collectives)} of every record the worker writes."""
     want = {}
     single = data["strict"][0]["want"]
@@ -84,7 +82,7 @@ def expected(data, vm=True):
         want[c["name"]] = (c["want"], 0, 1)
     for c in data["rlc"]:
         for i, (_seed, w) in enumerate(c["runs"]):
-            want[f"{c['name']} [seed {i}]"] = (w, 0, 1) if vm else (None, ERR_BAD_ARG, 0)
+            want[f"{c['name']} [seed {i}]"] = (w, 0, 1)
     w = data["world"]
     want["comm_all_gather_codes"] = ([int(x) for r in range(w) for x in sh.gather_codes(r)], 0, 1)
     for n in data["gather"]:
@@ -96,9 +94,9 @@ def expected(data, vm=True):
     return want
 
 
-def check(ranks, data, vm=True, sections=None):
+def check(ranks, data, sections=None):
     """Mismatches of every rank against the expected values, and between ranks; returns (records per rank, mismatches)."""
-    want = expected(data, vm)
+    want = expected(data)
     bad = []
     for r, recs in enumerate(ranks):
         for sec, name, value, rc, ncoll in recs:
@@ -151,11 +149,10 @@ def test_sharded_entry_points_over_loopback(cases, world, env, tmp_path):
     (box / "cases.pkl").write_bytes((src / "cases.pkl").read_bytes())
     t = time.time()
     ranks = run_ranks(box, world, env=env)
-    n, bad = check(ranks, data, vm=env.get("B200_PAIRING_VM") != "0")
+    n, bad = check(ranks, data)
     print(f"world {world} {env}: {n} records, {len(bad)} mismatches, wall {time.time() - t:.1f} s")
     assert not bad, "\n".join(bad[:40])
-    if env.get("B200_PAIRING_VM") != "0":
-        for r, recs in enumerate(ranks):   # two identical RLC calls put the same bytes in the rank's slot: Gt, flag 0, zeros
-            slots = next(v for s, n_, v, *_ in recs if s == "slot" and n_ == "rlc slot twice")
-            assert len(slots) == 2 and slots[0] == slots[1], r
-            assert slots[0][576:] == bytes(16) and any(slots[0][:576]), r
+    for r, recs in enumerate(ranks):   # two identical RLC calls put the same bytes in the rank's slot: Gt, flag 0, zeros
+        slots = next(v for s, n_, v, *_ in recs if s == "slot" and n_ == "rlc slot twice")
+        assert len(slots) == 2 and slots[0] == slots[1], r
+        assert slots[0][576:] == bytes(16) and any(slots[0][:576]), r
