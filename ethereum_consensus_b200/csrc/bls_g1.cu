@@ -199,12 +199,9 @@ __global__ void k_g1_pair_operands(const G1Aff* __restrict__ keys, const uint32_
     p.xz = a.x; p.y = a.y; p.z3 = fp_one(); p.inf = a.inf;
     pre[i] = p;
 }
-__global__ void k_neg_g1(G1Aff* out, G1Pre* out_pre) {
+__global__ void k_neg_g1(G1Pre* out_pre) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
-        G1Aff g;
         const Fp x = B200_FP_G1_X, y = B200_FP_G1_NEG_Y;
-        g.x = x; g.y = y; g.inf = 0;
-        *out = g;
         G1Pre p;
         p.xz = x; p.y = y; p.z3 = fp_one(); p.inf = 0;
         *out_pre = p;
@@ -452,7 +449,7 @@ void launch_g1_compress_groups(const G1Aff* agg, const int32_t* pk_code, const u
     k_g1_compress_groups<<<(n_groups + t - 1) / t, t, with_pow_tab(k_g1_compress_groups, t), static_cast<cudaStream_t>(stream)>>>(
         agg, pk_code, flags, n_groups, out48, out_code);
 }
-void launch_neg_g1(G1Aff* out, G1Pre* out_pre, void* stream) { k_neg_g1<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(out, out_pre); }
+void launch_neg_g1(G1Pre* out_pre, void* stream) { k_neg_g1<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(out_pre); }
 void launch_fp_selftest(uint32_t n, uint32_t seed, uint32_t* out_mismatch, void* stream) {
     k_fp_selftest<<<(n + 127) / 128, 128, with_pow_tab(k_fp_selftest, 128), static_cast<cudaStream_t>(stream)>>>(n, seed, out_mismatch);
 }

@@ -61,17 +61,12 @@ void launch_g2_sig_decode(const uint8_t* sigs, uint32_t n, G2Aff* out, int32_t* 
 // K4: hash_to_G2 of message i = bytes [moff[i], moff[i+1]) of `msgs`
 //     `tmp_jac`: scratch for 2n Jacobian G2 points (288 B each)
 void launch_hash_to_g2(const uint8_t* msgs, const uint32_t* moff, uint32_t n, G2Aff* out, void* tmp_jac, void* stream);
-// K5: one Miller loop per pair (g1[g1_idx[i]], g2[g2_idx[i]]); pairs whose tuple already failed are skipped
-void launch_miller(const G1Aff* g1, const uint32_t* g1_idx, const G2Aff* g2, const uint32_t* g2_idx,
-                   const uint32_t* pair_tuple, const int32_t* pk_code, const uint32_t* flags, const int32_t* sig_code,
-                   uint32_t n_pairs, Fp12* f, void* stream);
-// K6: per tuple: merge codes with the reference's precedence, multiply its Miller values, final exponentiation
-void launch_final(const Fp12* f, const uint32_t* pair_off, const int32_t* pk_code, const uint32_t* flags,
-                  const int32_t* sig_code, uint32_t n_tuples, int32_t* out_codes, void* stream);
-// lane-parallel (team) versions of K5 / K6 for tuples with exactly two pairs (bls_vm.cu); vm_init returns 0 on success
+// the lane-parallel pairing VM (bls_vm.cu); vm_init returns 0 on success
 int vm_init(void* stream);
 // replaces one team size's scheduled programs (blob layout: bls_vm.cu); returns 0 on success, 1 on a malformed blob
 int vm_load_programs(const uint32_t* blob, size_t n_words, void* stream);
+// K5: one Miller loop per pair (g1[g1_idx[i]], g2[g2_idx[i]]); pairs whose tuple already failed are skipped
+// K6: per tuple: merge codes with the reference's precedence, final exponentiation of f[pair_off[t]] f[pair_off[t] + 1]
 void launch_vm_miller(const G1Pre* g1, const uint32_t* g1_idx, const G2Aff* g2, const uint32_t* g2_idx,
                       const uint32_t* pair_tuple, const int32_t* pk_code, const uint32_t* flags, const int32_t* sig_code,
                       uint32_t n_pairs, Fp12* f, void* stream);
@@ -89,8 +84,8 @@ void launch_g2_aggregate(const G2Aff* sigs, const int32_t* sig_code, const uint3
 // `eth_aggregate_public_keys` over T groups after K2 (affine sums, codes, flags): code and compressed sum per group
 void launch_g1_compress_groups(const G1Aff* agg, const int32_t* pk_code, const uint32_t* flags, uint32_t n_groups, uint8_t* out48,
                                int32_t* out_code, void* stream);
-// writes -g1 (the negated generator) to *out (and its G1Pre form)
-void launch_neg_g1(G1Aff* out, G1Pre* out_pre, void* stream);
+// writes -g1 (the negated generator) in its G1Pre form to *out_pre
+void launch_neg_g1(G1Pre* out_pre, void* stream);
 // on-device self-test of Fp arithmetic (portable vs tuned paths), returns mismatches in *out
 void launch_fp_selftest(uint32_t n, uint32_t seed, uint32_t* out_mismatch, void* stream);
 // on-device self-test: one field operation on n raw operand pairs, for comparison with big integers on the host.

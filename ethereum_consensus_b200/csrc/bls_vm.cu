@@ -1,7 +1,8 @@
 // Lane-parallel pairing kernels: a TEAM of 8 or 16 lanes per (G1, G2) pair / per tuple replays the statically
 // scheduled Fp2 programs of tools/gen_pairing_vm.py (Miller loop, final exponentiation) on a shared-memory register
-// file.  Replaces the one-thread-per-pair kernels of bls_pairing.cu on the batch path: those expose only 2T threads
-// (a latency floor of tens of ms at T = 4096); here 16x more lanes work on the same tuples, products stay inlined PTX.
+// file.  Every verification call pairs here.  One thread per pair, as bls_pairing.cu's reference kernels run, would expose
+// only 2T threads (a latency floor of tens of ms at T = 4096); here 16x more lanes work on the same tuples, products stay
+// inlined PTX.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -30,6 +31,8 @@ __device__ __forceinline__ void vm_run(const uint32_t* __restrict__ code, int n_
                                        const VmRfStrided& rf, uint32_t lane, bool active) {
     // the next round's instruction word is fetched while the current round executes: with one or two warps per scheduler
     // (small batches) the load's latency would otherwise sit on the critical path of every one of the ~2 500 / ~3 800 rounds
+    // A warp with no live team (failed or padding tuples) skips the rounds; all its lanes leave together.
+    if (!__any_sync(~0u, active)) return;
     uint32_t w = __ldg(code + lane);
 #pragma unroll 1
     for (int r = 0; r < n_rounds; r++) {

@@ -1,7 +1,7 @@
 // extern "C" entry points — the BLS half of include/b200_consensus.h — and the host orchestration of the batch
 // pipeline.  Every function below is a drop-in for one body in
 // ethereum-consensus/src/crypto/bls.rs (line ranges in the header); all curve arithmetic runs in
-// the kernels of bls_g1.cu / bls_g2.cu / bls_pairing.cu.  The host only stages bytes and index arrays.
+// the kernels of bls_g1.cu / bls_g2.cu / bls_vm.cu / bls_rlc.cu.  The host only stages bytes and index arrays.
 //
 // Flow for T tuples with NK public keys in total (strict mode):
 //   stream A: H2D offsets, keys (100 MB) ........ wait(B,C) | K1 key_validate (NK threads) | K2 per-tuple aggregate
@@ -46,7 +46,6 @@ struct BlsState {
     // aggregate_verify batches: the segmented Gt product's ping-pong levels
     DevBuf fold_a, fold_b;
     PinnedBuf stage;
-    G1Aff* d_negg1 = nullptr;
     G1Pre* d_negg1_pre = nullptr;
     // registry (validated keys resident on the device)
     DevBuf reg_aff, reg_code;
@@ -64,7 +63,6 @@ struct BlsState {
         for (cudaStream_t st : {sb, sc, se}) if (st) cudaStreamDestroy(st);
         for (cudaEvent_t ev : ev_t) if (ev) cudaEventDestroy(ev);
         for (cudaEvent_t ev : {ev_e, ev_in, ev_b, ev_c, ev_k0, ev_k1, ev_d0, ev_d1}) if (ev) cudaEventDestroy(ev);
-        cudaFree(d_negg1);
         cudaFree(d_negg1_pre);
     }
 };
@@ -112,9 +110,8 @@ static int32_t bls_state(Engine& e, BlsState** out) {
         B200_CUDA_TRY(cudaEventCreate(&s->ev_k1));
         B200_CUDA_TRY(cudaEventCreate(&s->ev_d0));
         B200_CUDA_TRY(cudaEventCreate(&s->ev_d1));
-        B200_CUDA_TRY(cudaMalloc(&s->d_negg1, sizeof(G1Aff)));
         B200_CUDA_TRY(cudaMalloc(&s->d_negg1_pre, sizeof(G1Pre)));
-        launch_neg_g1(s->d_negg1, s->d_negg1_pre, e.stream);
+        launch_neg_g1(s->d_negg1_pre, e.stream);
         e.launches++;
         if (vm_init(e.stream) != 0) { e.last_error = "pairing VM initialisation failed"; return B200_ERR_CUDA; }
         e.launches++;
@@ -126,7 +123,7 @@ static int32_t bls_state(Engine& e, BlsState** out) {
     return B200_SUCCESS;
 }
 
-enum PairMode { MODE_FAST_AGGREGATE = 0, MODE_AGGREGATE = 1, MODE_AGGREGATE_BATCH = 2 };
+enum PairMode { MODE_FAST_AGGREGATE = 0, MODE_AGGREGATE_BATCH = 1 };
 // message offsets travel as uint32 (32 bytes per tuple on the batch paths): 32 * T must not wrap
 constexpr size_t kMaxBatchTuples = size_t(1) << 26;
 // keys a `..._batch_mixed` call may bring along (a block carries <= 16 deposits + 16 bls-to-execution changes)
@@ -142,8 +139,8 @@ struct RlcReq {
 };
 
 // One call's work: T tuples.  MODE_FAST_AGGREGATE: tuple t sums keys [key_off[t], key_off[t+1]) and checks
-// e(sum, H(msg_t)) e(-g1, sig_t) == 1.  MODE_AGGREGATE: one tuple, pairs (key_i, H(msg_i)) + (-g1, sig).
-// MODE_AGGREGATE_BATCH: T such tuples, tuple t pairing keys [key_off[t], ..) with messages [msg_group[t], ..).
+// e(sum, H(msg_t)) e(-g1, sig_t) == 1.  MODE_AGGREGATE_BATCH: tuple t pairs keys [key_off[t], ..) with messages
+// [msg_group[t], ..), (key_i, H(msg_i)) for each, plus (-g1, sig_t).
 struct Batch {
     PairMode mode = MODE_FAST_AGGREGATE;
     // host key bytes (strict); with `index` as well: n_keys EXTRA keys (deposits, bls-to-execution changes) validated by this
@@ -159,7 +156,6 @@ struct Batch {
     const uint32_t* msg_group = nullptr;   // MODE_AGGREGATE_BATCH: T + 1 offsets into the messages
     const uint8_t* sigs = nullptr;
     uint32_t T = 0;
-    bool force_fail_shape = false;     // MODE_AGGREGATE: no pairs, the tuple is flagged EMPTY
     RlcReq* rlc = nullptr;
 };
 
@@ -228,10 +224,10 @@ struct VerifyRun {
     BlsState& s;
     const Batch& b;
     const uint32_t T = b.T, n_keys = b.n_keys, n_msgs = b.n_msgs;
-    const bool fa = b.mode == MODE_FAST_AGGREGATE, avb = b.mode == MODE_AGGREGATE_BATCH, registry = b.index != nullptr;
+    const bool fa = b.mode == MODE_FAST_AGGREGATE, registry = b.index != nullptr;
     const uint32_t n_ops = registry ? b.n_index : n_keys;   // MODE_AGGREGATE_BATCH: one G1 operand per key of the call
-    const uint32_t n_g1 = (fa ? T : avb ? n_ops : n_keys) + 1;  // + (-g1)
-    const uint32_t n_pairs = fa ? 2 * T : avb ? av_pairs(b) : (b.force_fail_shape ? 0 : n_msgs + 1);
+    const uint32_t n_g1 = (fa ? T : n_ops) + 1;  // + (-g1)
+    const uint32_t n_pairs = fa ? 2 * T : av_pairs(b);
     const uint32_t n_g2 = n_msgs + T;
     const uint32_t msg_bytes = b.msg_off[n_msgs];
     const uint32_t rlc_world = b.rlc && b.rlc->exchange ? uint32_t(comm().world) : 1u;
@@ -273,7 +269,7 @@ int32_t VerifyRun::run(int32_t* out_codes) {
 
 int32_t VerifyRun::reserve_buffers() {
     B200_CUDA_TRY(s.keys.reserve(size_t(n_keys) * 48 + 64));
-    B200_CUDA_TRY(s.key_aff.reserve(size_t(n_keys + 1) * sizeof(G1Aff)));
+    B200_CUDA_TRY(s.key_aff.reserve(size_t(n_keys) * sizeof(G1Aff)));
     B200_CUDA_TRY(s.key_code.reserve(size_t(n_keys + 1) * 4));
     B200_CUDA_TRY(s.g1pre.reserve(size_t(n_g1) * sizeof(G1Pre)));
     B200_CUDA_TRY(s.pk_code.reserve(size_t(T + 1) * 4));
@@ -304,12 +300,10 @@ int32_t VerifyRun::reserve_buffers() {
 // small host-built arrays, one staged copy on stream A: [key_off | index | msg_off | g1_idx | g2_idx | pair_tuple | pair_off],
 // then for MODE_AGGREGATE_BATCH [tuple flags | 0, 2, .., 2T | the fold levels' maps and offsets]
 int32_t VerifyRun::stage_small() {
-    const uint32_t n_koff = (fa || avb) ? T + 1 : 2;
     std::vector<uint32_t> small;
-    small.reserve(size_t(n_koff) + b.n_index + n_msgs + 1 + 3 * size_t(n_pairs) + T + 1 + 8);
+    small.reserve(size_t(T) + 1 + b.n_index + n_msgs + 1 + 3 * size_t(n_pairs) + T + 1 + 8);
     o_koff = small.size();
-    if (fa || avb) small.insert(small.end(), b.key_off, b.key_off + T + 1);
-    else { small.push_back(0); small.push_back(n_keys); }
+    small.insert(small.end(), b.key_off, b.key_off + T + 1);
     o_index = small.size();
     if (registry) small.insert(small.end(), b.index, b.index + b.n_index);
     o_moff = small.size();
@@ -328,7 +322,7 @@ int32_t VerifyRun::stage_small() {
             poff[t] = 2 * t;
         }
         poff[T] = 2 * T;
-    } else if (avb) {   // tuple t: (key_i, H(msg_i)) for its n keys and messages, then (-g1, sig_t); none without a pairing
+    } else {   // tuple t: (key_i, H(msg_i)) for its n keys and messages, then (-g1, sig_t); none without a pairing
         uint32_t p = 0;
         for (uint32_t t = 0; t < T; t++) {
             poff[t] = p;
@@ -348,10 +342,6 @@ int32_t VerifyRun::stage_small() {
         for (const FoldLevel& l : fold) most = std::max(most, l.n_out);
         B200_CUDA_TRY(s.fold_a.reserve((size_t(most) + 1) * sizeof(Fp12)));
         B200_CUDA_TRY(s.fold_b.reserve((size_t(most) + 1) * sizeof(Fp12)));
-    } else {
-        for (uint32_t i = 0; i + 1 < n_pairs; i++) { g1i[i] = i; g2i[i] = i; ptu[i] = 0; }
-        if (n_pairs) { g1i[n_pairs - 1] = n_keys; g2i[n_pairs - 1] = n_msgs; ptu[n_pairs - 1] = 0; }
-        poff[0] = 0; poff[1] = n_pairs;
     }
     const size_t small_bytes = small.size() * 4;
     B200_CUDA_TRY(s.stage.reserve(small_bytes + size_t(T + 1) * 4 + 64 +
@@ -410,21 +400,17 @@ int32_t VerifyRun::key_phase() {
     }
     B200_CUDA_TRY(cudaEventRecord(s.ev_d1, sa));
     if (s.trace) cudaEventRecord(s.ev_t[0], sa);
-    launch_g1_aggregate(key_aff, key_code, registry ? d_small + o_index : nullptr, d_small + o_koff, (fa || avb) ? T : 1,
+    launch_g1_aggregate(key_aff, key_code, registry ? d_small + o_index : nullptr, d_small + o_koff, T,
                         nullptr, fa ? static_cast<G1Pre*>(s.g1pre.p) : nullptr,
                         static_cast<int32_t*>(s.pk_code.p), static_cast<uint32_t*>(s.flags.p),
-                        b.force_fail_shape ? uint32_t(TUPLE_FLAG_EMPTY) : 0u, sa, b.rlc ? static_cast<G1Jac*>(s.rlc_jac.p) : nullptr,
-                        avb ? d_small + o_tflags : nullptr);
+                        0u, sa, b.rlc ? static_cast<G1Jac*>(s.rlc_jac.p) : nullptr, fa ? nullptr : d_small + o_tflags);
     e.launches++;
-    if (fa) {
-        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + T, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
-    } else if (avb) {   // every key's pair operand for the VM, -g1 behind them
+    if (!fa) {   // every key's pair operand for the VM
         launch_g1_pair_operands(key_aff, registry ? d_small + o_index : nullptr, n_ops, static_cast<G1Pre*>(s.g1pre.p), sa);
         if (n_ops) e.launches++;
-        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + n_ops, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
-    } else {   // MODE_AGGREGATE: the pairs read the key array itself (pairing_tail)
-        B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Aff*>(s.key_aff.p) + n_keys, s.d_negg1, sizeof(G1Aff), cudaMemcpyDeviceToDevice, sa));
     }
+    // -g1 behind the tuples' aggregates or the keys' operands
+    B200_CUDA_TRY(cudaMemcpyAsync(static_cast<G1Pre*>(s.g1pre.p) + n_g1 - 1, s.d_negg1_pre, sizeof(G1Pre), cudaMemcpyDeviceToDevice, sa));
     // ---- join, pairing
     if (s.trace) cudaEventRecord(s.ev_t[1], sa);
     B200_CUDA_TRY(cudaStreamWaitEvent(sa, s.ev_b, 0));
@@ -448,37 +434,26 @@ int32_t VerifyRun::launch_small() {
     return B200_SUCCESS;
 }
 
-// Miller loops and final exponentiations per tuple on stream A: the lane-parallel VM for the batches, one thread per pair
-// for the single aggregate_verify
+// Miller loops and final exponentiations per tuple on stream A, on the lane-parallel VM.  An aggregate_verify tuple's
+// n + 1 Miller values are folded level by level to the two the final exponentiation reads; fast-aggregate tuples have
+// two already (no fold levels).
 void VerifyRun::pairing_tail() {
     const G2Aff* d_g2 = static_cast<const G2Aff*>(s.g2pts.p);
     const int32_t* d_pk = static_cast<const int32_t*>(s.pk_code.p);
     const uint32_t* d_fl = static_cast<const uint32_t*>(s.flags.p);
     const int32_t* d_sc = static_cast<const int32_t*>(s.sig_code.p);
-    if (fa) {
-        launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
-        if (s.trace) cudaEventRecord(s.ev_t[3], sa);
-        launch_vm_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
-    } else if (avb) {
-        // n_t + 1 Miller values per tuple, folded level by level to the two per tuple the final exponentiation reads
-        launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
-        if (s.trace) cudaEventRecord(s.ev_t[3], sa);
-        const Fp12* fin = static_cast<const Fp12*>(s.f.p);
-        Fp12* const buf[2] = {static_cast<Fp12*>(s.fold_a.p), static_cast<Fp12*>(s.fold_b.p)};
-        for (size_t k = 0; k < fold.size(); k++) {
-            const FoldLevel& l = fold[k];
-            launch_fold_segments(fin, l.n_in, d_small + l.o_map, d_small + l.o_in, l.o_out == kFinalLevel ? nullptr : d_small + l.o_out,
-                                 d_pk, d_fl, d_sc, buf[k & 1], sa);
-            if (l.n_in) e.launches++;
-            fin = buf[k & 1];
-        }
-        launch_vm_final(fin, fold.empty() ? d_poff : d_small + o_two, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
-    } else {
-        // aggregate_verify pairs the keys themselves: len(msgs) != len(pks) or no keys was flagged EMPTY by K2 -> VERIFY_FAIL
-        // after the decoding checks
-        launch_miller(static_cast<const G1Aff*>(s.key_aff.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
-        launch_final(static_cast<const Fp12*>(s.f.p), d_poff, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
+    launch_vm_miller(static_cast<const G1Pre*>(s.g1pre.p), d_g1i, d_g2, d_g2i, d_ptu, d_pk, d_fl, d_sc, n_pairs, static_cast<Fp12*>(s.f.p), sa);
+    if (s.trace) cudaEventRecord(s.ev_t[3], sa);
+    const Fp12* fin = static_cast<const Fp12*>(s.f.p);
+    Fp12* const buf[2] = {static_cast<Fp12*>(s.fold_a.p), static_cast<Fp12*>(s.fold_b.p)};
+    for (size_t k = 0; k < fold.size(); k++) {
+        const FoldLevel& l = fold[k];
+        launch_fold_segments(fin, l.n_in, d_small + l.o_map, d_small + l.o_in, l.o_out == kFinalLevel ? nullptr : d_small + l.o_out,
+                             d_pk, d_fl, d_sc, buf[k & 1], sa);
+        if (l.n_in) e.launches++;
+        fin = buf[k & 1];
     }
+    launch_vm_final(fin, fold.empty() ? d_poff : d_small + o_two, d_pk, d_fl, d_sc, T, static_cast<int32_t*>(s.out.p), sa);
     e.launches += (n_pairs ? 1 : 0) + (T ? 1 : 0);
 }
 
@@ -1440,13 +1415,15 @@ int32_t b200_aggregate_verify(const uint8_t* pks_flat, size_t n_pks, const uint8
             moff.push_back(uint32_t(flat.size()));
         }
     }
+    // a batch of one tuple; with a bad shape it has no messages, so av_shape_ok flags it EMPTY
+    const uint32_t key_off[2] = {0, uint32_t(n_pks)}, msg_group[2] = {0, uint32_t(moff.size() - 1)};
     int32_t code = B200_ERR_CUDA;
-    rc = run_verify(e, *s, {.mode = MODE_AGGREGATE, .keys = pks_flat, .n_keys = uint32_t(n_pks), .msgs = flat.data(), .msg_off = moff.data(),
-                            .n_msgs = uint32_t(moff.size() - 1), .sigs = sig, .T = 1, .force_fail_shape = shape_fail}, &code);
+    rc = run_verify(e, *s, {.mode = MODE_AGGREGATE_BATCH, .keys = pks_flat, .n_keys = uint32_t(n_pks), .key_off = key_off, .msgs = flat.data(),
+                            .msg_off = moff.data(), .n_msgs = msg_group[1], .msg_group = msg_group, .sigs = sig, .T = 1}, &code);
     return rc ? rc : code;
 }
 
-// crypto/bls.rs:95-112 over T tuples: the same codes as T calls of b200_aggregate_verify, on the lane-parallel pairing
+// crypto/bls.rs:95-112 over T tuples: the same codes as T calls of b200_aggregate_verify
 int32_t b200_aggregate_verify_batch(const uint8_t* pks_flat, const uint32_t* pk_offsets, const uint8_t* msgs, const uint32_t* msg_offsets,
                                     const uint32_t* msg_group, const uint8_t* sigs, size_t n_tuples, int32_t* out_codes) {
     Engine& e = engine();

@@ -3,7 +3,7 @@ it launches (b200_launch_count).  Which phases run, on how many key ranges and i
 so a launch count that moves means a path changed; the codes say it still computes the same thing.
 
 Launch names: K1 per-key validation, K3 signature decode, K4 hash_to_G2 (two kernels: map, finish), K2 per-tuple
-aggregate, K5 Miller loops, K6 final exponentiations."""
+aggregate, K5 Miller loops and K6 final exponentiations on the pairing VM."""
 import json
 
 import numpy as np
@@ -29,11 +29,12 @@ def rlc(t):
             if n <= 1:
                 return k
     return 1 + folds(t) + 1 + 1 + folds(t + 1) + 1 + 1
-# aggregate_verify: K1 + K3 + K4 (2) + K2 + one-thread-per-pair Miller + final exponentiation
-AGG_VERIFY = 1 + 1 + 2 + 1 + 1 + 1
-# aggregate_verify with len(pks) != len(msgs): no messages to hash, no pairs: K1 + K3 + K2 + final exponentiation
-AGG_VERIFY_MISMATCH = 1 + 1 + 1 + 1
-# aggregate_verify with no keys and no messages: K3 + K2 + final exponentiation
+# aggregate_verify, a batch of one tuple with 4 messages: K1 + K3 + K4 (2) + K2 + pair operands + K5 + one fold level
+# (5 Miller values, one piece) + K6
+AGG_VERIFY = 1 + 1 + 2 + 1 + 1 + 1 + 1 + 1
+# aggregate_verify with len(pks) != len(msgs): no messages to hash, no pairs, no fold: K1 + K3 + K2 + pair operands + K6
+AGG_VERIFY_MISMATCH = 1 + 1 + 1 + 1 + 1
+# aggregate_verify with no keys and no messages: K3 + K2 + K6
 AGG_VERIFY_EMPTY = 1 + 1 + 1
 AGGREGATE = 2          # signature decode + sum / compress
 AGG_PUBKEYS = 3        # K1 + aggregate + compress
@@ -110,9 +111,6 @@ def shared_shapes() -> dict:
     res["verify_signature"] = _counted_code(crypto.verify_signature, h(one["pks"][0]), h(one["msg"]), h(one["sig"]))
     res["fast_aggregate_verify"] = _counted_code(crypto.fast_aggregate_verify, [h(p) for p in k3["pks"]], h(k3["msg"]), h(k3["sig"]))
     res["fast_aggregate_verify_no_keys"] = _counted_code(crypto.fast_aggregate_verify, [], h(none["msg"]), h(none["sig"]))
-    for name in ("4 distinct messages", "length mismatch", "empty"):
-        c = _case("aggregate_verify", name)
-        res[f"aggregate_verify {name}"] = _counted_code(crypto.aggregate_verify, [h(p) for p in c["pks"]], [h(m) for m in c["msgs"]], h(c["sig"]))
     c = _case("aggregate", "4 sigs")
     out, n = _counted(crypto.aggregate, [h(s) for s in c["sigs"]])
     res["aggregate"] = (bytes(out).hex(), n)
@@ -132,9 +130,6 @@ def check_shared(res: dict):
     assert res["verify_signature"] == [0, STRICT]
     assert res["fast_aggregate_verify"] == [0, STRICT]
     assert res["fast_aggregate_verify_no_keys"] == [5, STRICT - 1]          # no keys: no K1
-    assert res["aggregate_verify 4 distinct messages"] == [0, AGG_VERIFY]
-    assert res["aggregate_verify length mismatch"] == [5, AGG_VERIFY_MISMATCH]
-    assert res["aggregate_verify empty"] == [5, AGG_VERIFY_EMPTY]
     assert res["aggregate"] == [_case("aggregate", "4 sigs")["out"], AGGREGATE]
     assert res["eth_aggregate_public_keys"] == [_case("eth_aggregate_public_keys", "8 keys")["out"], AGG_PUBKEYS]
 
@@ -158,6 +153,21 @@ def default_shapes(engine):
 
 def test_shared_shapes_default_process(default_shapes):
     check_shared(default_shapes)
+
+
+def test_aggregate_verify_single_call_is_batch_of_one(knobs):
+    """The single aggregate_verify call runs as an aggregate_verify batch of one tuple: its codes and launches per shape,
+    and on a valid tuple the same code and launch count as aggregate_verify_batch."""
+    crypto.fast_aggregate_verify_batch(*_batch_inputs(FAV)[:4])   # first use builds the pipeline's state (2 launches)
+    h = bytes.fromhex
+    for name, want in (("4 distinct messages", (0, AGG_VERIFY)), ("length mismatch", (5, AGG_VERIFY_MISMATCH)),
+                       ("empty", (5, AGG_VERIFY_EMPTY))):
+        c = _case("aggregate_verify", name)
+        assert _counted_code(crypto.aggregate_verify, [h(p) for p in c["pks"]], [h(m) for m in c["msgs"]], h(c["sig"])) == want, name
+    c = _case("aggregate_verify", "4 distinct messages")
+    codes, n = _counted(crypto.aggregate_verify_batch, _flat(c["pks"]), [0, len(c["pks"])], [h(m) for m in c["msgs"]],
+                        [0, len(c["msgs"])], np.frombuffer(h(c["sig"]), dtype=np.uint8))
+    assert (codes.tolist(), n) == ([0], AGG_VERIFY)
 
 
 def test_whole_batch_calls(knobs):

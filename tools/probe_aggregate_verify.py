@@ -1,6 +1,6 @@
 """What aggregate_verify in batches costs on the GPU: one JSON line (DESIGN.md §8).
 
-  single_vs_batch   T = 1, n in {1, 16, 128, 512}: b200_aggregate_verify (one thread per pair) against
+  single_vs_batch   T = 1, n in {1, 16, 128, 512}: b200_aggregate_verify against
                     aggregate_verify_batch (lane-parallel Miller loops, segmented product, lane-parallel final exponentiation)
   t64_n128          T = 64, n = 128: one batch call against 64 single calls
   t4096_n1          T = 4096, n = 1: aggregate_verify_batch against fast_aggregate_verify_batch with K = 1 on the same tuples
