@@ -73,6 +73,7 @@ _PROTOS = {
     "b200_state_attesting_indices": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_void_p, C.c_void_p]),
     "b200_state_process_epoch": (C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(C.c_int32)]),
+    "b200_state_epoch_deltas": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "b200_state_serialized_len": (C.c_int32, [C.c_void_p, C.POINTER(C.c_uint64)]),
     "b200_state_read_bytes": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t]),
     # multi-GPU (comm.cu): the exchange step lives inside the library

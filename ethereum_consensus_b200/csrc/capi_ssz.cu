@@ -1212,6 +1212,31 @@ bool block_root(const b200_state* h, const Preset& P, uint64_t slot, uint64_t ep
 }
 constexpr uint32_t kPerValidatorSteps = B200_EPOCH_INACTIVITY_UPDATES | B200_EPOCH_REWARDS_AND_PENALTIES |
                                         B200_EPOCH_REGISTRY_UPDATES | B200_EPOCH_SLASHINGS | B200_EPOCH_EFFECTIVE_BALANCE_UPDATES;
+// get_total_balance (:2857-2868) of sum k of the totals pass: the checked sum, then at least one increment
+uint64_t total_balance(const EpochTotals& T, int k, uint64_t inc) { return std::max(T.lo[k], inc); }
+// The scalars of the reward deltas, shared by b200_state_process_epoch and b200_state_epoch_deltas.  `read` has bit k set
+// for every sum k of T the caller's sub-steps read; one that overflows u64 refuses with B200_ERR_LIMIT before anything is
+// filled.  Otherwise fills p's total_active, base_per_inc (get_base_reward_per_increment, the exact integer_sqrt),
+// active_inc, part_inc, increment and inactivity_denominator.
+int32_t reward_scalars(Engine& e, const EpochTotals& T, const Preset& P, uint32_t read, const char* who, EpochParams* p) {
+    for (int k = 0; k < 5; k++)
+        if ((read >> k & 1) && T.hi[k]) {
+            e.last_error = std::string(who) + ": get_total_balance overflows u64";
+            return B200_ERR_LIMIT;
+        }
+    const uint64_t inc = P.effective_balance_increment;
+    p->total_active = total_balance(T, 0, inc);
+    p->base_per_inc = inc * P.base_reward_factor / integer_sqrt(p->total_active);
+    p->active_inc = p->total_active / inc;
+    for (int f = 0; f < 3; f++) p->part_inc[f] = total_balance(T, 1 + f, inc) / inc;
+    p->increment = inc;
+    p->inactivity_denominator = P.inactivity_score_bias * P.inactivity_penalty_quotient_bellatrix;
+    return B200_SUCCESS;
+}
+// is_in_inactivity_leak; get_finality_delay wraps
+bool inactivity_leak(const Preset& P, uint64_t prev, uint64_t finalized_epoch) {
+    return prev - finalized_epoch > P.min_epochs_to_inactivity_penalty;
+}
 }  // namespace
 
 int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_code) {
@@ -1241,13 +1266,12 @@ int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_cod
     const bool run_sync = (steps & B200_EPOCH_SYNC_COMMITTEE_UPDATES) && next % P.epochs_per_sync_committee_period == 0;
     const bool run_summary = (steps & B200_EPOCH_HISTORICAL_SUMMARIES_UPDATE) &&
                              next % (P.slots_per_historical_root / P.slots_per_epoch) == 0;
-    // get_total_balance: checked sum, then at least one increment
+    // get_total_balance: the sums a selected sub-step reads
     const bool total_read = run_jf || run_rewards || (steps & B200_EPOCH_SLASHINGS);
-    if ((total_read && T.hi[0]) || (run_jf && (T.hi[2] || T.hi[4])) || (run_rewards && (T.hi[1] || T.hi[2] || T.hi[3]))) {
-        e.last_error = "process_epoch: get_total_balance overflows u64";
-        return B200_ERR_LIMIT;
-    }
-    auto total = [&](int k) { return std::max(T.lo[k], inc); };
+    const uint32_t read = (total_read ? 1u : 0u) | (run_jf ? 0x14u : 0u) | (run_rewards ? 0xeu : 0u);
+    EpochParams p{};
+    if ((rc = reward_scalars(e, T, P, read, "process_epoch", &p))) return rc;
+    auto total = [&](int k) { return total_balance(T, k, inc); };
     uint8_t jf[121];   // justification_bits, previous_justified, current_justified, finalized (adjacent)
     memcpy(jf, h->shadow + h->so.justification_bits, sizeof(jf));
     if (run_jf) {   // weigh_justification_and_finalization (:1469-1520)
@@ -1272,17 +1296,12 @@ int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_cod
         if ((bits & 0x07) == 0x07 && old_cj + 2 == cur) memcpy(jf + 81, cp_cj, 40);
         if ((bits & 0x03) == 0x03 && old_cj + 1 == cur) memcpy(jf + 81, cp_cj, 40);
     }
-    EpochParams p{};
     p.steps = steps & kPerValidatorSteps;
     if (!run_inactivity) p.steps &= ~uint32_t(B200_EPOCH_INACTIVITY_UPDATES);
     if (!run_rewards) p.steps &= ~uint32_t(B200_EPOCH_REWARDS_AND_PENALTIES);
     p.cur = cur; p.prev = prev;
     p.finalized_epoch = le64(jf + 81);
-    p.leak = prev - p.finalized_epoch > P.min_epochs_to_inactivity_penalty;   // get_finality_delay wraps
-    p.total_active = total(0);
-    p.base_per_inc = inc * P.base_reward_factor / integer_sqrt(p.total_active);
-    p.active_inc = p.total_active / inc;
-    for (int f = 0; f < 3; f++) p.part_inc[f] = total(1 + f) / inc;
+    p.leak = inactivity_leak(P, prev, p.finalized_epoch);
     // the exit queue (initiate_validator_exit, :3062-3111) in closed form, and the activation churn
     p.churn = std::max(P.min_per_epoch_churn_limit, T.n_active_cur / P.churn_limit_quotient);
     p.activation_epoch = cur + 1 + P.max_seed_lookahead;
@@ -1303,14 +1322,12 @@ int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_cod
     uint64_t slashings_sum = 0;   // `.sum::<Gwei>()` wraps in a release build
     for (uint64_t k = 0; k < P.epochs_per_slashings_vector; k++) slashings_sum += le64(h->shadow + h->so.slashings + 8 * k);
     p.adjusted_slashing = std::min(slashings_sum * P.proportional_slashing_multiplier_bellatrix, p.total_active);
-    p.increment = inc;
     p.max_effective = P.max_effective_balance;
     p.ejection_balance = P.ejection_balance;
     p.hysteresis_down = inc / P.hysteresis_quotient * P.hysteresis_downward_multiplier;
     p.hysteresis_up = inc / P.hysteresis_quotient * P.hysteresis_upward_multiplier;
     p.score_bias = P.inactivity_score_bias;
     p.score_recovery = P.inactivity_score_recovery_rate;
-    p.inactivity_denominator = P.inactivity_score_bias * P.inactivity_penalty_quotient_bellatrix;
     p.withdraw_delay = P.min_validator_withdrawability_delay;
     if (run_sync && T.n_active_next == 0) { e.last_error = "process_epoch: no active validator for the next sync committee"; return B200_ERR_BAD_ARG; }
     const uint64_t n_summaries = (h->so.var[9] - h->so.var[8]) / 64;
@@ -1390,6 +1407,41 @@ int32_t b200_state_process_epoch(b200_state* h, uint32_t steps, int32_t* out_cod
         ms += e.last_kernel_ms;
     }
     e.last_kernel_ms = ms;
+    return B200_SUCCESS;
+}
+
+int32_t b200_state_epoch_deltas(b200_state* h, uint64_t* out, size_t n_out) {
+    Engine& e = engine();
+    Guard g(e);
+    int32_t rc = check_ready(e);
+    if (rc) return rc;
+    if (!resident(h) || (n_out && !out)) return B200_ERR_BAD_ARG;
+    const Preset& P = preset_of(h->preset);
+    const uint64_t n = chain(h, 0).len;
+    if (n_out != n) { e.last_error = "epoch_deltas: n is not the validator count"; return B200_ERR_BAD_ARG; }
+    for (int f = 1; f < 5; f++)
+        if (chain(h, f).len != n) { e.last_error = "epoch_deltas: the five big lists differ in length"; return B200_ERR_BAD_ARG; }
+    if (!n) {
+        e.last_kernel_ms = 0.f;
+        return B200_SUCCESS;
+    }
+    const uint64_t cur = shadow_slot(h) / P.slots_per_epoch, prev = cur ? cur - 1 : 0;
+    // get_unslashed_participating_indices(flag, prev) reads current_epoch_participation when prev == current (epoch 0)
+    const uint8_t* part = chain_dev(h, cur ? 2 : 3);
+    if ((rc = begin_timed(e))) return rc;
+    EpochTotals T;
+    rc = epoch_totals_on_device(e, chain_dev(h, 0), part, chain_dev(h, 3), n, cur, prev, P.ejection_balance, &T);
+    if (rc) return rc;
+    EpochParams p{};
+    if ((rc = reward_scalars(e, T, P, 0xfu, "epoch_deltas", &p))) return rc;   // the active and the three flag sums
+    p.cur = cur; p.prev = prev;
+    p.leak = inactivity_leak(P, prev, le64(h->shadow + h->so.justification_bits + 81));   // finalized_checkpoint.epoch
+    const uint64_t* d = nullptr;
+    rc = epoch_deltas_on_device(e, chain_dev(h, 0), reinterpret_cast<const uint64_t*>(chain_dev(h, 4)), part, n, p, &d);
+    if (rc) return rc;
+    if ((rc = end_timed(e))) return rc;   // the device time of the kernels; the lists then go to the host
+    B200_CUDA_TRY(cudaMemcpyAsync(out, d, size_t(n) * 64, cudaMemcpyDeviceToHost, e.stream));
+    B200_CUDA_TRY(cudaStreamSynchronize(e.stream));
     return B200_SUCCESS;
 }
 

@@ -9,6 +9,8 @@
 //                       pairs, activation eligibility and ejection, the slashing penalty, the effective-balance hysteresis.
 //                       Each CTA also leaves its best activation candidates by (activation_eligibility_epoch, index).
 //   k_activation_select: one CTA merges the candidates and activates at most MAX_PER_EPOCH_ACTIVATION_CHURN_LIMIT.
+//   k_epoch_deltas    : one thread per validator, read-only: the four (reward, penalty) pairs k_epoch_apply would add, as
+//                       eight lists of n u64 (the spec-test Deltas of source, target, head and the inactivity penalty).
 // Everything the kernels compute is integer arithmetic in wrapping u64 (a release build of the reference), decrease_balance
 // saturating at zero; the sums are order-independent, so the result does not depend on the launch shape.
 #include <cuda_runtime.h>
@@ -134,6 +136,18 @@ __global__ void __launch_bounds__(kReduceThreads) k_epoch_reduce(const BlockPart
 
 __device__ __forceinline__ uint64_t sat_sub(uint64_t a, uint64_t b) { return b > a ? 0 : a - b; }
 
+// The terms of get_flag_index_deltas (altair/helpers.rs:265) and get_inactivity_penalty_deltas (bellatrix/helpers.rs:13)
+// for one eligible validator, in wrapping u64 as the reference's release build: k_epoch_apply folds them into the balance
+// one by one, k_epoch_deltas stores them as the eight lists.
+__device__ __forceinline__ uint64_t base_reward(uint64_t eb, const EpochParams& p) { return eb / p.increment * p.base_per_inc; }
+__device__ __forceinline__ uint64_t flag_reward(uint64_t base, int f, const EpochParams& p) {
+    return base * flag_weight(f) * p.part_inc[f] / (p.active_inc * kWeightDenominator);
+}
+__device__ __forceinline__ uint64_t flag_penalty(uint64_t base, int f) { return base * flag_weight(f) / kWeightDenominator; }
+__device__ __forceinline__ uint64_t inactivity_penalty(uint64_t eb, uint64_t score, const EpochParams& p) {
+    return eb * score / p.inactivity_denominator;
+}
+
 // (eligibility epoch, index) keys of activation candidates; lexicographic
 __device__ __forceinline__ bool key_less(uint64_t e1, uint64_t i1, uint64_t e2, uint64_t i2) {
     return e1 < e2 || (e1 == e2 && i1 < i2);
@@ -205,16 +219,16 @@ __global__ void __launch_bounds__(kThreads) k_epoch_apply(uint8_t* __restrict__ 
     }
     // process_rewards_and_penalties (:1187-1230): flags 0, 1, 2, then the inactivity pair, each applied in turn
     if ((p.steps & kRewards) && eligible) {
-        const uint64_t base = eb / p.increment * p.base_per_inc;
+        const uint64_t base = base_reward(eb, p);
 #pragma unroll
         for (int f = 0; f < 3; f++) {
             if (a_prev && !slashed && ((pf >> f) & 1)) {
-                if (!p.leak) bal += base * flag_weight(f) * p.part_inc[f] / (p.active_inc * kWeightDenominator);
+                if (!p.leak) bal += flag_reward(base, f, p);
             } else if (f != 2) {
-                bal = sat_sub(bal, base * flag_weight(f) / kWeightDenominator);
+                bal = sat_sub(bal, flag_penalty(base, f));
             }
         }
-        if (!target) bal = sat_sub(bal, eb * score / p.inactivity_denominator);
+        if (!target) bal = sat_sub(bal, inactivity_penalty(eb, score, p));
     }
     // process_registry_updates (deneb/epoch_processing.rs:11-55): eligibility, then ejection through the exit queue's
     // closed form (the k-th ejection in index order, k = eject_off[cta] + rank in the CTA)
@@ -295,8 +309,40 @@ __global__ void __launch_bounds__(1024) k_activation_select(uint8_t* __restrict_
     }
 }
 
+// The pairs k_epoch_apply adds, without applying them (process_rewards_and_penalties' order and conditions, on the terms
+// above).  List-major: out[2 k n + i] the reward and out[(2 k + 1) n + i] the penalty of pair k for validator i, so that
+// each of the eight stores of a warp is one coalesced 256-byte segment.
+__global__ void __launch_bounds__(kThreads) k_epoch_deltas(const uint8_t* __restrict__ recs, const uint64_t* __restrict__ scores,
+                                                             const uint8_t* __restrict__ part, uint64_t n, EpochParams p,
+                                                             uint64_t* __restrict__ out) {
+    const uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint8_t* r = recs + i * 121;
+    const uint64_t eb = load_le64_unaligned(r + kRecEffectiveBalance);
+    const bool slashed = r[kRecSlashed] != 0;
+    const uint64_t act = load_le64_unaligned(r + kRecActivation), exit = load_le64_unaligned(r + kRecExit);
+    const uint64_t wd = load_le64_unaligned(r + kRecWithdrawable);
+    const uint8_t pf = part[i];
+    const bool a_prev = act <= p.prev && p.prev < exit;
+    uint64_t d[8] = {};   // pair k: d[2 k] reward, d[2 k + 1] penalty; zero for a validator that is not eligible
+    if (a_prev || (slashed && p.prev + 1 < wd)) {   // get_eligible_validator_indices
+        const uint64_t base = base_reward(eb, p);
+#pragma unroll
+        for (int f = 0; f < 3; f++) {
+            if (a_prev && !slashed && ((pf >> f) & 1)) {
+                if (!p.leak) d[2 * f] = flag_reward(base, f, p);
+            } else if (f != 2) {
+                d[2 * f + 1] = flag_penalty(base, f);
+            }
+        }
+        if (!(a_prev && !slashed && (pf & 2))) d[7] = inactivity_penalty(eb, scores[i], p);
+    }
+#pragma unroll
+    for (int k = 0; k < 8; k++) out[k * n + i] = d[k];
+}
+
 struct EpochScratch {
-    DevBuf parts, totals, eject_off, cand_e, cand_i, cand_n, changed, n_changed;
+    DevBuf parts, totals, eject_off, cand_e, cand_i, cand_n, changed, n_changed, deltas;
 };
 EpochScratch g_ep;
 
@@ -357,6 +403,19 @@ int32_t epoch_apply_on_device(Engine& e, uint8_t* recs, uint64_t* balances, uint
     B200_CUDA_TRY(cudaStreamSynchronize(s));
     *n_changed = *static_cast<const uint64_t*>(e.staging.p);
     *changed_dev = static_cast<const uint32_t*>(g_ep.changed.p);
+    return B200_SUCCESS;
+}
+
+int32_t epoch_deltas_on_device(Engine& e, const uint8_t* recs, const uint64_t* scores, const uint8_t* part, uint64_t n,
+                               const EpochParams& p, const uint64_t** out_dev) {
+    *out_dev = nullptr;
+    if (n == 0) return B200_SUCCESS;
+    const uint32_t nb = uint32_t((n + kThreads - 1) / kThreads);
+    B200_CUDA_TRY(g_ep.deltas.reserve(size_t(n) * 64));
+    k_epoch_deltas<<<nb, kThreads, 0, e.stream>>>(recs, scores, part, n, p, static_cast<uint64_t*>(g_ep.deltas.p));
+    e.launches++;
+    B200_CUDA_TRY(cudaGetLastError());
+    *out_dev = static_cast<const uint64_t*>(g_ep.deltas.p);
     return B200_SUCCESS;
 }
 

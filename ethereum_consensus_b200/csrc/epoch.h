@@ -1,4 +1,5 @@
-// Device half of deneb process_epoch on a resident state (epoch.cu), driven by b200_state_process_epoch in capi_ssz.cu.
+// Device half of deneb process_epoch on a resident state (epoch.cu), driven by b200_state_process_epoch in capi_ssz.cu,
+// and of the read-only b200_state_epoch_deltas beside it.
 #pragma once
 #include "engine.h"
 
@@ -14,7 +15,7 @@ struct EpochTotals {
     uint64_t n_at_max_exit;   // validators whose exit_epoch is that epoch
 };
 
-// What the host step decided, passed by value to k_epoch_apply
+// What the host step decided, passed by value to k_epoch_apply (and to k_epoch_deltas, which reads the reward fields)
 struct EpochParams {
     uint32_t steps;               // the B200_EPOCH_* bits whose per-validator work runs
     uint32_t leak;                // is_in_inactivity_leak, after justification
@@ -40,5 +41,11 @@ int32_t epoch_totals_on_device(Engine& e, const uint8_t* recs, const uint8_t* pr
 // *n_changed (host) gets the number of Validator records written; their indices, possibly repeated, are at *changed_dev.
 int32_t epoch_apply_on_device(Engine& e, uint8_t* recs, uint64_t* balances, uint64_t* scores, const uint8_t* prev_part,
                               uint64_t n, const EpochParams& p, const uint32_t** changed_dev, uint64_t* n_changed);
+// The (reward, penalty) pairs of k_epoch_apply without applying them (after epoch_totals_on_device with the same
+// participation list): *out_dev (device, valid until the next call) holds eight lists of n u64, source rewards, source
+// penalties, target ..., head ..., inactivity rewards (zero), inactivity penalties.  Reads p's prev, leak, base_per_inc,
+// part_inc, active_inc, increment and inactivity_denominator.
+int32_t epoch_deltas_on_device(Engine& e, const uint8_t* recs, const uint64_t* scores, const uint8_t* part, uint64_t n,
+                               const EpochParams& p, const uint64_t** out_dev);
 
 }  // namespace b200

@@ -1,5 +1,6 @@
 """Epoch processing on a device-resident deneb `BeaconState` (`ssz.DeviceBeaconState`): `process_epoch`
-(ethereum-consensus/src/deneb/spec/mod.rs:965-1003) in one call, its sub-steps selectable by name.
+(ethereum-consensus/src/deneb/spec/mod.rs:965-1003) in one call, its sub-steps selectable by name, and the reward and
+penalty deltas of `process_rewards_and_penalties` read without applying them (`deltas`).
 
 The per-validator sub-steps run as CUDA kernels over the records, balances, inactivity scores and participation lists in
 HBM (csrc/epoch.cu); the small fields go through the state's update and reshape paths.  Rules the reference leaves to its
@@ -9,6 +10,8 @@ from __future__ import annotations
 
 import ctypes as C
 
+import numpy as np
+
 from . import _lib
 
 # sub-step bits, named as the spec-test handlers of epoch_processing (include/b200_consensus.h: B200_EPOCH_*)
@@ -17,6 +20,9 @@ STEPS = ("justification_and_finalization", "inactivity_updates", "rewards_and_pe
          "historical_summaries_update", "participation_flag_updates", "sync_committee_updates")
 STEP = {name: 1 << k for k, name in enumerate(STEPS)}
 ALL = (1 << len(STEPS)) - 1
+# the (reward, penalty) pairs of `deltas`, in the order process_rewards_and_penalties applies them (the spec-test
+# `rewards` handler's source, target, head and inactivity-penalty Deltas)
+DELTAS = ("source", "target", "head", "inactivity_penalty")
 
 
 def mask(steps) -> int:
@@ -40,3 +46,13 @@ def process_epoch(dev_state, steps=ALL) -> None:
     if code.value:
         from .crypto import BLSTError
         raise BLSTError(code.value)
+
+
+def deltas(dev_state) -> np.ndarray:
+    """get_flag_index_deltas for flags 0, 1, 2 and get_inactivity_penalty_deltas on the resident state as it is, as a
+    uint64 array of shape (4, 2, n): [k, 0] the rewards and [k, 1] the penalties of pair DELTAS[k].  Reads the state and
+    never writes it; a refusal raises _lib.EngineError carrying the library's code."""
+    n = dev_state.n_validators
+    out = np.zeros((len(DELTAS), 2, n), dtype=np.uint64)
+    _lib.check(_lib.lib().b200_state_epoch_deltas(dev_state._h, out.ctypes.data if n else None, n), "state_epoch_deltas")
+    return out

@@ -310,6 +310,25 @@ B200_API int32_t b200_state_attesting_indices(b200_state* handle, size_t n_att, 
  *    b200_state_update_bytes takes, after any updates, reshapes or epochs: bytes inside the five big lists come from
  *    HBM, the rest from the host copy.  A range past the end -> B200_ERR_BAD_ARG. */
 B200_API int32_t b200_state_process_epoch(b200_state* handle, uint32_t steps, int32_t* out_code);
+/*  - b200_state_epoch_deltas: the reward and penalty deltas of process_rewards_and_penalties on the state as it is, without
+ *    applying them: get_flag_index_deltas (altair/helpers.rs:265) for flags 0, 1, 2 and get_inactivity_penalty_deltas
+ *    (bellatrix/helpers.rs:13), the four spec-test Deltas pairs of the `rewards` handler.  `out` is list-major, eight
+ *    lists of n u64: source rewards, source penalties, target rewards, target penalties, head rewards, head penalties,
+ *    inactivity rewards (always zero), inactivity penalties; list j is out[j n .. j n + n).  Each is the Vec<Gwei> the
+ *    reference returns.  The call reads the state and never writes it: the serialization, both roots, the incremental
+ *    root's pending work and the committee cache stay as they were.
+ *    Semantics of the reference functions as they stand, with no other sub-step run first: previous = max(current - 1,
+ *    0); the leak test reads the state's finalized_checkpoint (get_finality_delay wraps); the inactivity penalty reads
+ *    the state's scores; only get_eligible_validator_indices receive deltas; there is no genesis shortcut.  At the
+ *    current epoch 0, previous == current and get_unslashed_participating_indices reads current_epoch_participation.
+ *    Arithmetic wraps in u64 as in b200_state_process_epoch (base_reward * weight * increments, effective_balance *
+ *    inactivity_score).  Refusals before any write: a NULL, not uploaded or sharded handle, out == NULL with n > 0,
+ *    n != the validator count, or five big lists of different lengths -> B200_ERR_BAD_ARG; get_total_balance's
+ *    checked_add overflowing u64 for the total active balance or any flag's unslashed participating balance ->
+ *    B200_ERR_LIMIT (the reference's Err, which its rewards handler unwraps).  n == 0 succeeds and launches nothing.
+ *    Three launches (the totals pass, its fold, k_epoch_deltas).  b200_last_kernel_ms: the device time of the call's
+ *    kernels, without the copy of the lists to the host. */
+B200_API int32_t b200_state_epoch_deltas(b200_state* handle, uint64_t* out /* 8 x n */, size_t n);
 B200_API int32_t b200_state_serialized_len(b200_state* handle, uint64_t* out_len);
 B200_API int32_t b200_state_read_bytes(b200_state* handle, uint64_t ssz_offset, uint8_t* out, size_t n);
 
